@@ -1,29 +1,35 @@
 // wgmma implicit-GEMM convolution / FC for sm_90a with FP32-class accuracy via 3xTF32 / 3xFP16 error compensation.
 //
-//   D[128 x 64] (fp32)  =  sum over K chunks of   A_hi*B_hi  +  (A_lo*B_hi + A_hi*B_lo)
+//   D[128 x BN] (fp32)  =  sum over K chunks of   A_hi*B_hi  +  (A_lo*B_hi + A_hi*B_lo)
 //
-// A (activations) never exists in HBM in im2col form: eight producer warps gather the 128-row tile of one K chunk
-// (zero padding, stride, per-channel BN/GN affine + ReLU prologue fused; up to three chunks of loads in flight per
-// thread), split every value into its head `hi` (rounded to nearest: TF32 = low 13 mantissa bits clear, or fp16) and
-// the remainder `lo`, and store both straight into the 128-byte-swizzled K-major layout the wgmma shared-memory
-// descriptor expects -- or, for pre-split fp16 activations, cp.async the pair there unchanged.  B (weights, pre-split
-// offline into hi/lo, K-major) arrives by TMA.  Two consumer warpgroups issue wgmma, each for 64 of the 128 rows.
+// A (activations) never exists in HBM in im2col form.  For pre-split fp16 activations (every ResNet trunk layer, the SMPL
+// blend GEMM) one producer warpgroup cp.asyncs the 128-row hi/lo pair of one K chunk straight into the 128-byte-swizzled
+// K-major layout the wgmma shared-memory descriptor expects.  Otherwise eight producer warps gather the tile (zero padding,
+// stride, per-channel BN/GN affine + ReLU prologue fused; up to three chunks of loads in flight per thread), split every
+// value into its head `hi` (rounded to nearest: TF32 = low 13 mantissa bits clear, or fp16) and the remainder `lo`, and
+// store both there.  B (weights, pre-split offline into hi/lo, K-major) arrives by TMA in 64-row boxes.  Two consumer
+// warpgroups issue wgmma, each for 64 of the 128 rows.
 //
 // Accumulation precision: the tensor core does not round the fp32 accumulator to nearest on every MMA, so a long K
 // summed in one accumulator drifts (relative error grows linearly with K).  Accumulation is therefore two-level: the
 // dominant A_hi*B_hi term is summed by the tensor core for only PCH K-chunks, then added -- round-to-nearest, on the
 // CUDA cores -- into per-thread fp32 running sums.  The two cross terms (2^-11 smaller) accumulate in their own
-// register fragment for the whole tile.  Per consumer thread that is 3 x 32 fp32 registers, which is why the N tile is
-// 64 wide: a 128-wide tile would need 192 accumulator registers per thread.
+// register fragment for the whole tile.  Per consumer thread that is 3 x BN/2 fp32 registers.
+//
+// N tile: 128 for pre-split layers with Cout > 64 that give the SMs enough tiles (wide_n_tile), 64 otherwise.  The 128-wide
+// tile needs 3 x 64 accumulator registers per consumer thread and halves the A gathers and the shared-memory reads per MMA
+// of the 64-wide one.
 //
 // Persistent: grid = min(#tiles, #SMs); each CTA walks tiles blockIdx.x, +gridDim.x, ...  Barrier phases run
 // continuously across tiles, and the producers keep prefetching the next tile's chunks while the consumers run the
 // fused epilogue (scale/shift, residual, ReLU, fp32 output or its strided subsample, the next layer's fp16 pair)
 // straight from the accumulator fragments.
 //
-// Warp roles (512 threads; 16 warps = 4 per scheduler leave 128 registers a thread):
-//   warps 0-7   two consumer warpgroups: wgmma issue, drains, epilogue (warpgroup g owns tile rows 64 g .. 64 g + 63)
-//   warps 8-15  A producers; producer thread 0 also issues the chunk's B tile (TMA)
+// Warp roles:
+//   warps 0-7    two consumer warpgroups: wgmma issue, drains, epilogue (warpgroup g owns tile rows 64 g .. 64 g + 63)
+//   warps 8-11   BN = 128 (384 threads): the cp.async A producers, 8 rows each; registers 256 x 232 + 128 x 40
+//   warps 8-15   BN = 64 (512 threads): the A producers, 4 rows each; registers 256 x 152 + 256 x 104
+// Producer thread 0 also issues the chunk's B tile (TMA).
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cstdlib>
@@ -34,16 +40,23 @@ namespace hd {
 namespace {
 
 constexpr int BM = 128;
-constexpr int BN = 64;
 constexpr int A_TILE_BYTES = BM * 128;      // 16 KiB: 128 rows x one 128-byte swizzle row (32 tf32 or 64 fp16 of K)
-constexpr int W_PROD = 8, NUM_WARPS = 16;   // first producer warp, warps per CTA
+constexpr int BOX_BYTES = 64 * 128;         // one 64-row weight box (hd_make_weight_tmap)
+constexpr int W_PROD = 8;                   // first producer warp
 
 using namespace ptx;
 
-template <bool HALF>
+template <bool HALF, bool ASPLIT, int BN>
 struct Cfg {
-  static constexpr int STAGES = 4;
-  static constexpr int NUM_THREADS = NUM_WARPS * 32;
+  static_assert(BN == 64 || (BN == 128 && HALF && ASPLIT), "128-wide N tiles: pre-split fp16 path only");
+  static constexpr int PROD_THREADS = BN == 128 ? 128 : 256;
+  static constexpr int NUM_THREADS = 256 + PROD_THREADS;
+  static constexpr int ROW_STEP = PROD_THREADS / 8;             // a producer thread's rows: rb + ROW_STEP * i
+  static constexpr int ROWS = BM / ROW_STEP;
+  static constexpr int PROD_REGS = BN == 128 ? 40 : 104, CONS_REGS = BN == 128 ? 232 : 152;
+  static_assert(256 * CONS_REGS + PROD_THREADS * PROD_REGS <= 65536, "setmaxnreg split beyond the register file");
+  static constexpr int NACC = BN / 2;                           // fp32 registers of one m64nBN fragment per thread
+  static constexpr int STAGES = BN == 128 ? 3 : 4;
   static constexpr int BKE = HALF ? 64 : 32;                    // K elements per chunk (one 128-byte row)
   static constexpr int B_TILE_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
@@ -54,15 +67,16 @@ struct Cfg {
   static constexpr int V = HALF ? 2 : 1;                        // float4 loads per row per chunk per thread
 };
 
-struct RowState {       // 4 output rows of one producer thread: image index and top-left input coordinate
-  int n[4], iy[4], ix[4];
+template <int R>
+struct RowState {       // R output rows of one producer thread: image index and top-left input coordinate
+  int n[R], iy[R], ix[R];
 };
 
-template <bool SPLIT, int PCH, bool HALF, bool GATHER, bool ASPLIT>
-__global__ void __launch_bounds__((Cfg<HALF>::NUM_THREADS), 1)
+template <bool SPLIT, int PCH, bool HALF, bool GATHER, bool ASPLIT, int BN>
+__global__ void __launch_bounds__((Cfg<HALF, ASPLIT, BN>::NUM_THREADS), 1)
 conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap_hi, const __grid_constant__ CUtensorMap tmap_lo) {
-  using C = Cfg<HALF>;
-  constexpr int BKE = C::BKE, PF = C::PF, V = C::V, STAGES = C::STAGES;
+  using C = Cfg<HALF, ASPLIT, BN>;
+  constexpr int BKE = C::BKE, PF = C::PF, V = C::V, STAGES = C::STAGES, R = C::ROWS, RS = C::ROW_STEP, NA = C::NACC;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t *smem = smem_raw + (smem_base - smem_u32(smem_raw));
@@ -78,7 +92,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), ASPLIT ? 257 : 9);   // 8 producer warps (ASPLIT: 256 threads, hardware arrive per thread when its cp.asyncs land)
+      mbar_init(full_bar(s), ASPLIT ? C::PROD_THREADS + 1 : 9);   // 8 producer warps (ASPLIT: every producer thread, hardware arrive when its cp.asyncs land)
                                                   // + 1 arrive.expect_tx from the thread that issues the B load
       mbar_init(empty_bar(s), 8);    // one arrive per consumer warp once its wgmmas have read the stage
     }
@@ -88,32 +102,39 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
   const int xmode = p.dbg ? (int)p.dbg[15] : 0;      // timing experiments (hd_conv_gemm_profile only; results invalid)
 
   if (warp >= W_PROD) {
-    // =============================== A producers (256 threads) ===============================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 104;");    // register pool 512 x 128: producers 256 x 104 + consumers 256 x 152
-    const int t = threadIdx.x - W_PROD * 32;  // 0..255
+    // =============================== A producers (PROD_THREADS) ===============================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(C::PROD_REGS));
+    const int t = threadIdx.x - W_PROD * 32;  // 0 .. PROD_THREADS - 1
     const int j = t & 7;                  // 16-byte chunk within the 128-byte K row
-    const int rb = t >> 3;                // rows rb + 32*i, i < 4
+    const int rb = t >> 3;                // rows rb + RS*i, i < R (all with the same row & 7, so one swizzle offset)
     const uint32_t sw_off = (uint32_t)((j ^ (rb & 7)) << 4);
     const bool prof = p.dbg != nullptr && blockIdx.x == 0 && t == 0;
-    long long t_wait = 0, t_start = prof ? clock64() : 0;
+    long long t_wait = 0, t_start = prof && BN == 64 ? clock64() : 0;
+    if (BN == 128 && prof) p.dbg[0] = clock64();   // start stamp in memory, replaced by the loop's length: keeps 40 registers spill-free
     const int total = my_tiles * num_k;
     auto load_b = [&](int s, int ti, int kc) {      // producer thread 0: the chunk's B tile (weights, hi and lo) by TMA
       if (t != 0) return;
       const int n0 = (((int)blockIdx.x + ti * (int)gridDim.x) % tiles_n) * BN;
       const uint32_t b_hi = smem_base + s * C::STAGE_BYTES + 2 * A_TILE_BYTES;
       if (xmode & 2) { mbar_arrive(full_bar(s)); return; }
-      mbar_arrive_expect_tx(full_bar(s), SPLIT ? 2 * C::B_TILE_BYTES : C::B_TILE_BYTES);
-      tma_load_2d(b_hi, &tmap_hi, full_bar(s), kc * BKE, n0);
-      if (SPLIT) tma_load_2d(b_hi + C::B_TILE_BYTES, &tmap_lo, full_bar(s), kc * BKE, n0);
+      // BN = 128: two 64-row boxes.  Weight rows are padded to 64, so the second box is either wholly inside the weights or
+      // wholly past Cout; then it is not loaded, and the stale columns it would have filled only reach outputs c >= Cout,
+      // which the epilogue never stores.
+      const int boxes = (BN == 128 && n0 + 64 < p.Cout) ? 2 : 1;
+      mbar_arrive_expect_tx(full_bar(s), (SPLIT ? 2 : 1) * boxes * BOX_BYTES);
+      for (int b = 0; b < boxes; ++b) {
+        tma_load_2d(b_hi + b * BOX_BYTES, &tmap_hi, full_bar(s), kc * BKE, n0 + 64 * b);
+        if (SPLIT) tma_load_2d(b_hi + C::B_TILE_BYTES + b * BOX_BYTES, &tmap_lo, full_bar(s), kc * BKE, n0 + 64 * b);
+      }
     };
 
-    auto enter_tile = [&](int ti, RowState &rs) {
+    auto enter_tile = [&](int ti, RowState<R> &rs) {
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
       const int m0 = (tile / tiles_n) * BM;
       const int hw = p.Ho * p.Wo;
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int m = m0 + rb + 32 * i;
+      for (int i = 0; i < R; ++i) {
+        const int m = m0 + rb + RS * i;
         if (m < p.M) {
           const int n = m / hw;
           const int r = m - n * hw;
@@ -124,7 +145,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         }
       }
     };
-    if (ASPLIT) {
+    if constexpr (ASPLIT) {
       // ---- pre-split fp16 activations: cp.async straight into the swizzled tile, STAGES chunks in flight, no registers ----
       const __half *ihi = reinterpret_cast<const __half *>(p.in_hi);
       const __half *ilo = reinterpret_cast<const __half *>(p.in_lo);
@@ -134,9 +155,9 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         // element offset and one tap-validity bit mask per row.  Per chunk: (tap, channel) advance incrementally -- a 64-wide chunk
         // lies inside one tap because Cin % 64 == 0 -- and a row costs a shift, an add and two cp.asyncs.  Taken when the input's
         // element offsets fit 32 bits and the kernel window fits the 32-bit tap mask; anything else runs the general loop.
-        const uint32_t off0 = (uint32_t)rb * 128u + sw_off;       // row rb + 32 i of the tile: + i * 4096
-        int base[4];
-        uint32_t mask[4];
+        const uint32_t off0 = (uint32_t)rb * 128u + sw_off;       // row rb + RS i of the tile: + i * RS * 128
+        int base[R];
+        uint32_t mask[R];
         int kc = 0, ti = 0, tap = 0, ci0 = 0, kx = 0, ky = 0, tap_off = 0;
         for (int q = 0; q < total; ++q) {
           if (kc == 0) {
@@ -144,8 +165,8 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
             const int m0 = (tile / tiles_n) * BM + rb;
             const int hw = p.Ho * p.Wo;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int m = m0 + 32 * i;
+            for (int i = 0; i < R; ++i) {
+              const int m = m0 + RS * i;
               uint32_t mk = 0;
               int b = 0;
               if (m < p.M) {
@@ -173,11 +194,11 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           const uint32_t a_hi = smem_base + s * C::STAGE_BYTES + off0;
           const int eo = tap_off + ci0;
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
+          for (int i = 0; i < R; ++i) {
             const bool ok = (mask[i] >> tap) & 1u;
             const int e = ok ? base[i] + eo : 0;
-            cp_async16(a_hi + i * 4096, ihi + e, ok ? 16u : 0u);
-            cp_async16(a_hi + A_TILE_BYTES + i * 4096, ilo + e, ok ? 16u : 0u);
+            cp_async16(a_hi + i * RS * 128, ihi + e, ok ? 16u : 0u);
+            cp_async16(a_hi + A_TILE_BYTES + i * RS * 128, ilo + e, ok ? 16u : 0u);
           }
           asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(full_bar(s)) : "memory");
           ci0 += BKE;
@@ -195,7 +216,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         const uint32_t off0 = (uint32_t)rb * 128u + sw_off;
         const int jt = j >> 2;
         const int row_step = 2 * p.W * (int)p.in_ld;                // two kernel rows per chunk
-        int base[4];
+        int base[R];
         int kc = 0, ti = 0;
         for (int q = 0; q < total; ++q) {
           if (kc == 0) {
@@ -203,8 +224,8 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
             const int m0 = (tile / tiles_n) * BM + rb;
             const int hw = p.Ho * p.Wo;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int m = m0 + 32 * i;
+            for (int i = 0; i < R; ++i) {
+              const int m = m0 + RS * i;
               int b = -1;
               if (m < p.M) {
                 const int n = m / hw;
@@ -225,18 +246,18 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           const bool tap_ok = 2 * kc + jt < 7;
           const int eo = kc * row_step;
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
+          for (int i = 0; i < R; ++i) {
             const bool ok = tap_ok && base[i] >= 0;
             const int e = ok ? base[i] + eo : 0;
             // neighbouring output pixels read overlapping 64-byte windows (each 16-byte piece 4x): keep them in L1
-            cp_async16_ca(a_hi + i * 4096, ihi + e, ok ? 16u : 0u);
-            cp_async16_ca(a_hi + A_TILE_BYTES + i * 4096, ilo + e, ok ? 16u : 0u);
+            cp_async16_ca(a_hi + i * RS * 128, ihi + e, ok ? 16u : 0u);
+            cp_async16_ca(a_hi + A_TILE_BYTES + i * RS * 128, ilo + e, ok ? 16u : 0u);
           }
           asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(full_bar(s)) : "memory");
           if (++kc == num_k) { kc = 0; ++ti; }
         }
       } else {
-      RowState rs;
+      RowState<R> rs;
       int kc = 0, ti = 0;
       for (int q = 0; q < total; ++q) {
         if (kc == 0) enter_tile(ti, rs);
@@ -256,11 +277,11 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         const bool tap_ok = !p.planes || tap < 7;
         const uint32_t a_hi = smem_base + s * C::STAGE_BYTES, a_lo = a_hi + A_TILE_BYTES;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
+        for (int i = 0; i < R; ++i) {
           const int iy = rs.iy[i] + ky, ix = rs.ix[i] + kx;
           const bool ok = tap_ok && rs.n[i] >= 0 && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
           const size_t e = ok ? ((size_t)((size_t)rs.n[i] * p.H + iy) * p.W + ix) * p.in_ld + ci : 0;
-          const uint32_t off = (uint32_t)(rb + 32 * i) * 128u + sw_off;
+          const uint32_t off = (uint32_t)(rb + RS * i) * 128u + sw_off;
           if (p.planes) {        // conv1: neighbouring output pixels read overlapping 64-byte windows (each 16-byte piece 4x): keep them in L1
             cp_async16_ca(a_hi + off, ihi + e, ok ? 16u : 0u);
             cp_async16_ca(a_lo + off, ilo + e, ok ? 16u : 0u);
@@ -278,9 +299,9 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
       }
       cp_async_commit();
       cp_async_wait<0>();
-      if (prof) { p.dbg[0] = clock64() - t_start; p.dbg[1] = t_wait; }
+      if (prof) { p.dbg[0] = clock64() - (BN == 128 ? p.dbg[0] : t_start); p.dbg[1] = t_wait; }
     } else {
-    RowState pf_rs, st_rs;                 // prefetch-side and store-side row state (may be one tile apart)
+    RowState<R> pf_rs, st_rs;              // prefetch-side and store-side row state (may be one tile apart)
     float4 ring[PF][4 * V];
     uint32_t vmask[PF];
     int pf_kc = 0, pf_ti = 0;              // next chunk to prefetch
@@ -412,22 +433,22 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     }   // !ASPLIT
   } else if (warp < W_PROD) {
     // =============================== consumers: wgmma, drains, epilogue ===============================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 152;");
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(C::CONS_REGS));
     const int wg = warp >> 2;                             // rows 64 wg .. 64 wg + 63 of the tile
     const bool prof = p.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0;
     long long t_wait = 0, t_epi = 0, t_start = prof ? clock64() : 0;
     const int hw = p.Ho * p.Wo;
     const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's fragment rows: frow, frow + 8
     const int fcol = 2 * (lane & 3);                            // and columns 8 j + fcol, + 1
-    float acc[32], accx[32], sums[32];
+    float acc[NA], accx[NA], sums[NA];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) { acc[i] = 0.f; accx[i] = 0.f; }
+    for (int i = 0; i < NA; ++i) { acc[i] = 0.f; accx[i] = 0.f; }
     int q = 0;
     for (int ti = 0; ti < my_tiles; ++ti) {
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
       const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) sums[i] = 0.f;
+      for (int i = 0; i < NA; ++i) sums[i] = 0.f;
       for (int kc = 0; kc < num_k; ++kc, ++q) {
         const int s = q % STAGES;
         const uint32_t ph = (uint32_t)(q / STAGES) & 1u;
@@ -448,7 +469,11 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
 #pragma unroll
         for (int k = 0; k < 4; ++k) {                // K = 8 tf32 / 16 fp16 = 32 bytes per wgmma: advance inside the swizzle row
           const uint64_t adv = (uint64_t)((k * 32) >> 4);
-          if (HALF) {
+          if constexpr (BN == 128) {
+            wgmma_m64n128k16_f16(accx, da_lo + adv, db_hi + adv, (kc | k) != 0);
+            wgmma_m64n128k16_f16(accx, da_hi + adv, db_lo + adv, 1u);
+            wgmma_m64n128k16_f16(acc, da_hi + adv, db_hi + adv, !(group_start && k == 0));
+          } else if constexpr (HALF) {
             wgmma_m64n64k16_f16(accx, da_lo + adv, db_hi + adv, (kc | k) != 0);
             wgmma_m64n64k16_f16(accx, da_hi + adv, db_lo + adv, 1u);
             wgmma_m64n64k16_f16(acc, da_hi + adv, db_hi + adv, !(group_start && k == 0));
@@ -468,12 +493,12 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         if (lane == 0) mbar_arrive(empty_bar(s));       // this warp's share of the stage has been read
         if ((kc % PCH) == PCH - 1 || kc == num_k - 1) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) sums[i] += acc[i];      // round-to-nearest fp32 adds
+          for (int i = 0; i < NA; ++i) sums[i] += acc[i];      // round-to-nearest fp32 adds
         }
       }
       if (SPLIT) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) sums[i] += accx[i] * (HALF ? (1.0f / 2048.0f) : 1.0f);
+        for (int i = 0; i < NA; ++i) sums[i] += accx[i] * (HALF ? (1.0f / 2048.0f) : 1.0f);
       }
       long long te0 = prof ? clock64() : 0;
       // Epilogue from the fragments: per row, per pair of adjacent columns (8-byte fp32 / 4-byte fp16-pair stores; the four
@@ -507,7 +532,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         __half *hrow = p.out_hi ? reinterpret_cast<__half *>(p.out_hi) + (size_t)m * p.out2_ld : nullptr;
         __half *lrow = p.out_hi ? reinterpret_cast<__half *>(p.out_lo) + (size_t)m * p.out2_ld : nullptr;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
+        for (int j = 0; j < BN / 8; ++j) {
           const int c = n0 + 8 * j + fcol;
           if (c >= p.Cout) continue;
           const bool two = c + 1 < p.Cout;
@@ -568,9 +593,9 @@ EncodeTiledFn get_encode_fn() {
 
 constexpr int kMaxDevices = 64;
 
-template <bool SPLIT, int PCH, bool HALF, bool GATHER = false, bool ASPLIT = false>
+template <bool SPLIT, int PCH, bool HALF, bool GATHER = false, bool ASPLIT = false, int BN = 64>
 int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
-  using C = Cfg<HALF>;
+  using C = Cfg<HALF, ASPLIT, BN>;
   // function attributes and the SM count are per device: a process may drive several GPUs through this library
   static bool configured[kMaxDevices] = {};
   static int num_sms[kMaxDevices] = {};
@@ -578,14 +603,14 @@ int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= kMaxDevices) { set_last_error_text("conv_gemm_tc: device ordinal out of range"); return HD_ERR_UNSUPPORTED; }
   if (!configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT>,
+    cudaError_t e = cudaFuncSetAttribute(conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (e != cudaSuccess) { set_last_error("conv_gemm_tc attr", e); return HD_ERR_CUDA; }
     cudaDeviceGetAttribute(&num_sms[dev], cudaDevAttrMultiProcessorCount, dev);
     if (num_sms[dev] <= 0) { set_last_error_text("conv_gemm_tc: no multiprocessor count"); return HD_ERR_CUDA; }
     configured[dev] = true;
   }
-  // weight maps with the 64-row box of the N tile (hd_make_weight_tmap accepts no other)
+  // weight maps with the 64-row box (hd_make_weight_tmap accepts no other; a 128-wide N tile loads two boxes)
   alignas(64) CUtensorMap thi, tlo;
   const void *mhi = d->tmap_hi_n64 ? d->tmap_hi_n64 : d->tmap_hi;
   const void *mlo = d->tmap_hi_n64 ? d->tmap_lo_n64 : d->tmap_lo;
@@ -593,8 +618,21 @@ int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
   memcpy(&tlo, mlo ? mlo : mhi, sizeof(CUtensorMap));     // mlo is null only for 1xTF32, which never loads it (launch_conv_tc)
   const int num_tiles = ceil_div(p.M, BM) * ceil_div(p.Cout, BN);
   dim3 grid(num_tiles < num_sms[dev] ? num_tiles : num_sms[dev]);     // persistent: one CTA per SM walks the tile list
-  conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT><<<grid, C::NUM_THREADS, C::SMEM_BYTES, st>>>(p, thi, tlo);
+  conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN><<<grid, C::NUM_THREADS, C::SMEM_BYTES, st>>>(p, thi, tlo);
   return check_launch("conv_gemm_tc_kernel");
+}
+
+// A 128-wide tile does the work of two 64-wide ones in less time, but there are half as many to spread over the SMs.  Take it
+// unless that costs more than an eighth in whole waves of tiles (the small late layers of a small batch).
+bool wide_n_tile(const ConvParams &p) {
+  if (p.Cout <= 64) return false;
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (sms <= 0) return true;
+  const long long m_tiles = ceil_div(p.M, BM);
+  const long long w128 = (m_tiles * ceil_div(p.Cout, 128) + sms - 1) / sms, w64 = (m_tiles * ceil_div(p.Cout, 64) + sms - 1) / sms;
+  return 16 * w128 <= 9 * w64;      // 2 w128 <= 1.125 w64
 }
 
 }  // namespace
@@ -637,7 +675,7 @@ int launch_conv_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) 
       set_last_error_text("hd_conv_gemm(tc split-A): needs Cin % 64 == 0, in_ld % 8 == 0, aligned in_hi/in_lo, no prologue");
       return HD_ERR_INVALID;
     }
-    return launch_tc<true, 2, true, false, true>(p, d, st);
+    return wide_n_tile(p) ? launch_tc<true, 2, true, false, true, 128>(p, d, st) : launch_tc<true, 2, true, false, true>(p, d, st);
   }
   if (half && p.Cin % bke != 0) {      // ragged Cin (resnet conv1: 7x7x3): element-wise gather producer, K zero-padded
     const int segp = (p.KW * p.Cin + 7) & ~7;
@@ -659,7 +697,8 @@ int launch_conv_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) 
 }  // namespace hd
 
 // K-major weight matrix [rows, k_pad] (fp32 for the tf32 path, fp16 for the fp16 path) -> CUtensorMap with a
-// {128 bytes x box_rows} box and 128-byte swizzle.  box_rows must equal the kernel's N tile, 64.
+// {128 bytes x box_rows} box and 128-byte swizzle.  box_rows must be 64: the kernel loads its 64- or 128-wide N tile as
+// one or two such boxes.
 extern "C" int hd_make_weight_tmap(const void *w_nk, int rows, int k_pad, int box_rows, int elem_bytes, void *tmap_out) {
   HD_REQUIRE(w_nk && tmap_out && rows > 0 && k_pad > 0 && (elem_bytes == 4 || elem_bytes == 2) && k_pad % (128 / elem_bytes) == 0 &&
                  box_rows == 64 && rows % box_rows == 0 && hd::aligned16(w_nk),

@@ -87,7 +87,7 @@ class PackedConv(object):
             seg = self.KW * self.Cin
             segp = (seg + 7) // 8 * 8                        # gather layout: each kernel row's KW*Cin floats padded to x8
             self.K_pad = (self.KH * segp + 63) // 64 * 64 if gather else self.K
-            box = 64                                         # must equal the kernel's N tile (conv_tc.cu)
+            box = 64                                         # the TMA box the kernel loads its 64/128-wide N tile in (conv_tc.cu)
             rows = (self.Cout + box - 1) // box * box
             w_nk = np.zeros((rows, self.K_pad), np.float32)
             if gather:                                       # K index = ky*segp + (kx*Cin + ci)   (conv_tc.cu GATHER producer)

@@ -86,7 +86,8 @@ typedef struct {
    * accepted exactly when they are given and the flag is unset, as it was for the earlier TMA epilogue. */
   const void *tmap_res, *tmap_out, *tmap_out_hi, *tmap_out_lo;
   int flags;
-  /* optional: weight maps to use instead of tmap_hi / tmap_lo (64-row box, the kernel's N tile); give both or neither
+  /* optional: weight maps to use instead of tmap_hi / tmap_lo (64-row box; the kernel loads a 64- or 128-wide N tile as one or
+   * two boxes); give both or neither
    * (tmap_lo_n64 may be NULL for impl 2), else HD_ERR_INVALID. */
   const void *tmap_hi_n64, *tmap_lo_n64;
   /* out_subsample = s > 1 (only with the activation tensor maps above and HD_CONV_NO_TMA_EPILOGUE unset; HD_ERR_UNSUPPORTED
@@ -113,7 +114,8 @@ int hd_conv_gemm_profile(const hd_conv_desc *d, void *stream, long long *dbg);
 
 /* Encode the TMA descriptor (CUtensorMap, 128 B, written to host memory `tmap_out`) for a K-major weight matrix
  * [rows, k_pad] of elem_bytes-wide elements (4 = fp32/tf32 path, 2 = fp16 path) with a {128 bytes x box_rows} box and
- * 128-byte swizzle.  box_rows must be 64 (the N tile of the tensor-core kernel) and divide rows. */
+ * 128-byte swizzle.  box_rows must be 64 (the tensor-core kernel loads its 64- or 128-wide N tile as one or two boxes) and
+ * divide rows. */
 int hd_make_weight_tmap(const void *w_nk, int rows, int k_pad, int box_rows, int elem_bytes, void *tmap_out);
 /* Same for a row-major activation matrix [rows, cols] with leading dimension ld_elems (elem_bytes 4 = fp32, 2 = fp16): box
  * {32 columns x 128 rows}, 128-byte (fp32) / 64-byte (fp16) swizzle (see tmap_res above). */
