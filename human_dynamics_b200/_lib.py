@@ -56,6 +56,15 @@ class SmplConsts(C.Structure):
     ]
 
 
+class RenderParams(C.Structure):
+    """Mirror of hd_render_params."""
+    _fields_ = [
+        ('color', C.c_float * 3), ('light_dir', C.c_float * 3), ('ambient', C.c_float), ('directional', C.c_float),
+        ('bg', C.c_float * 3), ('near_z', C.c_float), ('far_z', C.c_float), ('eye_z', C.c_float),
+        ('rot', C.c_float * 9), ('use_rot', C.c_int),
+    ]
+
+
 # name -> (restype, argtypes); must list every symbol include/hd_b200.h declares.
 _vp, _i, _ll, _f, _sz = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_size_t
 SIGNATURES = {
@@ -102,6 +111,8 @@ SIGNATURES = {
     'hd_rot2aa': (_i, [_vp, _vp, _i, _vp]),
     'hd_global_rigid': (_i, [_vp, _vp, C.POINTER(C.c_int), _vp, _vp, _i, _i, _vp]),
     'hd_orth_proj': (_i, [_vp, _vp, _vp, _i, _i, _vp]),
+    'hd_render_workspace_bytes': (_sz, [_i, _i, _i]),
+    'hd_render_mesh': (_i, [_vp, _ll, _i, _i, _vp, _i, _vp, _i, C.POINTER(RenderParams), _vp, _i, _vp, _vp, _vp, _sz, _vp]),
 }
 
 

@@ -81,6 +81,28 @@ def make_synthetic_smpl(seed: int = 2, num_kps: int = 25, dense_weights: bool = 
     }
 
 
+def make_smooth_mesh(seed: int = 11):
+    """A closed genus-0 mesh with SMPL's vertex and face counts for rendering tests and benchmarks: 84 rings of 82 vertices + 2
+    poles (V = 6890, F = 2V - 4 = 13776), radially perturbed by a few seeded low-frequency harmonics and stretched to a body-like
+    0.5 x 1.7 x 0.4 ellipsoid.  -> (verts float32 [V,3], faces int64 [F,3])."""
+    rng = np.random.RandomState(seed)
+    Rn, K = 84, 82
+    th = np.pi * (np.arange(1, Rn + 1) / (Rn + 1.0))
+    ph = 2 * np.pi * np.arange(K) / K
+    T, P = np.meshgrid(th, ph, indexing='ij')
+    rad = 1.0 + sum(rng.uniform(-0.08, 0.08) * np.cos(a * T + rng.uniform(0, 6)) * np.cos(b * P + rng.uniform(0, 6))
+                    for a, b in ((2, 1), (3, 2), (1, 3), (4, 1)))
+    pts = np.stack([rad * np.sin(T) * np.cos(P), rad * np.cos(T), rad * np.sin(T) * np.sin(P)], -1).reshape(-1, 3)
+    verts = np.concatenate([[[0, 1.0, 0]], pts, [[0, -1.0, 0]]]) * np.array([0.25, 0.85, 0.2])
+    ring = lambda r, k: 1 + r * K + (k % K)
+    faces = [[0, ring(0, k + 1), ring(0, k)] for k in range(K)]
+    for r in range(Rn - 1):
+        for k in range(K):
+            faces += [[ring(r, k), ring(r, k + 1), ring(r + 1, k)], [ring(r, k + 1), ring(r + 1, k + 1), ring(r + 1, k)]]
+    faces += [[len(verts) - 1, ring(Rn - 1, k), ring(Rn - 1, k + 1)] for k in range(K)]
+    return verts.astype(np.float32), np.array(faces, np.int64)
+
+
 def make_mean_param(seed: int = 3) -> np.ndarray:
     """mean_param [1,85] as built by tester.py:118-141: cam [0.9,0,0], pose root [pi,0,0]."""
     rng = np.random.RandomState(seed)

@@ -275,6 +275,32 @@ int hd_global_rigid(const float *Rs, const float *Js, const int *parents_host, f
 /* batch_orth_proj_idrot: X [N,P,3], cam [N,3] -> out [N,P,2]. */
 int hd_orth_proj(const float *X, const float *cam, float *out, int N, int P, void *stream);
 
+/* ---- Mesh rendering (the visualiser of src/util/render/nmr_renderer.py:43-240: NMR with camera_mode='look_at',
+ * perspective=False, anti_aliasing and fill_back on), one colour per mesh.  The model is R1-R8 of oracle/render_ref.py:
+ *   x = s*(X + tx), y = -s*(Y + ty), z = Z - eye_z  (R1); a 2S x 2S sample grid whose sample (r, c) sits at image
+ *   ((2c + 1 - 2S) / 2S, (2r + 1 - 2S) / 2S), the convention of kps (R2); strict barycentric coverage (R3); depth 1/sum(w_i/z_i),
+ *   dropped outside (near_z, far_z), nearest wins, ties to the lower face index (R4); each face once, lit with its eye-facing
+ *   normal (R5): colour * (ambient + directional * relu(n . light_dir)), light_dir used as given (R6); pixel = mean of its 2x2
+ *   samples with bg where empty, alpha = covered fraction (R7); out = uint8(rend) or, with a background image in [-1, 1],
+ *   uint8(img255 * (1 - alpha) + rend * alpha), rend = clip(rgb, 0, 1) * 255, img255 = (img + 1) * 0.5 * 255, float32 (R8).
+ * verts [N,V,3] with frame stride verts_ld floats (>= 3V), cam rows of 3 at stride cam_ld (so slices of verts_delta / omegas are read in
+ * place); faces int32 [F,3] (a face with an index outside [0, V) is skipped); background [N,S,S,3] fp32 or NULL; out_rgb uint8
+ * [N,S,S,3]; out_alpha fp32 [N,S,S] or NULL.  use_rot: vertices become rot * (v - mean_v) + mean_v with the per-frame vertex mean
+ * (VisRenderer.rotated, nmr_renderer.py:176-225); rot is row-major.  Bit-identical across launches, batch sizes and chunkings.
+ * Workspace: a [N, 2S, 2S] 64-bit z-buffer plus a [N, F] colour table, hd_render_workspace_bytes(N, S, F) bytes (0 when an
+ * argument is <= 0).  When the stream reaches the end of the call, the workspace starts with that z-buffer: uint64
+ * key = (float_bits(depth) << 32) | face per sample, all ones where empty (an inspection aid for tests and debugging).  HD_ERR_INVALID: a null pointer, S outside [1, 2048], N < 0, V or F <= 0, verts_ld < 3V or cam_ld < 3. */
+typedef struct {
+  float color[3], light_dir[3], ambient, directional, bg[3], near_z, far_z, eye_z;   /* NMR: eye_z = -(1/tan 30deg + 1) */
+  float rot[9];
+  int use_rot;
+} hd_render_params;                                   /* host struct */
+size_t hd_render_workspace_bytes(int N, int S, int F);
+int hd_render_mesh(const float *verts, long long verts_ld, int N, int V, const int *faces, int F, const float *cam, int cam_ld,
+                   const hd_render_params *p, const float *background /* [N,S,S,3] in [-1,1], nullable */, int S,
+                   unsigned char *out_rgb /* [N,S,S,3] */, float *out_alpha /* [N,S,S], nullable */, void *ws, size_t ws_bytes,
+                   void *stream);
+
 #ifdef __cplusplus
 }
 #endif
