@@ -56,6 +56,18 @@ class SmplConsts(C.Structure):
     ]
 
 
+class SmplGradConsts(C.Structure):
+    """Mirror of hd_smpl_grad_consts."""
+    _fields_ = [
+        ('num_verts', C.c_int), ('num_kps', C.c_int), ('num_tiles', C.c_int), ('tile_verts', C.c_int),
+        ('kpv_ptr', C.c_void_p), ('kpv_kidx', C.c_void_p), ('kpv_w', C.c_void_p),
+        ('lbt_ptr', C.c_void_p), ('lbt_v', C.c_void_p), ('lbt_w', C.c_void_p),
+    ]
+
+
+SMPL_GRAD_TILE, SMPL_GRAD_CLD = 256, 224       # HD_SMPL_GRAD_TILE, HD_SMPL_GRAD_CLD
+
+
 class RenderParams(C.Structure):
     """Mirror of hd_render_params."""
     _fields_ = [
@@ -111,6 +123,12 @@ SIGNATURES = {
     'hd_rot2aa': (_i, [_vp, _vp, _i, _vp]),
     'hd_global_rigid': (_i, [_vp, _vp, C.POINTER(C.c_int), _vp, _vp, _i, _i, _vp]),
     'hd_orth_proj': (_i, [_vp, _vp, _vp, _i, _i, _vp]),
+    'hd_smpl_backward_workspace_bytes': (_sz, [_i, _i]),
+    'hd_smpl_lbs_backward': (_i, [C.POINTER(SmplConsts), C.POINTER(SmplGradConsts), _vp, _ll, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    'hd_smpl_pose_backward': (_i, [C.POINTER(SmplConsts), _vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _i, _vp]),
+    'hd_rodrigues_backward': (_i, [_vp, _vp, _vp, _i, _vp]),
+    'hd_global_rigid_backward': (_i, [_vp, _vp, C.POINTER(C.c_int), _vp, _vp, _vp, _vp, _i, _i, _vp]),
+    'hd_orth_proj_backward': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     'hd_render_workspace_bytes': (_sz, [_i, _i, _i]),
     'hd_render_mesh': (_i, [_vp, _ll, _i, _i, _vp, _i, _vp, _i, C.POINTER(RenderParams), _vp, _i, _vp, _vp, _vp, _sz, _vp]),
 }

@@ -4,80 +4,14 @@
 // Replaces src/tf_smpl/batch_smpl.py:89-162, batch_lbs.py:15-60,133-194, projection.py:16-29 of the
 // reference (one TF op + HBM round trip per line there; three kernels and no materialised W/T here).
 #include "conv_common.cuh"
+#include "smpl_common.cuh"
 
 namespace {
 
-struct Tree {
-  int parent[24];
-  int depth[24];
-  int maxdepth;
-};
-
-__host__ bool build_tree(const int *parents, Tree &t) {
-  t.maxdepth = 0;
-  for (int i = 0; i < 24; ++i) {
-    int p = parents[i];
-    if (i == 0) { t.parent[0] = 0; t.depth[0] = 0; continue; }
-    if (p < 0 || p >= i) return false;           // batch_lbs.py:172-177 needs parent[i] < i
-    t.parent[i] = p;
-    t.depth[i] = t.depth[p] + 1;
-    if (t.depth[i] > t.maxdepth) t.maxdepth = t.depth[i];
-  }
-  return true;
-}
-
-// batch_lbs.py:42-60 (+ batch_skew :15-39): same operation order as the reference.
-__device__ __forceinline__ void rodrigues(float tx, float ty, float tz, float *R) {
-  const float eps = 1e-8f;
-  const float sx = tx + eps, sy = ty + eps, sz = tz + eps;
-  const float angle = sqrtf(sx * sx + sy * sy + sz * sz);
-  const float rx = tx / angle, ry = ty / angle, rz = tz / angle;
-  const float c = cosf(angle), s = sinf(angle);
-  const float oc = 1.0f - c;
-  R[0] = c + oc * (rx * rx);
-  R[1] = oc * (rx * ry) + s * (-rz);
-  R[2] = oc * (rx * rz) + s * ry;
-  R[3] = oc * (ry * rx) + s * rz;
-  R[4] = c + oc * (ry * ry);
-  R[5] = oc * (ry * rz) + s * (-rx);
-  R[6] = oc * (rz * rx) + s * (-ry);
-  R[7] = oc * (rz * ry) + s * rx;
-  R[8] = c + oc * (rz * rz);
-}
-
-// Forward kinematics over the tree, one lane per joint (lanes >= 24 idle but take part in shuffles).
-// In: local rotation Rl, rest joint J (per lane).  Out: world rotation Rw, world translation tw.
-__device__ __forceinline__ void fk_chain(const Tree &tree, int lane, const float *Rl, const float *J,
-                                         float *Rw, float *tw) {
-  const bool active = lane < 24;
-  const int par = active ? tree.parent[lane] : 0;
-  const int dep = active ? tree.depth[lane] : -1;
-  float tl[3];
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const float jp = __shfl_sync(0xffffffffu, J[c], par);
-    tl[c] = (dep == 0) ? J[c] : J[c] - jp;          // batch_lbs.py:170,173
-    tw[c] = tl[c];
-  }
-#pragma unroll
-  for (int i = 0; i < 9; ++i) Rw[i] = Rl[i];
-  for (int level = 1; level <= tree.maxdepth; ++level) {
-    float pR[9], pt[3];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) pR[i] = __shfl_sync(0xffffffffu, Rw[i], par);
-#pragma unroll
-    for (int i = 0; i < 3; ++i) pt[i] = __shfl_sync(0xffffffffu, tw[i], par);
-    if (dep == level) {                               // results[parent] x A_here, batch_lbs.py:175
-#pragma unroll
-      for (int r = 0; r < 3; ++r) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c)
-          Rw[r * 3 + c] = pR[r * 3 + 0] * Rl[0 * 3 + c] + pR[r * 3 + 1] * Rl[1 * 3 + c] + pR[r * 3 + 2] * Rl[2 * 3 + c];
-        tw[r] = pR[r * 3 + 0] * tl[0] + pR[r * 3 + 1] * tl[1] + pR[r * 3 + 2] * tl[2] + pt[r];
-      }
-    }
-  }
-}
+using hd_smpl::Tree;
+using hd_smpl::build_tree;
+using hd_smpl::rodrigues;
+using hd_smpl::fk_chain;
 
 // One warp per pose.  Writes Rs [N,24,9], Jtr [N,24,3] (optional), A12 [N,24,12] (rows of [R | t - R J]).
 __global__ void __launch_bounds__(128) smpl_pose_kernel(Tree tree, const float *__restrict__ beta, int beta_ld,

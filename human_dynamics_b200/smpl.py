@@ -11,6 +11,7 @@ import pickle
 
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 from ._lib import lib, check, fptr, dptr, current_stream
@@ -162,6 +163,10 @@ class SMPLConstants(object):
             self.w_lo = torch.from_numpy((wd - w_hi.astype(np.float32)).astype(np.float16)).to(dev)
         self.lbs_tc = bool(tc) and os.environ.get('HD_LBS_TC', '1') != '0' and (V * 3 * 4) % 8 == 0
         self.lbs_tc_min_batch = int(os.environ.get('HD_LBS_TC_MIN', '2112'))         # 132 SMs x 16 poses
+        # host copies for the backward's extra arrays, packed and uploaded on the first backward call (grad_state)
+        self._grad_src = (weights, kreg, dirs)
+        self._grad = None
+        self._bw_bufs = {}
 
     def workspace(self, N):
         need = int(lib.hd_smpl_workspace_bytes(N))
@@ -244,6 +249,138 @@ class SMPLConstants(object):
                                      N, mul, off, st), 'hd_smpl_joints')
 
 
+    # ---------------------------------------------------------------- backward (smpl_grad.cu) ----------------------------------------
+
+    def grad_state(self):
+        """Device arrays of hd_smpl_grad_consts and the packed dirs^T of the dc GEMM, built once on first use."""
+        if self._grad is None:
+            if self.blend is None:
+                raise _lib.HDError('the SMPL backward recomputes v_posed on the tensor-core blend: build SMPLConstants with tc=True')
+            from .nets import PackedConv
+            weights, kreg, dirs = self._grad_src
+            V, dev = self.num_verts, self.device
+            pk = pack_grad_arrays(weights, kreg)
+            keep = {k: torch.from_numpy(np.ascontiguousarray(v if len(v) else np.zeros(1, v.dtype))).to(dev) for k, v in pk.items()}
+            g = _lib.SmplGradConsts()
+            g.num_verts, g.num_kps = V, self.num_kps
+            g.tile_verts, g.num_tiles = _lib.SMPL_GRAD_TILE, (V + _lib.SMPL_GRAD_TILE - 1) // _lib.SMPL_GRAD_TILE
+            for k in ('kpv_ptr', 'kpv_kidx', 'kpv_w', 'lbt_ptr', 'lbt_v', 'lbt_w'):
+                setattr(g, k, keep[k].data_ptr())
+            # dc = dv_posed . dirs^T: K = vp_ld (zero rows past 3V), Cout = 224 (zero columns past 217), 3xTF32 on the fp32 operand.
+            # Gradients carry the loss's arbitrary scale, so they never go through the fp16 head / remainder split.
+            wt = np.zeros((self.vp_ld, _lib.SMPL_GRAD_CLD), np.float32)
+            wt[:V * 3, :217] = dirs.T
+            gemm = PackedConv(wt, dev, tc='tc3')
+            if gemm.tc != 'tf32':
+                raise _lib.HDError('dirs^T did not get the TF32 tensor-core packing (vp_ld %% 32 != 0?)')
+            self._grad = (g, keep, gemm)
+        return self._grad
+
+    def backward_workspace(self, N):
+        """Per-N buffers of one backward (hd_smpl_backward_workspace_bytes layout) plus the two bound GEMMs; bounded cache."""
+        if N in self._bw_bufs:
+            return self._bw_bufs[N]
+        g, keep, gemm = self.grad_state()
+        while len(self._bw_bufs) >= 2:
+            self._bw_bufs.pop(next(iter(self._bw_bufs)))
+        dev = self.device
+        ws = torch.empty(int(lib.hd_smpl_backward_workspace_bytes(N, self.num_verts)), dtype=torch.uint8, device=dev)
+        views, off = {}, 0
+        for name, cols, dt in (('A12', 288, torch.float32), ('dA12', 288, torch.float32), ('dc', _lib.SMPL_GRAD_CLD, torch.float32),
+                               ('rs', 216, torch.float32), ('coef_hi', 256, torch.float16), ('coef_lo', 256, torch.float16),
+                               ('vpos', self.vp_ld, torch.float32), ('dvpos', self.vp_ld, torch.float32)):
+            nb = N * cols * (4 if dt == torch.float32 else 2)
+            views[name] = ws[off:off + nb].view(dt).view(N, cols)
+            off += (nb + 255) // 256 * 256
+        assert off == ws.numel()
+        blend = self.blend.bind(None, N, 1, 1, views['vpos'], inp_split=(views['coef_hi'], views['coef_lo']), impl='tc3h')
+        dc = gemm.bind(views['dvpos'], N, 1, 1, views['dc'], impl='tc3')
+        if dc.d.impl != _lib.HD_IMPL_TC_3XTF32:
+            raise _lib.HDError('the dc GEMM must run on the 3xTF32 tensor-core kernel')
+        self._bw_bufs[N] = (ws, views, blend, dc)
+        return self._bw_bufs[N]
+
+    def backward(self, beta, theta, dverts=None, djoints=None, dRs=None, dJtr=None, dbeta=None, dtheta=None):
+        """Gradients of (verts, joints, Rs, Jtr) = forward(beta, theta) w.r.t. beta (N,10) and theta (N,72).
+
+        beta / theta: the forward's inputs (float32 CUDA, unit inner stride, any row stride).  d*: upstream gradients of the outputs,
+        dense, or None for zero.  dbeta / dtheta: optional output views (unit inner stride, any row stride), else allocated.
+        v_posed is recomputed (hd_smpl_pose + the tensor-core blend), not saved by the forward."""
+        for name, t, w in (('beta', beta, 10), ('theta', theta, 72)):
+            if not t.is_cuda or t.dtype != torch.float32:
+                raise _lib.HDError('SMPL %s must be a float32 CUDA tensor (no CPU fallback exists)' % name)
+            if t.dim() != 2 or t.shape[1] != w or t.stride(1) != 1:
+                raise _lib.HDError('SMPL %s must be (N,%d) with unit inner stride, got %s' % (name, w, tuple(t.shape)))
+        N, V, K = beta.shape[0], self.num_verts, self.num_kps
+        if theta.shape[0] != N:
+            raise _lib.HDError('SMPL batch mismatch')
+        dev = beta.device
+        dbeta = torch.empty((N, 10), dtype=torch.float32, device=dev) if dbeta is None else dbeta
+        dtheta = torch.empty((N, 72), dtype=torch.float32, device=dev) if dtheta is None else dtheta
+        if N == 0:
+            return dbeta, dtheta
+
+        def dense(t, shape, name):
+            if t is None:
+                return None
+            if not t.is_cuda or t.dtype != torch.float32 or tuple(t.shape) != shape:
+                raise _lib.HDError('SMPL gradient %s must be a float32 CUDA tensor of shape %s' % (name, shape))
+            return t.contiguous()
+        dverts = dense(dverts, (N, V, 3), 'dverts')
+        djoints = dense(djoints, (N, K, 3), 'djoints')
+        dRs = dense(dRs, (N, 24, 3, 3), 'dRs')
+        dJtr = dense(dJtr, (N, 24, 3), 'dJtr')
+        st = current_stream()
+        mesh = dverts is not None or (djoints is not None and K > 0)
+        dA12, dc = None, None
+        if mesh:
+            g, _, _ = self.grad_state()
+            ws, b, blend, dcop = self.backward_workspace(N)
+            if dverts is None:
+                dverts = torch.zeros((N, V, 3), dtype=torch.float32, device=dev)
+            check(lib.hd_smpl_pose(C.byref(self.c), fptr(beta), beta.stride(0), fptr(theta), theta.stride(0), N, None, None,
+                                   fptr(b['A12']), None, 256, dptr(b['coef_hi']), dptr(b['coef_lo']), None, None, 1, 0,
+                                   dptr(b['rs']), b['rs'].numel() * 4, st), 'hd_smpl_pose')
+            blend.run(st)
+            check(lib.hd_smpl_lbs_backward(C.byref(self.c), C.byref(g), fptr(b['vpos']), self.vp_ld, fptr(b['A12']), fptr(dverts),
+                                           fptr(djoints) if (djoints is not None and K > 0) else None, fptr(b['dvpos']),
+                                           fptr(b['dA12']), N, st), 'hd_smpl_lbs_backward')
+            dcop.run(st)
+            dA12, dc = b['dA12'], b['dc']
+        check(lib.hd_smpl_pose_backward(C.byref(self.c), fptr(beta), beta.stride(0), fptr(theta), theta.stride(0), N,
+                                        fptr(dA12) if dA12 is not None else None, fptr(dc) if dc is not None else None,
+                                        _lib.SMPL_GRAD_CLD, fptr(dRs) if dRs is not None else None,
+                                        fptr(dJtr) if dJtr is not None else None, fptr(dbeta), dbeta.stride(0), fptr(dtheta),
+                                        dtheta.stride(0), st), 'hd_smpl_pose_backward')
+        return dbeta, dtheta
+
+
+def pack_grad_arrays(weights, kp_regressor, tile=None):
+    """Host packing of the backward's extra SMPL arrays (hd_smpl_grad_consts), from the dense float64 skinning weights [V,24] and
+    keypoint regressor [K,V]:
+      kpv_ptr / kpv_kidx / kpv_w: the regressor vertex-major (CSR over vertices, keypoint ids ascending);
+      lbt_ptr / lbt_v / lbt_w:    the non-zero skinning weights joint-major inside each tile of `tile` vertices."""
+    tile = _lib.SMPL_GRAD_TILE if tile is None else tile
+    weights = np.asarray(weights, np.float64)
+    kreg = np.asarray(kp_regressor, np.float64)
+    V = weights.shape[0]
+    kv, kk = np.nonzero(kreg.T)                                            # row-major over (v, k): vertices, then keypoints ascending
+    kpv_ptr = np.zeros(V + 1, np.int64)
+    np.add.at(kpv_ptr, kv + 1, 1)
+    ptr, vv, ww = [0], [], []
+    for t in range((V + tile - 1) // tile):
+        blk = weights[t * tile:(t + 1) * tile]
+        for k in range(weights.shape[1]):
+            nz = np.nonzero(blk[:, k])[0]
+            vv.append(nz + t * tile)
+            ww.append(blk[nz, k])
+            ptr.append(ptr[-1] + len(nz))
+    return {'kpv_ptr': np.cumsum(kpv_ptr).astype(np.int32), 'kpv_kidx': kk.astype(np.int32),
+            'kpv_w': kreg.T[kv, kk].astype(np.float32),
+            'lbt_ptr': np.asarray(ptr, np.int32), 'lbt_v': np.concatenate(vv).astype(np.int32),
+            'lbt_w': np.concatenate(ww).astype(np.float32)}
+
+
 def _noop():
     pass
 
@@ -302,3 +439,102 @@ def batch_orth_proj_idrot(X, camera):
     out = torch.empty((N, P, 2), dtype=torch.float32, device=X.device)
     check(lib.hd_orth_proj(fptr(X), fptr(camera), fptr(out), N, P, current_stream()), 'hd_orth_proj')
     return out
+
+
+# ------------------------------------------------------------------------ autograd ---------------------------------------------------
+# The four entry points below are what src/tf_smpl/* switch to when grad mode is on and an input requires grad.  Each node saves only
+# its inputs (a few hundred bytes per pose for SMPL: v_posed is recomputed in the backward) and is once-differentiable: asking for
+# a second derivative raises.
+
+class SMPLFunction(torch.autograd.Function):
+    """(beta (N,10), theta (N,72)) -> (verts, joints, Rs, Jtr) of SMPLConstants.forward, differentiable w.r.t. beta and theta."""
+
+    @staticmethod
+    def forward(ctx, consts, beta, theta):
+        o = consts.forward(beta, theta)
+        ctx.consts = consts
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(beta, theta)
+        return o['verts'], o['joints'], o['Rs'], o['Jtr']
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dverts, djoints, dRs, dJtr):
+        beta, theta = ctx.saved_tensors
+        dbeta, dtheta = ctx.consts.backward(beta, theta, dverts, djoints, dRs, dJtr)
+        return None, (dbeta if ctx.needs_input_grad[1] else None), (dtheta if ctx.needs_input_grad[2] else None)
+
+
+class RodriguesFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, theta):
+        theta = theta.contiguous()
+        ctx.save_for_backward(theta)
+        return batch_rodrigues(theta)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dR):
+        theta, = ctx.saved_tensors
+        dR = dR.contiguous()
+        dtheta = torch.empty_like(theta)
+        check(lib.hd_rodrigues_backward(fptr(theta), fptr(dR), fptr(dtheta), theta.shape[0], current_stream()), 'hd_rodrigues_backward')
+        return dtheta
+
+
+class GlobalRigidFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, Rs, Js, parent, rotate_base):
+        Rs, Js = Rs.contiguous(), Js.contiguous()
+        new_J, A = batch_global_rigid_transformation(Rs, Js, parent, rotate_base)
+        ctx.par = (C.c_int * 24)(*[(-1 if (int(p) < 0 or int(p) >= 2 ** 31) else int(p)) for p in np.asarray(parent).tolist()])
+        ctx.rotate_base = int(bool(rotate_base))
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(Rs, Js)
+        return new_J, A
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dnew_J, dA):
+        Rs, Js = ctx.saved_tensors
+        N = Rs.shape[0]
+        dnew_J = dnew_J.contiguous() if dnew_J is not None else None
+        dA = dA.contiguous() if dA is not None else None
+        dRs, dJs = torch.empty_like(Rs), torch.empty_like(Js)
+        check(lib.hd_global_rigid_backward(fptr(Rs), fptr(Js), ctx.par, fptr(dnew_J) if dnew_J is not None else None,
+                                           fptr(dA) if dA is not None else None, fptr(dRs), fptr(dJs), N, ctx.rotate_base,
+                                           current_stream()), 'hd_global_rigid_backward')
+        return dRs, dJs, None, None
+
+
+class OrthProjFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, X, camera):
+        X = X.contiguous()
+        cam = camera.reshape(-1, 3).contiguous()
+        ctx.cam_shape = camera.shape
+        ctx.save_for_backward(X, cam)
+        return batch_orth_proj_idrot(X, cam)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout):
+        X, cam = ctx.saved_tensors
+        N, P = X.shape[0], X.shape[1]
+        dout = dout.contiguous()
+        dX, dcam = torch.empty_like(X), torch.empty_like(cam)
+        check(lib.hd_orth_proj_backward(fptr(X), fptr(cam), fptr(dout), fptr(dX), fptr(dcam), N, P, current_stream()),
+              'hd_orth_proj_backward')
+        return dX, dcam.reshape(ctx.cam_shape)
+
+
+def _needs_grad(*ts):
+    return torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in ts)
+
+
+def _cuda_f32(name, *ts):
+    for t in ts:
+        if not t.is_cuda:
+            raise _lib.HDError('%s: CUDA tensors required (no CPU fallback exists)' % name)
+        if t.dtype != torch.float32:
+            raise _lib.HDError('%s: the differentiable path takes float32 tensors, got %s' % (name, t.dtype))

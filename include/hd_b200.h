@@ -275,6 +275,58 @@ int hd_global_rigid(const float *Rs, const float *Js, const int *parents_host, f
 /* batch_orth_proj_idrot: X [N,P,3], cam [N,3] -> out [N,P,2]. */
 int hd_orth_proj(const float *X, const float *cam, float *out, int N, int P, void *stream);
 
+/* ---- SMPL backward (reverse mode of the forward above; gradients w.r.t. beta / theta / the helpers' inputs, never the constants) ----
+ * Deterministic: no floating-point atomics, every reduction runs in a fixed order, and pose n's gradients depend only on pose n's
+ * inputs and upstream gradients (bit-identical across launches, batch splits and permutations).  Any upstream gradient pointer marked
+ * nullable stands for zeros.
+ *
+ * Extra model arrays the backward reads, packed once on the host (human_dynamics_b200/smpl.py:pack_grad_arrays) and passed explicitly:
+ *   kpv_ptr [V+1] / kpv_kidx / kpv_w [kp_nnz_total]: the keypoint regressor vertex-major (CSR over vertices, keypoint ids ascending) --
+ *     the transpose of hd_smpl_consts' CSC copy;
+ *   lbt_ptr [num_tiles*24+1] / lbt_v / lbt_w: the non-zero skinning weights joint-major within each tile of HD_SMPL_GRAD_TILE vertices
+ *     (entries of tile t, joint k at [lbt_ptr[t*24+k], lbt_ptr[t*24+k+1]), vertex ids ascending), num_tiles = ceil(V / HD_SMPL_GRAD_TILE).
+ * Full sequence for one batch (see INTEGRATION.md):
+ *   hd_smpl_pose (recompute A12 and the blend operand) -> hd_conv_gemm (recompute v_posed) -> hd_smpl_lbs_backward (g_v, dL/dv_posed,
+ *   dL/dA) -> hd_conv_gemm (dL/dc = dL/dv_posed . dirs^T, 3xTF32) -> hd_smpl_pose_backward (FK + Rodrigues backward -> dL/dbeta, dL/dtheta).
+ * hd_smpl_backward_workspace_bytes(N, V): one buffer holding, in this order and each at a 256-byte boundary, A12 f32 [N,288],
+ * dA12 f32 [N,288], dc f32 [N,HD_SMPL_GRAD_CLD], rs f32 [N,216] (hd_smpl_pose's ws), coef_hi / coef_lo f16 [N,256] each,
+ * v_posed f32 [N,vp_ld] and dv_posed f32 [N,vp_ld], vp_ld = roundup4(3V).  0 when N <= 0 or V <= 0. */
+enum { HD_SMPL_GRAD_TILE = 256, HD_SMPL_GRAD_CLD = 224 };
+typedef struct {
+  int num_verts, num_kps, num_tiles, tile_verts;   /* tile_verts must be HD_SMPL_GRAD_TILE */
+  const int *kpv_ptr;          /* [V+1] */
+  const int *kpv_kidx;         /* [kp_nnz_total] */
+  const float *kpv_w;          /* [kp_nnz_total] */
+  const int *lbt_ptr;          /* [num_tiles*24+1] */
+  const int *lbt_v;            /* [lbt_ptr[num_tiles*24]] */
+  const float *lbt_w;          /* [lbt_ptr[num_tiles*24]] */
+} hd_smpl_grad_consts;
+size_t hd_smpl_backward_workspace_bytes(int N, int V);
+/* Skinning + keypoint backward (batch_smpl.py:141-157 reversed):  g_v = dverts_v + sum_k Kreg[k,v] djoints_k;
+ * dv_posed_v = (sum_k w_vk R_k)^T g_v;  dA12_k = sum_v w_vk g_v (x) [v_posed_v; 1]  (rows of [R | t], 12 per joint).
+ * v_posed [N, vp_ld] (recomputed), A12 [N,288] from hd_smpl_pose, dverts [N,V,3], djoints [N,K,3] (nullable) -> dv_posed [N, vp_ld]
+ * (columns 3V..vp_ld-1 set to 0, so it can be the A operand of the dc GEMM), dA12 [N,288]. */
+int hd_smpl_lbs_backward(const hd_smpl_consts *c, const hd_smpl_grad_consts *g, const float *v_posed, long long vp_ld, const float *A12,
+                         const float *dverts, const float *djoints, float *dv_posed, float *dA12, int N, void *stream);
+/* Pose-side backward, one warp per pose (batch_smpl.py:115-137, batch_lbs.py:42-60,133-194 reversed): recomputes J, R and the FK chain
+ * from beta / theta, walks the tree levels in reverse from dA12 (nullable) and dJtr [N,24,3] (nullable), adds dRs [N,24,3,3] (nullable)
+ * and dc[n, 10:217] (the pose-blend coefficients R_j - I, j = 1..23) to the local rotations, differentiates Rodrigues in fp64 (the
+ * reference's expression with the +1e-8 shift; finite at theta = 0), and writes
+ *   dbeta[n*dbeta_ld + b] = dc[n, b] + sum_j J_shapedirs[b, j] . dJ_j,   dtheta[n*dtheta_ld + 3j + i].
+ * dc rows of >= 217 at stride dc_ld (nullable). */
+int hd_smpl_pose_backward(const hd_smpl_consts *c, const float *beta, int beta_ld, const float *theta, int theta_ld, int N,
+                          const float *dA12, const float *dc, int dc_ld, const float *dRs, const float *dJtr, float *dbeta, int dbeta_ld,
+                          float *dtheta, int dtheta_ld, void *stream);
+/* batch_rodrigues backward: theta [M,3], dR [M,3,3] -> dtheta [M,3]. */
+int hd_rodrigues_backward(const float *theta, const float *dR, float *dtheta, int M, void *stream);
+/* batch_global_rigid_transformation backward: Rs [N,24,3,3], Js [N,24,3], parents host int[24], dnew_J [N,24,3] (nullable),
+ * dA [N,24,4,4] (nullable; its constant last rows are ignored) -> dRs [N,24,3,3], dJs [N,24,3]. */
+int hd_global_rigid_backward(const float *Rs, const float *Js, const int *parents_host, const float *dnew_J, const float *dA44, float *dRs,
+                             float *dJs, int N, int rotate_base, void *stream);
+/* batch_orth_proj_idrot backward: X [N,P,3], cam [N,3], dout [N,P,2] -> dX [N,P,3] (z column 0), dcam [N,3]:
+ * dX_xy = s dout, ds = sum_p (xy + t) . dout_p, dt = s sum_p dout_p. */
+int hd_orth_proj_backward(const float *X, const float *cam, const float *dout, float *dX, float *dcam, int N, int P, void *stream);
+
 /* ---- Mesh rendering (the visualiser of src/util/render/nmr_renderer.py:43-240: NMR with camera_mode='look_at',
  * perspective=False, anti_aliasing and fill_back on), one colour per mesh.  The model is R1-R8 of oracle/render_ref.py:
  *   x = s*(X + tx), y = -s*(Y + ty), z = Z - eye_z  (R1); a 2S x 2S sample grid whose sample (r, c) sits at image

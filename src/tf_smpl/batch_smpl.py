@@ -5,7 +5,7 @@ To get original smpl joints, use self.J_transformed.
 """
 import torch
 
-from human_dynamics_b200.smpl import SMPLConstants
+from human_dynamics_b200.smpl import SMPLConstants, SMPLFunction, _needs_grad, _cuda_f32
 
 
 class SMPL(object):
@@ -24,6 +24,9 @@ class SMPL(object):
 
         Updates self.J_transformed (N x 24 x 3).  Returns joints (N x K x 3), or
         (verts N x 6890 x 3, joints, Rs N x 24 x 3 x 3) if get_skin.   (batch_smpl.py:89-162)
+
+        When grad mode is on and beta or theta requires grad, all four outputs are on the autograd graph (backward on the GPU,
+        human_dynamics_b200/csrc/smpl_grad.cu); otherwise no graph is built.
         """
         N = beta.shape[0]
         beta = beta.reshape(N, 10)
@@ -32,6 +35,10 @@ class SMPL(object):
             beta = beta.contiguous()
         if theta.stride(1) != 1:
             theta = theta.contiguous()
+        if _needs_grad(beta, theta):
+            _cuda_f32('SMPL', beta, theta)
+            verts, joints, Rs, self.J_transformed = SMPLFunction.apply(self.consts, beta, theta)
+            return (verts, joints, Rs) if get_skin else joints
         o = self.consts.forward(beta.float(), theta.float())
         self.J_transformed = o['Jtr']
         if get_skin:
