@@ -23,7 +23,8 @@
 // Persistent: grid = min(#tiles, #SMs); each CTA walks tiles blockIdx.x, +gridDim.x, ...  Barrier phases run
 // continuously across tiles, and the producers keep prefetching the next tile's chunks while the consumers run the
 // fused epilogue (scale/shift, residual, ReLU, fp32 output or its strided subsample, the next layer's fp16 pair)
-// straight from the accumulator fragments.
+// straight from the accumulator fragments.  RES (pre-split input, residual row-aligned with the output, K <= 512): each
+// consumer warpgroup's 64 residual rows arrive by TMA in a shared-memory slot while the tile's main loop runs.
 //
 // Warp roles:
 //   warps 0-7    two consumer warpgroups: wgmma issue, drains, epilogue (warpgroup g owns tile rows 64 g .. 64 g + 63)
@@ -46,9 +47,10 @@ constexpr int W_PROD = 8;                   // first producer warp
 
 using namespace ptx;
 
-template <bool HALF, bool ASPLIT, int BN>
+template <bool HALF, bool ASPLIT, int BN, bool RES = false>
 struct Cfg {
   static_assert(BN == 64 || (BN == 128 && HALF && ASPLIT), "128-wide N tiles: pre-split fp16 path only");
+  static_assert(!RES || ASPLIT, "residual by TMA: pre-split fp16 path only");
   static constexpr int PROD_THREADS = BN == 128 ? 128 : 256;
   static constexpr int NUM_THREADS = 256 + PROD_THREADS;
   static constexpr int ROW_STEP = PROD_THREADS / 8;             // a producer thread's rows: rb + ROW_STEP * i
@@ -56,11 +58,14 @@ struct Cfg {
   static constexpr int PROD_REGS = BN == 128 ? 40 : 104, CONS_REGS = BN == 128 ? 232 : 152;
   static_assert(256 * CONS_REGS + PROD_THREADS * PROD_REGS <= 65536, "setmaxnreg split beyond the register file");
   static constexpr int NACC = BN / 2;                           // fp32 registers of one m64nBN fragment per thread
-  static constexpr int STAGES = BN == 128 ? 3 : 4;
+  // RES, BN = 128: the 64 KB residual tile does not fit beside three 64 KB stages.  Residual layers have K <= 512 (<= 8 chunks).
+  static constexpr int STAGES = BN == 128 ? (RES ? 2 : 3) : 4;
   static constexpr int BKE = HALF ? 64 : 32;                    // K elements per chunk (one 128-byte row)
   static constexpr int B_TILE_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
-  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int RES_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int RES_SLOT_BYTES = RES ? 64 * BN * 4 : 0; // one warpgroup's 64 rows x BN fp32 residual (BN / 32 TMA boxes)
+  static constexpr int BAR_OFFSET = RES_OFFSET + 2 * RES_SLOT_BYTES;
   static constexpr int SMEM_BYTES = BAR_OFFSET + 128 + 1024;    // + alignment slack
   static_assert(SMEM_BYTES <= 232448, "dynamic shared memory beyond the 227 KB a CTA can opt into");
   static constexpr int PF = HALF ? 2 : 3;                       // producer prefetch ring depth (chunks in flight per thread)
@@ -72,10 +77,11 @@ struct RowState {       // R output rows of one producer thread: image index and
   int n[R], iy[R], ix[R];
 };
 
-template <bool SPLIT, int PCH, bool HALF, bool GATHER, bool ASPLIT, int BN>
-__global__ void __launch_bounds__((Cfg<HALF, ASPLIT, BN>::NUM_THREADS), 1)
-conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap_hi, const __grid_constant__ CUtensorMap tmap_lo) {
-  using C = Cfg<HALF, ASPLIT, BN>;
+template <bool SPLIT, int PCH, bool HALF, bool GATHER, bool ASPLIT, int BN, bool RES>
+__global__ void __launch_bounds__((Cfg<HALF, ASPLIT, BN, RES>::NUM_THREADS), 1)
+conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap_hi, const __grid_constant__ CUtensorMap tmap_lo,
+                    const __grid_constant__ CUtensorMap tmap_res) {
+  using C = Cfg<HALF, ASPLIT, BN, RES>;
   constexpr int BKE = C::BKE, PF = C::PF, V = C::V, STAGES = C::STAGES, R = C::ROWS, RS = C::ROW_STEP, NA = C::NACC;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -83,6 +89,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
   const uint32_t bar_base = smem_base + C::BAR_OFFSET;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  auto res_bar = [&](int g) { return bar_base + 8u * (2 * STAGES + g); };   // RES: warpgroup g's residual slot has landed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_k = (GATHER ? p.K_pad : p.K) / BKE;   // GATHER: ragged Cin (conv1: K=147 zero-padded to 192)
@@ -96,6 +103,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
                                                   // + 1 arrive.expect_tx from the thread that issues the B load
       mbar_init(empty_bar(s), 8);    // one arrive per consumer warp once its wgmmas have read the stage
     }
+    if (RES) for (int g = 0; g < 2; ++g) mbar_init(res_bar(g), 1);   // one arrive.expect_tx per tile
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -436,13 +444,30 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(C::CONS_REGS));
     const int wg = warp >> 2;                             // rows 64 wg .. 64 wg + 63 of the tile
     const bool prof = p.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0;
-    long long t_wait = 0, t_epi = 0, t_start = prof ? clock64() : 0;
+    long long t_wait = 0, t_epi = 0, t_start = prof && !RES ? clock64() : 0;
+    if (RES && prof) p.dbg[2] = clock64();    // start stamp in memory (RES, BN = 128: keeps the consumers within 232 registers spill-free)
     const int hw = p.Ho * p.Wo;
     const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's fragment rows: frow, frow + 8
     const int fcol = 2 * (lane & 3);                            // and columns 8 j + fcol, + 1
     float acc[NA], accx[NA], sums[NA];
 #pragma unroll
     for (int i = 0; i < NA; ++i) { acc[i] = 0.f; accx[i] = 0.f; }
+    // RES: the warpgroup's 64 residual rows of a tile arrive by TMA in 32-column boxes (128-byte swizzle: row r at r * 128 B, its
+    // 16-byte piece k at (k ^ (r & 7)) * 16), issued by the warpgroup's first thread as soon as the previous tile's epilogue has read
+    // the slot, so the load overlaps the tile's main loop.  Boxes wholly past M or Cout are not loaded (their values are never read);
+    // partial ones are zero-filled by TMA and count their full bytes.
+    const uint8_t *res_sm = smem + C::RES_OFFSET + wg * C::RES_SLOT_BYTES;
+    const bool res_issuer = RES && (threadIdx.x & 127) == 0;
+    auto load_res = [&](int ti) {
+      const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
+      const int r0 = (tile / tiles_n) * BM + 64 * wg, c0 = (tile % tiles_n) * BN;
+      const int cols = p.Cout - c0 < BN ? p.Cout - c0 : BN;
+      const int boxes = r0 < p.M ? (cols + 31) / 32 : 0;
+      const uint32_t slot = smem_base + C::RES_OFFSET + wg * C::RES_SLOT_BYTES;
+      mbar_arrive_expect_tx(res_bar(wg), boxes * (64 * 128));
+      for (int b = 0; b < boxes; ++b) tma_load_2d(slot + b * (64 * 128), &tmap_res, res_bar(wg), c0 + 32 * b, r0);
+    };
+    if (res_issuer && my_tiles > 0) load_res(0);
     int q = 0;
     for (int ti = 0; ti < my_tiles; ++ti) {
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
@@ -501,6 +526,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         for (int i = 0; i < NA; ++i) sums[i] += accx[i] * (HALF ? (1.0f / 2048.0f) : 1.0f);
       }
       long long te0 = prof ? clock64() : 0;
+      if (RES) mbar_wait(res_bar(wg), (uint32_t)ti & 1u);
       // Epilogue from the fragments: per row, per pair of adjacent columns (8-byte fp32 / 4-byte fp16-pair stores; the four
       // threads of a quad cover 8 contiguous columns of a row).  v = acc * scale + shift (+ residual) (ReLU) -> fp32 output
       // (or its strided subsample), and the next layer's pre-activation relu?(v * s2 + b2) as an fp16 head / remainder pair.
@@ -509,13 +535,16 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         const int m = m0 + frow + 8 * h;
         if (m >= p.M) continue;
         int n_img = 0, oy = 0, ox = 0;
-        if (p.out_sub || (p.res && !(p.res_stride == 1 && p.res_H == p.Ho && p.res_W == p.Wo))) {
+        if (p.out_sub || (!RES && p.res && !(p.res_stride == 1 && p.res_H == p.Ho && p.res_W == p.Wo))) {
           n_img = m / hw;
           const int r = m - n_img * hw;
           oy = r / p.Wo; ox = r - oy * p.Wo;
         }
+        // RES: this thread's residual row in the slot; its 8-byte pair of columns 8 j + fcol lies in box j / 4, piece 2 (j % 4) + fcol / 4
+        const uint8_t *rsrow = res_sm + (frow - 64 * wg + 8 * h) * 128 + 8 * (lane & 1);
+        const uint32_t rsw = (uint32_t)(lane >> 2);            // the row's swizzle: (frow + 8 h) & 7
         const float *rrow = nullptr;
-        if (p.res) {
+        if (!RES && p.res) {
           const size_t rr = (p.res_stride == 1 && p.res_H == p.Ho && p.res_W == p.Wo)
                                 ? (size_t)m
                                 : ((size_t)n_img * p.res_H + (size_t)oy * p.res_stride) * p.res_W + (size_t)ox * p.res_stride;
@@ -540,7 +569,11 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           if (p.vec_out) {                              // Cout % 4 == 0, 16-byte aligned rows and vectors: pairs are 8-byte aligned
             if (p.post_scale) { const float2 sc = __ldg(reinterpret_cast<const float2 *>(p.post_scale + c)); y[0] *= sc.x; y[1] *= sc.y; }
             if (p.post_shift) { const float2 sh = __ldg(reinterpret_cast<const float2 *>(p.post_shift + c)); y[0] += sh.x; y[1] += sh.y; }
-            if (rrow) { const float2 r = *reinterpret_cast<const float2 *>(rrow + c); y[0] += r.x; y[1] += r.y; }
+            if (RES) {
+              const uint32_t piece = (uint32_t)(2 * (j & 3) + ((lane & 3) >> 1)) ^ rsw;
+              const float2 r = *reinterpret_cast<const float2 *>(rsrow + (j >> 2) * (64 * 128) + piece * 16);
+              y[0] += r.x; y[1] += r.y;
+            } else if (rrow) { const float2 r = *reinterpret_cast<const float2 *>(rrow + c); y[0] += r.x; y[1] += r.y; }
             if (p.post_relu) { y[0] = fmaxf(y[0], 0.f); y[1] = fmaxf(y[1], 0.f); }
             if (orow) *reinterpret_cast<float2 *>(orow + c) = make_float2(y[0], y[1]);
             if (hrow) {       // the next layer's A operand: second affine (+ReLU) = its pre-activation, split into fp16 head/remainder
@@ -567,9 +600,13 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           }
         }
       }
+      if (RES && ti + 1 < my_tiles) {
+        named_bar_sync(1 + wg, 128);                       // every thread of the warpgroup has read the slot
+        if (res_issuer) load_res(ti + 1);
+      }
       if (prof) t_epi += clock64() - te0;
     }
-    if (prof) { p.dbg[2] = clock64() - t_start; p.dbg[3] = t_wait; p.dbg[4] = t_epi; }
+    if (prof) { p.dbg[2] = clock64() - (RES ? p.dbg[2] : t_start); p.dbg[3] = t_wait; p.dbg[4] = t_epi; }
   }
 }
 
@@ -593,9 +630,9 @@ EncodeTiledFn get_encode_fn() {
 
 constexpr int kMaxDevices = 64;
 
-template <bool SPLIT, int PCH, bool HALF, bool GATHER = false, bool ASPLIT = false, int BN = 64>
+template <bool SPLIT, int PCH, bool HALF, bool GATHER = false, bool ASPLIT = false, int BN = 64, bool RES = false>
 int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
-  using C = Cfg<HALF, ASPLIT, BN>;
+  using C = Cfg<HALF, ASPLIT, BN, RES>;
   // function attributes and the SM count are per device: a process may drive several GPUs through this library
   static bool configured[kMaxDevices] = {};
   static int num_sms[kMaxDevices] = {};
@@ -603,7 +640,7 @@ int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= kMaxDevices) { set_last_error_text("conv_gemm_tc: device ordinal out of range"); return HD_ERR_UNSUPPORTED; }
   if (!configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN>,
+    cudaError_t e = cudaFuncSetAttribute(conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (e != cudaSuccess) { set_last_error("conv_gemm_tc attr", e); return HD_ERR_CUDA; }
     cudaDeviceGetAttribute(&num_sms[dev], cudaDevAttrMultiProcessorCount, dev);
@@ -616,9 +653,31 @@ int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
   const void *mlo = d->tmap_hi_n64 ? d->tmap_lo_n64 : d->tmap_lo;
   memcpy(&thi, mhi, sizeof(CUtensorMap));
   memcpy(&tlo, mlo ? mlo : mhi, sizeof(CUtensorMap));     // mlo is null only for 1xTF32, which never loads it (launch_conv_tc)
+  // RES: the residual map is encoded here from p.res on every launch, never taken from the descriptor's activation maps, so it
+  // always describes the buffer this launch reads.  Box: 32 fp32 columns (one 128-byte swizzle row) x 64 rows (one warpgroup).
+  alignas(64) CUtensorMap tres;
+  if (RES) {
+    EncodeTiledFn fn = get_encode_fn();
+    if (!fn) { set_last_error_text("cuTensorMapEncodeTiled unavailable (no CUDA driver?)"); return HD_ERR_UNSUPPORTED; }
+    const cuuint64_t gdim[2] = {(cuuint64_t)p.Cout, (cuuint64_t)p.M};
+    const cuuint64_t gstride[1] = {(cuuint64_t)p.res_ld * 4u};
+    const cuuint32_t box[2] = {32u, 64u};
+    const cuuint32_t estr[2] = {1u, 1u};
+    CUresult r = fn(&tres, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(p.res), gdim, gstride, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      char msg[96];
+      snprintf(msg, sizeof(msg), "cuTensorMapEncodeTiled (residual) failed with CUresult %d", (int)r);
+      set_last_error_text(msg);
+      return HD_ERR_CUDA;
+    }
+  } else {
+    memcpy(&tres, &thi, sizeof(CUtensorMap));             // not read
+  }
   const int num_tiles = ceil_div(p.M, BM) * ceil_div(p.Cout, BN);
   dim3 grid(num_tiles < num_sms[dev] ? num_tiles : num_sms[dev]);     // persistent: one CTA per SM walks the tile list
-  conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN><<<grid, C::NUM_THREADS, C::SMEM_BYTES, st>>>(p, thi, tlo);
+  conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES><<<grid, C::NUM_THREADS, C::SMEM_BYTES, st>>>(p, thi, tlo, tres);
   return check_launch("conv_gemm_tc_kernel");
 }
 
@@ -675,7 +734,13 @@ int launch_conv_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) 
       set_last_error_text("hd_conv_gemm(tc split-A): needs Cin % 64 == 0, in_ld % 8 == 0, aligned in_hi/in_lo, no prologue");
       return HD_ERR_INVALID;
     }
-    return wide_n_tile(p) ? launch_tc<true, 2, true, false, true, 128>(p, d, st) : launch_tc<true, 2, true, false, true>(p, d, st);
+    // A residual row-aligned with the output (row m of `res` belongs to output row m) is loaded by TMA into shared memory ahead of
+    // the epilogue; vec_out (checked above) gives it the 16-byte aligned base and row pitch a tensor map needs.  Residual layers
+    // have short K, so the 128-wide tile gives up its third stage for the slots.
+    const bool res_rows = p.res && p.res_stride == 1 && p.res_H == p.Ho && p.res_W == p.Wo && p.K <= 8 * 64;
+    if (wide_n_tile(p))
+      return res_rows ? launch_tc<true, 2, true, false, true, 128, true>(p, d, st) : launch_tc<true, 2, true, false, true, 128>(p, d, st);
+    return res_rows ? launch_tc<true, 2, true, false, true, 64, true>(p, d, st) : launch_tc<true, 2, true, false, true>(p, d, st);
   }
   if (half && p.Cin % bke != 0) {      // ragged Cin (resnet conv1: 7x7x3): element-wise gather producer, K zero-padded
     const int segp = (p.KW * p.Cin + 7) & ~7;
