@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(_HERE, 'libhd_b200.so')
 HD_IMPL_SIMT, HD_IMPL_TC_3XTF32, HD_IMPL_TC_1XTF32, HD_IMPL_TC_3XF16 = 0, 1, 2, 3
 HD_CONV_NO_TMA_EPILOGUE = 1
 HD_CONV_INPUT_PLANES = 2
+HD_PACK_FORWARD, HD_PACK_BACKWARD_DATA = 0, 1
 IMPL_BY_NAME = {'simt': HD_IMPL_SIMT, 'tc3': HD_IMPL_TC_3XTF32, 'tc1': HD_IMPL_TC_1XTF32, 'tc3h': HD_IMPL_TC_3XF16}
 
 
@@ -129,6 +130,14 @@ SIGNATURES = {
     'hd_rodrigues_backward': (_i, [_vp, _vp, _vp, _i, _vp]),
     'hd_global_rigid_backward': (_i, [_vp, _vp, C.POINTER(C.c_int), _vp, _vp, _vp, _vp, _i, _i, _vp]),
     'hd_orth_proj_backward': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
+    'hd_pack_weight': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp]),
+    'hd_transpose_split': (_i, [_vp, _ll, _i, _ll, _i, _vp, _vp, _ll, _i, _ll, _vp]),
+    'hd_im2col_t': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp, _ll, _ll, _vp]),
+    'hd_groupnorm_relu_backward': (_i, [_vp] * 8 + [_i, _i, _i, _i, _f, _i, _vp]),
+    'hd_col_sum': (_i, [_vp, _ll, _i, _ll, _vp, _vp]),
+    'hd_relu_backward': (_i, [_vp, _vp, _vp, _ll, _vp]),
+    'hd_fc_small_dgrad': (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp]),
+    'hd_add_strided': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _vp]),
     'hd_render_workspace_bytes': (_sz, [_i, _i, _i]),
     'hd_render_mesh': (_i, [_vp, _ll, _i, _i, _vp, _i, _vp, _i, C.POINTER(RenderParams), _vp, _i, _vp, _vp, _vp, _sz, _vp]),
 }

@@ -1,0 +1,741 @@
+"""Training surface of the temporal model: f_movie ("az_fc2_groupnorm"), the IEF heads (main + delta), `mean_param` and the fc2_res
+hallucinator as torch parameters, differentiable on the GPU.
+
+This is what the reference trains in its default configuration (freeze_phi=True, precomputed_phi=True: src/config.py): everything
+after the ResNet.  Each forward runs the kernels and the packing of the inference plans (nets.FMoviePlan / IEFPlan fast heads,
+engine.PackedHal), so its outputs are bit-identical to HMMREngine's; the weights are packed on the device (hd_pack_weight) and repacked
+before a forward whenever a parameter was changed in place (optimizer.step()).  The backward (csrc/net_grad.cu + hd_conv_gemm in its
+3xTF32 mode) is first-order, deterministic and follows the inference graph: dropout is the identity (is_training=False).
+
+All arithmetic goes through libhd_b200.so; torch provides buffers, streams and the autograd plumbing.  The user's loss and optimizer
+are ordinary torch code:
+
+    model = TemporalModel(weights)                     # anything engine.load_weights accepts
+    opt = torch.optim.Adam(model.parameters(), 1e-5)
+    out = model.predict_from_features(phi, smpl)       # phi (B,T,2048), smpl = src.tf_smpl.batch_smpl.SMPL
+    loss = keypoint_loss(out['kps'], gt)               # any torch expression
+    loss.backward(); opt.step(); opt.zero_grad()
+    model.save_checkpoint('/path/model.ckpt-1000')     # HMMREngine / Tester load it unchanged
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+import torch
+from torch import nn
+from torch.autograd.function import once_differentiable
+
+from . import _lib
+from ._lib import lib, check, fptr, current_stream, ConvDesc
+from .nets import FAST_HEADS, GN_EPS, GN_GROUPS, PackedConv
+
+F32 = torch.float32
+
+
+def _vp(t, off=0):
+    return C.c_void_p(t.data_ptr() + off)
+
+
+def _round(x, m):
+    return (x + m - 1) // m * m
+
+
+def _tmap(t, rows, k_pad, eb):
+    m = (C.c_ubyte * 128)()
+    check(lib.hd_make_weight_tmap(_vp(t), rows, k_pad, 64, eb, C.cast(m, C.c_void_p)), 'hd_make_weight_tmap')
+    return m
+
+
+class DevicePackedConv(PackedConv):
+    """A PackedConv whose K-major head / remainder packs are written on the device from an fp32 weight tensor (hd_pack_weight),
+    so a training step never round-trips the weights through the host.
+
+    mode HD_PACK_FORWARD: the layer itself, fp16 packing (impl tc3h), exactly what PackedConv(tc='f16') holds; w_kn / post_shift point
+    at the parameter storage.  mode HD_PACK_BACKWARD_DATA: the transposed, tap-flipped layer whose conv is dX (TF32 packing, impl tc3)."""
+
+    def __init__(self, weight, KH, Cin, Cout, mode=_lib.HD_PACK_FORWARD, bias=None, post_relu=False, pad=0):
+        fwd = mode == _lib.HD_PACK_FORWARD
+        self.src, self.mode, self.src_shape = weight, mode, (KH, Cin, Cout)
+        self.KH, self.KW = KH, 1
+        self.Cin, self.Cout = (Cin, Cout) if fwd else (Cout, Cin)
+        self.K = self.K_pad = KH * self.Cin
+        self.stride, self.pad_t, self.pad_l = 1, pad, 0
+        self.device = weight.device
+        self.w_kn = weight
+        self.post_scale = None
+        self.post_shift = bias
+        self.post_relu = bool(post_relu)
+        self.gather = False
+        self.tc = 'f16' if fwd else 'tf32'
+        self.eb = 2 if fwd else 4
+        if self.K % (32 if self.eb == 4 else 64) != 0:
+            raise _lib.HDError('DevicePackedConv: K = %d does not fit the tensor-core packing' % self.K)
+        self.rows = _round(self.Cout, 64)
+        dt = torch.float16 if fwd else F32
+        self.w_nk_hi = torch.empty((self.rows, self.K), dtype=dt, device=self.device)
+        self.w_nk_lo = torch.empty((self.rows, self.K), dtype=dt, device=self.device)
+        self.tmap_hi = _tmap(self.w_nk_hi, self.rows, self.K, self.eb)
+        self.tmap_lo = _tmap(self.w_nk_lo, self.rows, self.K, self.eb)
+
+    def repack(self, stream):
+        KH, Cin, Cout = self.src_shape
+        check(lib.hd_pack_weight(fptr(self.src), KH, Cin, Cout, self.mode, self.eb, _vp(self.w_nk_hi), _vp(self.w_nk_lo), self.rows, self.K,
+                                 stream), 'hd_pack_weight')
+
+
+def _tf32_gemm(a, M, K, a_ld, b, out, out_ld, res=None, T=1, KH=1, pad=0, stream=None):
+    """out[M', Cout] = (implicit conv of) a . B on the 3xTF32 tensor-core kernel.  b: a DevicePackedConv (backward-data pack) or an
+    operand tuple (hi, lo, tmap_hi, tmap_lo, Cout) from _bt_operand.  T / KH / pad > 1: a KH x 1 conv over T of M = B clips."""
+    d = ConvDesc()
+    d.in_, d.in_ld = a.data_ptr(), a_ld
+    d.n_img, d.H, d.W, d.Cin = M, T, 1, K
+    d.Ho, d.Wo, d.KH, d.KW, d.stride, d.pad_t, d.pad_l = T, 1, KH, 1, 1, pad, 0
+    if isinstance(b, DevicePackedConv):
+        hi, lo, th, tl, Cout = b.w_nk_hi, b.w_nk_lo, b.tmap_hi, b.tmap_lo, b.Cout
+    else:
+        hi, lo, th, tl, Cout = b
+    d.w_kn = hi.data_ptr()
+    d.w_nk_hi, d.w_nk_lo = hi.data_ptr(), lo.data_ptr()
+    d.Cout, d.K_pad = Cout, KH * K
+    if res is not None:
+        d.res, d.res_ld, d.res_H, d.res_W, d.res_stride = res.data_ptr(), out_ld, T, 1, 1
+    d.out, d.out_ld = out.data_ptr(), out_ld
+    d.impl = _lib.HD_IMPL_TC_3XTF32
+    d.tmap_hi, d.tmap_lo = C.cast(th, C.c_void_p), C.cast(tl, C.c_void_p)
+    check(lib.hd_conv_gemm(C.byref(d), current_stream() if stream is None else stream), 'hd_conv_gemm (backward, 3xTF32)')
+
+
+def _bt_operand(pieces, cols, k_pad, st):
+    """B operand of a weight-gradient GEMM: the row blocks `pieces` = [(x, rows, ld)] of an upstream gradient stacked along K,
+    transposed and TF32-split into [roundup64(cols), k_pad] (zero past the real rows / columns)."""
+    rows = _round(cols, 64)
+    hi = torch.empty((rows, k_pad), dtype=F32, device=pieces[0][0].device)
+    lo = torch.empty_like(hi)
+    _stack_t(pieces, cols, k_pad, 1, hi, lo, rows, st)
+    return (hi, lo, _tmap(hi, rows, k_pad, 4), _tmap(lo, rows, k_pad, 4), cols), (hi, lo)
+
+
+def _stack_t(pieces, cols, k_pad, mode, hi, lo, out_rows, st):
+    off = 0
+    for i, (x, n, ld) in enumerate(pieces):
+        last = i == len(pieces) - 1
+        check(lib.hd_transpose_split(fptr(x), n, cols, ld, mode, _vp(hi, off * 4), _vp(lo, off * 4) if lo is not None else None, k_pad,
+                                     out_rows, (k_pad - off) if last else n, st), 'hd_transpose_split')
+        off += n
+
+
+def _xt(pieces, cols, k_pad, st):
+    """A operand of a weight-gradient GEMM for an FC layer: input rows stacked along K, transposed to [cols, k_pad] fp32."""
+    out = torch.empty((cols, k_pad), dtype=F32, device=pieces[0][0].device)
+    _stack_t(pieces, cols, k_pad, 0, out, None, cols, st)
+    return out
+
+
+def _col_sum(x, rows, cols, ld, out, st):
+    check(lib.hd_col_sum(fptr(x), rows, cols, ld, fptr(out), st), 'hd_col_sum')
+
+
+def _wgrad(xt, M, k_pad, g_pieces, cols, out, st):
+    """out[M, cols] = xt . (stacked g) : the weight gradient, 3xTF32."""
+    op, _keep = _bt_operand(g_pieces, cols, k_pad, st)
+    _tf32_gemm(xt, M, k_pad, k_pad, op, out, cols, stream=st)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------------
+# f_movie
+# ------------------------------------------------------------------------------------------------------------------------------------
+def fmovie_forward(model, x, save):
+    """az_fc2_groupnorm over x (B,T,C) with the kernels of nets.FMoviePlan; returns (out, saved) with saved = [(block input, conv1
+    output)] per block when `save`."""
+    B, T, Cc = x.shape
+    st = current_stream()
+    dev = x.device
+    fast = FAST_HEADS and T * (Cc // GN_GROUPS) <= 1280
+    if fast:
+        act = (torch.empty((B * T, Cc), dtype=torch.float16, device=dev), torch.empty((B * T, Cc), dtype=torch.float16, device=dev))
+    else:
+        gain, offset = torch.empty((B, Cc), dtype=F32, device=dev), torch.empty((B, Cc), dtype=F32, device=dev)
+    saved, cur = [], x
+    for blk in model.fm_blocks:
+        mid = torch.empty((B, T, Cc), dtype=F32, device=dev)
+        out = torch.empty((B, T, Cc), dtype=F32, device=dev)
+        for k, src, dst in ((1, cur, mid), (2, mid, out)):
+            g, b = blk['gn%d' % k]
+            conv = blk['conv%d' % k]
+            res = dict(res=cur, res_geom=(Cc, T, 1, 1)) if k == 2 else {}
+            if fast:
+                check(lib.hd_groupnorm_relu_split(fptr(src), fptr(g), fptr(b), _vp(act[0]), _vp(act[1]), B, T, Cc, GN_GROUPS, GN_EPS, st),
+                      'hd_groupnorm_relu_split')
+                conv.bind(None, B, T, 1, dst, inp_split=act, impl='auto', **res).run(st)
+            else:
+                check(lib.hd_groupnorm_stats(fptr(src), fptr(g), fptr(b), fptr(gain), fptr(offset), B, T, Cc, GN_GROUPS, GN_EPS, st),
+                      'hd_groupnorm_stats')
+                conv.bind(src, B, T, 1, dst, pre=(gain, offset, Cc, 1), impl='auto', **res).run(st)
+        if save:
+            saved.append((cur, mid))
+        cur = out
+    return cur, saved
+
+
+def fmovie_backward(model, saved, g):
+    """Gradients of f_movie: returns (dx, [per block: dgamma1, dbeta1, dW1, db1, dgamma2, dbeta2, dW2, db2])."""
+    st = current_stream()
+    B, T, Cc = g.shape
+    BT = B * T
+    kp = _round(BT, 32)
+    dev = g.device
+    xt = torch.empty((3 * Cc, kp), dtype=F32, device=dev)
+    gain, offset = torch.empty((B, Cc), dtype=F32, device=dev), torch.empty((B, Cc), dtype=F32, device=dev)
+    pg, pb = torch.empty((B, Cc), dtype=F32, device=dev), torch.empty((B, Cc), dtype=F32, device=dev)
+    dact = torch.empty((B, T, Cc), dtype=F32, device=dev)
+    grads = [None] * len(model.fm_blocks)
+    g = g.contiguous()
+    for i in range(len(model.fm_blocks) - 1, -1, -1):
+        blk = model.fm_blocks[i]
+        x, mid = saved[i]
+        gr = {}
+        dmid = torch.empty((B, T, Cc), dtype=F32, device=dev)
+        dx = torch.empty((B, T, Cc), dtype=F32, device=dev)
+        for k, src, gin, gout, addend in ((2, mid, g, dmid, None), (1, x, dmid, dx, g)):
+            gam, bet = blk['gn%d' % k]
+            # dW = im2col(relu(gn(src)))^T . gin, db = colsum(gin)
+            check(lib.hd_groupnorm_stats(fptr(src), fptr(gam), fptr(bet), fptr(gain), fptr(offset), B, T, Cc, GN_GROUPS, GN_EPS, st),
+                  'hd_groupnorm_stats')
+            check(lib.hd_im2col_t(fptr(src), B, T, Cc, 3, 1, fptr(gain), fptr(offset), 1, fptr(xt), kp, kp, st), 'hd_im2col_t')
+            dW = torch.empty((3, 1, Cc, Cc), dtype=F32, device=dev)
+            _wgrad(xt, 3 * Cc, kp, [(gin, BT, Cc)], Cc, dW, st)
+            db = torch.empty(Cc, dtype=F32, device=dev)
+            _col_sum(gin, BT, Cc, Cc, db, st)
+            # d relu(gn(src)) = conv(gin, W'); then the GroupNorm + ReLU backward (+ the block's residual gradient for gn1)
+            _tf32_gemm(gin, B, Cc, Cc, model.fm_bwd[i][k - 1], dact, Cc, T=T, KH=3, pad=1, stream=st)
+            check(lib.hd_groupnorm_relu_backward(fptr(src), fptr(gam), fptr(bet), fptr(dact), fptr(addend) if addend is not None else None,
+                                                 fptr(gout), fptr(pg), fptr(pb), B, T, Cc, GN_GROUPS, GN_EPS, 1, st),
+                  'hd_groupnorm_relu_backward')
+            dg, dbe = torch.empty(Cc, dtype=F32, device=dev), torch.empty(Cc, dtype=F32, device=dev)
+            _col_sum(pg, B, Cc, Cc, dg, st)
+            _col_sum(pb, B, Cc, Cc, dbe, st)
+            gr[k] = (dg, dbe, dW, db)
+        grads[i] = list(gr[1]) + list(gr[2])
+        g = dx
+    return g, grads
+
+
+# ------------------------------------------------------------------------------------------------------------------------------------
+# IEF heads
+# ------------------------------------------------------------------------------------------------------------------------------------
+def ief_head_forward(model, head, phi_split, N, start, start_ld, out, out_ld, st):
+    """hmr_ief for one head with the kernels of IEFPlan's fast path.  Returns what the backward needs besides the head's start:
+    (h1 [3,N,1024], h2 [3,N,1024], the outputs of stages 0 and 1 [N,d])."""
+    dev = start.device
+    d = head['d']
+    P = torch.empty((N, 1024), dtype=F32, device=dev)
+    h1 = torch.empty((3, N, 1024), dtype=F32, device=dev)
+    h2 = torch.empty((3, N, 1024), dtype=F32, device=dev)
+    h1s = (torch.empty((N, 1024), dtype=torch.float16, device=dev), torch.empty((N, 1024), dtype=torch.float16, device=dev))
+    head['fc1_phi'].bind(None, N, 1, 1, P, inp_split=phi_split, impl='auto').run(st)
+    mids = [torch.empty((N, d), dtype=F32, device=dev) for _ in range(2)]
+    ins = [(start, start_ld), (mids[0], d), (mids[1], d)]
+    for s in range(3):
+        prev, pld = ins[s]
+        check(lib.hd_ief_fc1_theta(fptr(P), fptr(prev), pld, fptr(head['W1t']), d, 1024, _vp(h1s[0]), _vp(h1s[1]), fptr(h1[s]), N, st),
+              'hd_ief_fc1_theta')
+        head['fc2'].bind(None, N, 1, 1, h2[s], inp_split=h1s, impl='auto').run(st)
+        dst, dld = (mids[s], d) if s < 2 else (out, out_ld)
+        check(lib.hd_ief_fc3(fptr(h2[s]), fptr(head['W3']), fptr(head['b3']), fptr(prev), pld, fptr(dst), dld, N, 1024, d, st), 'hd_ief_fc3')
+    return h1, h2, mids[0], mids[1]
+
+
+def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st):
+    """Backward of one hmr_ief head.  saved = (h1, h2, start, start_ld, stage-0 output, stage-1 output); g: gradient of the head's
+    output (rows of d at stride g_ld).  Accumulates dL/dphi into `dphi`
+    (None: written).  Returns (dstart [N, d], [dW1, db1, dW2, db2, dW3, db3], dphi)."""
+    dev = phi.device
+    d = head['d']
+    h1, h2, start, start_ld, mid0, mid1 = saved
+    ins = [(start, start_ld), (mid0, d), (mid1, d)]
+    G = torch.empty((3, N, d), dtype=F32, device=dev)
+    DP2 = torch.empty((3, N, 1024), dtype=F32, device=dev)
+    DP1 = torch.empty((3, N, 1024), dtype=F32, device=dev)
+    dstart = torch.empty((N, d), dtype=F32, device=dev)
+    for s in range(2, -1, -1):
+        gs, gld = (g, g_ld) if s == 2 else (G[s], d)
+        if s == 2:
+            G[2].copy_(torch.as_strided(g, (N, d), (g_ld, 1)))
+        # dpre2 = (g . W3^T) * (h2 > 0);  dpre1 = (dpre2 . W2^T) * (h1 > 0);  dprev = g + dpre1 . W1theta^T
+        check(lib.hd_fc_small_dgrad(fptr(gs), gld, fptr(head['W3t']), 1024, d, fptr(h2[s]), fptr(DP2[s]), N, st), 'hd_fc_small_dgrad')
+        _tf32_gemm(DP2[s], N, 1024, 1024, head['fc2_bwd'], DP1[s], 1024, stream=st)
+        check(lib.hd_relu_backward(fptr(h1[s]), fptr(DP1[s]), fptr(DP1[s]), N * 1024, st), 'hd_relu_backward')
+        dst = G[s - 1] if s > 0 else dstart
+        check(lib.hd_ief_fc3(fptr(DP1[s]), fptr(head['W1tT']), fptr(model._zeros), fptr(gs), gld, fptr(dst), d, N, 1024, d, st),
+              'hd_ief_fc3')
+    kp3, kp1 = _round(3 * N, 32), _round(N, 32)
+    W1, W2, W3 = (torch.empty(p.shape, dtype=F32, device=dev) for p in (head['p'][0], head['p'][2], head['p'][4]))
+    b1, b2, b3 = (torch.empty(p.shape, dtype=F32, device=dev) for p in (head['p'][1], head['p'][3], head['p'][5]))
+    # dP = sum over the stages (fixed order), then the phi part of fc1
+    dP = torch.empty((N, 1024), dtype=F32, device=dev)
+    check(lib.hd_add_strided(fptr(DP1[0]), 1024, fptr(DP1[1]), 1024, fptr(dP), 1024, N, 1024, st), 'hd_add_strided')
+    check(lib.hd_add_strided(fptr(dP), 1024, fptr(DP1[2]), 1024, fptr(dP), 1024, N, 1024, st), 'hd_add_strided')
+    _col_sum(dP, N, 1024, 1024, b1, st)
+    _col_sum(DP2, 3 * N, 1024, 1024, b2, st)
+    _col_sum(G, 3 * N, d, d, b3, st)
+    feat = head['feat']
+    _wgrad(_xt([(phi, N, feat)], feat, kp1, st), feat, kp1, [(dP, N, 1024)], 1024, W1, st)
+    _wgrad(_xt([(t, N, ld) for t, ld in ins], d, kp3, st), d, kp3, [(DP1.view(3 * N, 1024), 3 * N, 1024)], 1024, W1[feat:], st)
+    _wgrad(_xt([(h1.view(3 * N, 1024), 3 * N, 1024)], 1024, kp3, st), 1024, kp3, [(DP2.view(3 * N, 1024), 3 * N, 1024)], 1024, W2, st)
+    _wgrad(_xt([(h2.view(3 * N, 1024), 3 * N, 1024)], 1024, kp3, st), 1024, kp3, [(G.view(3 * N, d), 3 * N, d)], d, W3, st)
+    out = torch.empty((N, feat), dtype=F32, device=dev) if dphi is None else dphi
+    _tf32_gemm(dP, N, 1024, 1024, head['fc1_bwd'], out, feat, res=dphi, stream=st)
+    return dstart, [W1, b1, W2, b2, W3, b3], out
+
+
+# ------------------------------------------------------------------------------------------------------------------------------------
+# fc2_res
+# ------------------------------------------------------------------------------------------------------------------------------------
+def hal_forward(model, x):
+    N = x.shape[0]
+    st = current_stream()
+    h1, h2, out = (torch.empty((N, 2048), dtype=F32, device=x.device) for _ in range(3))
+    L = model.hal
+    L['fc1'].bind(x, N, 1, 1, h1, impl='auto').run(st)
+    L['fc2'].bind(h1, N, 1, 1, h2, impl='auto').run(st)
+    L['fc3'].bind(h2, N, 1, 1, out, res=x, res_geom=(2048, 1, 1, 1), impl='auto').run(st)
+    return out, (h1, h2)
+
+
+def hal_backward(model, x, h1, h2, g):
+    N = x.shape[0]
+    st = current_stream()
+    dev = x.device
+    kp = _round(N, 32)
+    L = model.hal
+    grads = []
+    dh2, dh1, dx = (torch.empty((N, 2048), dtype=F32, device=dev) for _ in range(3))
+    for inp, gin, name in ((h2, g, 'fc3'), (h1, dh2, 'fc2'), (x, dh1, 'fc1')):
+        W, b = torch.empty((2048, 2048), dtype=F32, device=dev), torch.empty(2048, dtype=F32, device=dev)
+        _wgrad(_xt([(inp, N, 2048)], 2048, kp, st), 2048, kp, [(gin, N, 2048)], 2048, W, st)
+        _col_sum(gin, N, 2048, 2048, b, st)
+        grads = [W, b] + grads
+        if name == 'fc3':
+            _tf32_gemm(g, N, 2048, 2048, L['fc3_bwd'], dh2, 2048, stream=st)
+            check(lib.hd_relu_backward(fptr(h2), fptr(dh2), fptr(dh2), N * 2048, st), 'hd_relu_backward')
+        elif name == 'fc2':
+            _tf32_gemm(dh2, N, 2048, 2048, L['fc2_bwd'], dh1, 2048, stream=st)
+            check(lib.hd_relu_backward(fptr(h1), fptr(dh1), fptr(dh1), N * 2048, st), 'hd_relu_backward')
+        else:
+            _tf32_gemm(dh1, N, 2048, 2048, L['fc1_bwd'], dx, 2048, res=g, stream=st)
+    return dx, grads
+
+
+# ------------------------------------------------------------------------------------------------------------------------------------
+# autograd
+# ------------------------------------------------------------------------------------------------------------------------------------
+class FMovieFunction(torch.autograd.Function):
+    """phi (B,T,C) -> f_movie(phi); differentiable w.r.t. phi and every block's gamma / beta / weights / biases."""
+
+    @staticmethod
+    def forward(ctx, model, x, *params):
+        out, saved = fmovie_forward(model, x, True)
+        ctx.model = model
+        ctx.save_for_backward(*[t for pair in saved for t in pair])
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        ctx.model._ensure_bwd()
+        t = ctx.saved_tensors
+        dx, grads = fmovie_backward(ctx.model, [(t[2 * i], t[2 * i + 1]) for i in range(len(t) // 2)], g)
+        return (None, dx) + tuple(t for blk in grads for t in blk)
+
+
+class RegressFunction(torch.autograd.Function):
+    """call_hmr_ief as Tester wires it: phi (N,2048), start (N,85) or the tiled mean_param (1,85) -> (theta (N,85), deltas (N,85)...).
+    The delta heads start from theta's pose and carry its beta, so their gradients flow back into the main head; a tiled start's
+    gradient is its column sum."""
+
+    @staticmethod
+    def forward(ctx, model, keys, tiled, phi, start, *params):
+        N = phi.shape[0]
+        st = current_stream()
+        dev = phi.device
+        phi_split = (torch.empty((N, 2048), dtype=torch.float16, device=dev), torch.empty((N, 2048), dtype=torch.float16, device=dev))
+        check(lib.hd_split_f16(fptr(phi), _vp(phi_split[0]), _vp(phi_split[1]), phi.numel(), st), 'hd_split_f16')
+        s0 = start.expand(N, 85).contiguous() if tiled else start
+        theta = torch.empty((N, 85), dtype=F32, device=dev)
+        saved = list(ief_head_forward(model, model.ief['main'], phi_split, N, s0, 85, theta, 85, st))
+        outs = [theta]
+        for k in keys:
+            o = torch.empty((N, 85), dtype=F32, device=dev)
+            check(lib.hd_ief_delta_init(fptr(theta), fptr(o), 85, N, st), 'hd_ief_delta_init')
+            pose = torch.as_strided(theta, (N, 72), (85, 1), theta.storage_offset() + 3)
+            saved += ief_head_forward(model, model.ief[k], phi_split, N, pose, 85, torch.as_strided(o, (N, 72), (85, 1), o.storage_offset() + 3),
+                                      85, st)
+            outs.append(o)
+        # Everything the backward reads goes through save_for_backward (theta, an output, included): no tensor or view of one is held on
+        # ctx, so an unused graph is freed with its outputs and retain_graph works.  The delta heads' start is theta's pose, rebuilt there.
+        ctx.model, ctx.keys, ctx.tiled = model, keys, tiled
+        ctx.save_for_backward(phi, s0, theta, *saved)
+        ctx.set_materialize_grads(False)
+        return tuple(outs)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dtheta, *ddeltas):
+        model, keys = ctx.model, ctx.keys
+        model._ensure_bwd()
+        t = ctx.saved_tensors
+        phi, s0, theta = t[:3]
+        N = phi.shape[0]
+        pose = torch.as_strided(theta, (N, 72), (85, 1), theta.storage_offset() + 3)
+        heads = [t[3 + 4 * j:7 + 4 * j] for j in range(1 + len(keys))]
+        state = [(h1, h2, s0 if j == 0 else pose, 85, m0, m1) for j, (h1, h2, m0, m1) in enumerate(heads)]
+        st = current_stream()
+        dev = phi.device
+        # gradient reaching the main head's output: its own upstream + each delta head's start (pose) and carried beta, ascending dt
+        gm = torch.zeros((N, 85), dtype=F32, device=dev) if dtheta is None else dtheta.contiguous().clone()
+        dphi = None
+        head_grads = {}
+        for i, k in enumerate(keys):
+            dd = ddeltas[i]
+            if dd is None:
+                continue
+            dd = dd.contiguous()
+            ds, hg, dphi = ief_head_backward(model, model.ief[k], phi, N, state[1 + i], torch.as_strided(dd, (N, 72), (85, 1), dd.storage_offset() + 3),
+                                             85, dphi, st)
+            head_grads[k] = hg
+            check(lib.hd_add_strided(fptr(gm[:, 3:]), 85, fptr(ds), 72, fptr(gm[:, 3:]), 85, N, 72, st), 'hd_add_strided')
+            check(lib.hd_add_strided(fptr(gm[:, 75:]), 85, fptr(dd[:, 75:]), 85, fptr(gm[:, 75:]), 85, N, 10, st), 'hd_add_strided')
+        dstart, hg, dphi = ief_head_backward(model, model.ief['main'], phi, N, state[0], gm, 85, dphi, st)
+        head_grads['main'] = hg
+        if ctx.tiled:
+            ds = torch.empty((1, 85), dtype=F32, device=dev)
+            _col_sum(dstart, N, 85, 85, ds, st)
+            dstart = ds
+        flat = []
+        for k in ['main'] + list(keys):
+            flat += head_grads.get(k, [None] * 6)
+        return (None, None, None, dphi, dstart) + tuple(flat)
+
+
+class HalFunction(torch.autograd.Function):
+    """fc2_res: x (N,2048) -> x + fc3(relu(fc2(relu(fc1(x)))))."""
+
+    @staticmethod
+    def forward(ctx, model, x, *params):
+        out, (h1, h2) = hal_forward(model, x)
+        ctx.model = model
+        ctx.save_for_backward(x, h1, h2)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        ctx.model._ensure_bwd()
+        x, h1, h2 = ctx.saved_tensors
+        dx, grads = hal_backward(ctx.model, x, h1, h2, g.contiguous())
+        return (None, dx) + tuple(grads)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------------
+# the model
+# ------------------------------------------------------------------------------------------------------------------------------------
+def fmovie_names(i):
+    name = 'block_%d' % i
+    return ['AZ_FC_block_preact_gn1%s/gamma' % name, 'AZ_FC_block_preact_gn1%s/beta' % name,
+            'AZ_FC_block2_conv1%s/weights' % name, 'AZ_FC_block2_conv1%s/biases' % name,
+            'AZ_FC_block_preact_gn2%s/gamma' % name, 'AZ_FC_block_preact_gn2%s/beta' % name,
+            'AZ_FC_block2_conv2%s/weights' % name, 'AZ_FC_block2_conv2%s/biases' % name]
+
+
+def ief_scope(dt, scope='single_view_ief'):
+    return scope if dt == 0 else scope + ('_future%d' % dt if dt > 0 else '_past%d' % abs(dt))
+
+
+def ief_names(dt):
+    q = ief_scope(dt) + '/3D_module'
+    return [q + '/fc%d/%s' % (i, k) for i in (1, 2, 3) for k in ('weights', 'biases')]
+
+
+HAL_NAMES = ['fc2_res/fc%d/%s' % (i, k) for i in (1, 2, 3) for k in ('weights', 'biases')]
+
+
+def trainable_names(w, num_conv_layers=3, delta_t_values=(-5, 5)):
+    """TF variable names TemporalModel holds for a weight dict: exactly the f_movie / IEF / mean_param / fc2_res keys HMMREngine reads."""
+    names = []
+    if any(k.startswith('AZ_FC_block2_conv1') for k in w):
+        for i in range(num_conv_layers):
+            names += fmovie_names(i)
+    for dt in [0] + sorted(int(d) for d in delta_t_values if int(d) != 0):
+        names += ief_names(dt)
+    names.append('mean_param')
+    if 'fc2_res/fc1/weights' in w:
+        names += HAL_NAMES
+    return names
+
+
+class TemporalModel(nn.Module):
+    """The trainable part of HMMR (f_movie, the IEF heads, mean_param, fc2_res) as fp32 parameters on one CUDA device.
+
+    Parameters are addressable by their TF variable names (`model.param('single_view_ief/3D_module/fc2/weights')`); `parameters()`
+    feeds any torch optimizer.  A parameter changed in place (optimizer.step(), copy_) is repacked on the device before the next
+    forward (detected by its version counter).  Under torch.no_grad(), or when nothing requires grad, the methods run the inference
+    kernels and build no graph.
+
+    The forward follows HMMREngine's default configuration (impl 'auto'): f_movie takes the same branch as FMoviePlan (fused GroupNorm
+    + split for T*64 <= 1280 with HD_FAST_HEADS on, GroupNorm statistics + conv prologue otherwise), so it is bit-identical to the engine
+    at every T.  The IEF heads always run IEFPlan's fast-head kernels, whose saved h1 / h2 the backward reads; the HD_FAST_HEADS=0 A/B
+    switch of the inference plans (generic IEF descriptors) does not apply here, and with it set the engine's IEF outputs differ from
+    this model's in the last bits."""
+
+    def __init__(self, weights, config=None, device=None):
+        super().__init__()
+        from .config import HMMRConfig
+        from .engine import load_weights
+        if not torch.cuda.is_available():
+            raise _lib.HDError('TemporalModel needs a CUDA device: the hot path has no CPU fallback')
+        self.config = config or HMMRConfig()
+        self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+        w = load_weights(weights)
+        self._source = w                                       # frozen variables (the ResNet) for tf_variables / save_checkpoint
+        self.num_conv_layers = int(self.config.num_conv_layers)
+        self.delta_keys = sorted(int(d) for d in self.config.delta_t_values if int(d) != 0)
+        self.names = trainable_names(w, self.num_conv_layers, self.delta_keys)
+        self._params = nn.ParameterDict()
+        for n in self.names:
+            a = np.asarray(w[n], np.float32)
+            if n == 'mean_param':
+                a = a.reshape(1, 85)
+            self._params[n] = nn.Parameter(torch.from_numpy(np.ascontiguousarray(a)).to(self.device))
+        with torch.cuda.device(self.device):
+            self._build()
+        self._seen = {}
+        self._bwd_seen = {}
+
+    # ---------------------------------------------------------------- packing
+    def param(self, name):
+        return self._params[name]
+
+    def _build(self):
+        P = self.param
+        self.fm_blocks, self.fm_bwd, self._fwd_packs, self._bwd_packs = [], [], [], []
+        self.has_fmovie = 'AZ_FC_block2_conv1block_0/weights' in self.names
+        Cc = 2048
+        if self.has_fmovie:
+            for i in range(self.num_conv_layers):
+                n = fmovie_names(i)
+                blk = {'gn1': (P(n[0]).data, P(n[1]).data), 'gn2': (P(n[4]).data, P(n[5]).data)}
+                bwd = []
+                for k, wn, bn in ((1, n[2], n[3]), (2, n[6], n[7])):
+                    Cc = P(wn).shape[2]
+                    blk['conv%d' % k] = DevicePackedConv(P(wn).data, 3, Cc, Cc, bias=P(bn).data, pad=1)
+                    bwd.append(DevicePackedConv(P(wn).data, 3, Cc, Cc, mode=_lib.HD_PACK_BACKWARD_DATA, pad=1))
+                    self._fwd_packs.append((wn, blk['conv%d' % k]))
+                    self._bwd_packs.append((wn, bwd[-1]))
+                self.fm_blocks.append(blk)
+                self.fm_bwd.append(bwd)
+        self.ief = {}
+        for dt in [0] + self.delta_keys:
+            n = ief_names(dt)
+            W1, b1, W2, b2, W3, b3 = (P(x).data for x in n)
+            d = W3.shape[1]
+            feat = W1.shape[0] - d
+            h = {'d': d, 'feat': feat, 'p': [P(x) for x in n], 'W1t': W1[feat:], 'W3': W3, 'b3': b3,
+                 'fc1_phi': DevicePackedConv(W1, 1, feat, 1024, bias=b1),
+                 'fc1_bwd': DevicePackedConv(W1, 1, feat, 1024, mode=_lib.HD_PACK_BACKWARD_DATA),
+                 'fc2': DevicePackedConv(W2, 1, 1024, 1024, bias=b2, post_relu=True),
+                 'fc2_bwd': DevicePackedConv(W2, 1, 1024, 1024, mode=_lib.HD_PACK_BACKWARD_DATA),
+                 'W3t': torch.empty((d, 1024), dtype=F32, device=self.device),       # fc3^T  (input gradient of fc3)
+                 'W1tT': torch.empty((1024, d), dtype=F32, device=self.device)}      # fc1's theta rows, transposed
+            self._fwd_packs += [(n[0], h['fc1_phi']), (n[2], h['fc2'])]
+            self._bwd_packs += [(n[0], h['fc1_bwd']), (n[2], h['fc2_bwd']), (n[4], ('W3t', h)), (n[0], ('W1tT', h))]
+            self.ief['main' if dt == 0 else dt] = h
+        self._zeros = torch.zeros(96, dtype=F32, device=self.device)
+        self.hal = None
+        if 'fc2_res/fc1/weights' in self.names:
+            self.hal = {}
+            for i in (1, 2, 3):
+                wn, bn = HAL_NAMES[2 * i - 2], HAL_NAMES[2 * i - 1]
+                self.hal['fc%d' % i] = DevicePackedConv(P(wn).data, 1, 2048, 2048, bias=P(bn).data, post_relu=i < 3)
+                self.hal['fc%d_bwd' % i] = DevicePackedConv(P(wn).data, 1, 2048, 2048, mode=_lib.HD_PACK_BACKWARD_DATA)
+                self._fwd_packs.append((wn, self.hal['fc%d' % i]))
+                self._bwd_packs.append((wn, self.hal['fc%d_bwd' % i]))
+
+    def _repack(self, packs, seen):
+        st = current_stream()
+        stale = {n for n, _ in packs if seen.get(n) != self.param(n)._version}
+        for n, pk in packs:
+            if n not in stale:
+                continue
+            if isinstance(pk, tuple):
+                which, h = pk
+                src = h['W3'] if which == 'W3t' else h['W1t']
+                dst = h[which]
+                check(lib.hd_transpose_split(fptr(src), src.shape[0], src.shape[1], src.shape[1], 0, _vp(dst), None, dst.shape[1],
+                                             dst.shape[0], dst.shape[1], st), 'hd_transpose_split')
+            else:
+                pk.repack(st)
+        for n in stale:
+            seen[n] = self.param(n)._version
+        return len(stale)
+
+    def sync_packs(self):
+        """Repack every forward weight whose parameter changed since it was last packed (called by each forward).  Returns the count."""
+        return self._repack(self._fwd_packs, self._seen)
+
+    def _ensure_bwd(self):
+        return self._repack(self._bwd_packs, self._bwd_seen)
+
+    # ---------------------------------------------------------------- forward API
+    def _check_input(self, x, name, last=2048):
+        if not isinstance(x, torch.Tensor) or not x.is_cuda:
+            raise _lib.HDError('%s: a CUDA tensor is required (no CPU fallback exists)' % name)
+        if x.dtype != F32 or x.shape[-1] != last:
+            raise _lib.HDError('%s: expected float32 [..., %d], got %s %s' % (name, last, x.dtype, tuple(x.shape)))
+        if x.device != self.device:
+            raise _lib.HDError('%s: tensor is on %s, the model on %s' % (name, x.device, self.device))
+
+    def _grad_on(self, x, names):
+        return torch.is_grad_enabled() and (x.requires_grad or any(self.param(n).requires_grad for n in names))
+
+    def temporal_encode(self, phi):
+        """az_fc2_groupnorm ("f_movie"): (B,T,2048) -> (B,T,2048)."""
+        self._check_input(phi, 'temporal_encode')
+        if not self.has_fmovie:
+            raise _lib.HDError('no f_movie weights were loaded')
+        self.sync_packs()
+        phi = phi.contiguous()
+        names = [n for i in range(self.num_conv_layers) for n in fmovie_names(i)]
+        if self._grad_on(phi, names):
+            return FMovieFunction.apply(self, phi, *[self.param(n) for n in names])
+        with torch.no_grad():
+            return fmovie_forward(self, phi.detach(), False)[0]
+
+    def hallucinate(self, phi):
+        """fc2_res: (B,T,2048) -> (B,T,2048)   (pred_mode='hal')."""
+        self._check_input(phi, 'hallucinate')
+        if self.hal is None:
+            raise _lib.HDError('no fc2_res weights were loaded')
+        self.sync_packs()
+        x = phi.contiguous().reshape(-1, 2048)
+        if self._grad_on(x, HAL_NAMES):
+            return HalFunction.apply(self, x, *[self.param(n) for n in HAL_NAMES]).view(phi.shape)
+        with torch.no_grad():
+            return hal_forward(self, x.detach())[0].view(phi.shape)
+
+    def regress(self, feats, omega_start=None, delta_keys=None):
+        """call_hmr_ief: feats (N,2048) -> (omega (N,85), {dt: (N,85)}).  Starts from mean_param (tiled) unless omega_start (N,85) is
+        given; the delta heads start from the main prediction (use_delta_from_pred=True, use_optcam=True, as Tester wires them)."""
+        self._check_input(feats, 'regress')
+        keys = tuple(self.delta_keys) if delta_keys is None else tuple(sorted(int(k) for k in delta_keys if int(k) != 0))
+        for k in keys:
+            if k not in self.ief:
+                raise _lib.HDError('no IEF head for delta_t %d' % k)
+        self.sync_packs()
+        feats = feats.contiguous().reshape(-1, 2048)
+        tiled = omega_start is None
+        start = self.param('mean_param') if tiled else omega_start
+        if not tiled:
+            self._check_input(start, 'regress(omega_start)', 85)
+            start = start.contiguous()
+        names = [n for dt in (0,) + keys for n in ief_names(dt)]
+        params = [self.param(n) for n in names]
+        if self._grad_on(feats, names + ['mean_param']) or start.requires_grad and torch.is_grad_enabled():
+            outs = RegressFunction.apply(self, keys, tiled, feats, start, *params)
+        else:
+            with torch.no_grad():
+                outs = RegressFunction.forward(_NoCtx(), self, keys, tiled, feats.detach(), start.detach(), *params)
+        return outs[0], {k: outs[1 + i] for i, k in enumerate(keys)}
+
+    def predict_from_features(self, phi, smpl, single_frame=False):
+        """Tester's fetch dict (tester.py:217-255) from features phi (B,T,2048) through f_movie (or fc2_res with pred_mode 'hal'), the IEF
+        heads and the differentiable SMPL `smpl` (src.tf_smpl.batch_smpl.SMPL): cams, joints, kps, poses, shapes, verts, omegas and
+        their *_delta stackings [B,T,D,...]; the delta heads' cameras are the main prediction's (tester.py:210-213)."""
+        from src.tf_smpl.projection import batch_orth_proj_idrot
+        B, T = phi.shape[0], phi.shape[1]
+        N = B * T
+        if single_frame:
+            strips = phi
+            keys = ()
+        else:
+            strips = self.temporal_encode(phi) if self.config.pred_mode == 'pred' else self.hallucinate(phi)
+            keys = tuple(self.delta_keys)
+        omega, deltas = self.regress(strips.reshape(N, 2048), delta_keys=keys)
+        cams = omega[:, :3]
+
+        def smpl_out(om, cam):
+            verts, joints, Rs = smpl(om[:, 75:85], om[:, 3:75], get_skin=True)
+            kps = batch_orth_proj_idrot(joints, cam)
+            return {'cams': cam, 'joints': joints, 'kps': kps, 'poses': Rs, 'shapes': om[:, 75:85], 'verts': verts, 'omegas': om}
+        o0 = smpl_out(omega, cams)
+        out = {k: v.reshape((B, T) + tuple(v.shape[1:])) for k, v in o0.items()}
+        if keys:
+            per = [smpl_out(deltas[k], cams) for k in keys]
+            for k in o0:
+                out[k + '_delta'] = torch.stack([p[k] for p in per], 1).reshape((B, T, len(keys)) + tuple(per[0][k].shape[1:]))
+        out['_movie_strips'] = strips
+        return out
+
+    def relu_masks(self, phi=None, feats=None, hal=None, omega_start=None, delta_keys=None):
+        """The ReLU masks (pre-activation > 0) of the GPU forward, as CPU bool tensors keyed like oracle/nets_grad_ref's sites: f_movie
+        over phi (B,T,2048) ('fm<i>.gn1' / '.gn2', [B,T,1,C]), the IEF heads over feats (N,2048) ('main.s<k>.fc1', 'd<dt>.s<k>.fc2', ...)
+        and fc2_res over hal (N,2048) ('hal.fc1' / '.fc2').  An inspection aid for comparing against a float64 reference at near-tie
+        sites; runs its own forward."""
+        out = {}
+        st = current_stream()
+        with torch.no_grad():
+            self.sync_packs()
+            if phi is not None:
+                B, T, Cc = phi.shape
+                _, saved = fmovie_forward(self, phi.contiguous(), True)
+                gain, offset = torch.empty((B, Cc), dtype=F32, device=self.device), torch.empty((B, Cc), dtype=F32, device=self.device)
+                a = torch.empty((Cc, B * T), dtype=F32, device=self.device)
+                for i, (x, mid) in enumerate(saved):
+                    for k, src in ((1, x), (2, mid)):
+                        g, b = self.fm_blocks[i]['gn%d' % k]
+                        check(lib.hd_groupnorm_stats(fptr(src), fptr(g), fptr(b), fptr(gain), fptr(offset), B, T, Cc, GN_GROUPS, GN_EPS, st),
+                              'hd_groupnorm_stats')
+                        check(lib.hd_im2col_t(fptr(src), B, T, Cc, 1, 0, fptr(gain), fptr(offset), 1, fptr(a), B * T, B * T, st), 'hd_im2col_t')
+                        out['fm%d.gn%d' % (i, k)] = (a.t() > 0).reshape(B, T, 1, Cc).cpu()
+            if feats is not None:
+                keys = tuple(self.delta_keys) if delta_keys is None else tuple(sorted(int(k) for k in delta_keys if int(k) != 0))
+                ctx = _NoCtx()
+                tiled = omega_start is None
+                start = self.param('mean_param') if tiled else omega_start.contiguous()
+                RegressFunction.forward(ctx, self, keys, tiled, feats.contiguous(), start.detach(),
+                                        *[self.param(n) for dt in (0,) + keys for n in ief_names(dt)])
+                t = ctx.saved_tensors
+                for j, name in enumerate(['main'] + ['d%d' % k for k in keys]):
+                    h1, h2 = t[3 + 4 * j], t[4 + 4 * j]
+                    for s in range(3):
+                        out['%s.s%d.fc1' % (name, s)] = (h1[s] > 0).cpu()
+                        out['%s.s%d.fc2' % (name, s)] = (h2[s] > 0).cpu()
+            if hal is not None:
+                _, (h1, h2) = hal_forward(self, hal.contiguous())
+                out['hal.fc1'], out['hal.fc2'] = (h1 > 0).cpu(), (h2 > 0).cpu()
+        return out
+
+    # ---------------------------------------------------------------- export
+    def tf_variables(self):
+        """Every variable of the checkpoint the model came from, the trainable ones replaced by their current values: {name: ndarray}."""
+        out = {k: np.asarray(v) for k, v in self._source.items()}
+        for n in self.names:
+            a = self.param(n).detach().cpu().numpy()
+            out[n] = a.reshape(np.shape(self._source[n])).astype(np.asarray(self._source[n]).dtype)
+        return out
+
+    def save_checkpoint(self, prefix):
+        """Write tf_variables() as a TensorFlow V2 checkpoint (`prefix`.index / .data-00000-of-00001) that HMMREngine and Tester load."""
+        from .tf_checkpoint import save_checkpoint
+        save_checkpoint(prefix, self.tf_variables())
+        return prefix
+
+
+class _NoCtx(object):
+    """Stand-in ctx for running an autograd Function's forward without recording a graph."""
+
+    def save_for_backward(self, *a):
+        self.saved_tensors = a
+
+    def set_materialize_grads(self, v):
+        pass

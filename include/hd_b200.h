@@ -327,6 +327,51 @@ int hd_global_rigid_backward(const float *Rs, const float *Js, const int *parent
  * dX_xy = s dout, ds = sum_p (xy + t) . dout_p, dt = s sum_p dout_p. */
 int hd_orth_proj_backward(const float *X, const float *cam, const float *dout, float *dX, float *dcam, int N, int P, void *stream);
 
+/* ---- Backward of the trainable layers: f_movie, the IEF heads and fc2_res (csrc/net_grad.cu) ----
+ * The GEMMs of the backward run on hd_conv_gemm in its 3xTF32 mode (gradients carry an arbitrary scale, so they never go through the
+ * fp16 split with its +-65504 clamp); the entries below supply its operands and the non-GEMM parts.  For a KH x 1 SAME conv over T
+ * (f_movie, KH = 3, pad 1) or an FC layer (KH = 1, pad 0) with input x [B*T, Cin], weight W [KH, Cin, Cout] (TF HWIO) and output
+ * gradient dY [B*T, Cout]:
+ *   dX = conv(dY, W'), W'[k', co, ci] = W[KH-1-k', ci, co]        hd_conv_gemm (3xTF32, in = dY) over hd_pack_weight(BACKWARD_DATA)
+ *   dW = Xcol^T . dY   (M = KH*Cin, N = Cout, K = B*T)            hd_conv_gemm (3xTF32) with in = hd_im2col_t(x) as [KH*Cin, K_pad]
+ *                                                                 pixels and the B operand hd_transpose_split(dY, tf32) [Cout_pad, K_pad]
+ *   db = column sums of dY                                        hd_col_sum
+ * Deterministic: no floating-point atomics, every reduction in a fixed order; an input gradient's row depends only on that row. */
+enum { HD_PACK_FORWARD = 0, HD_PACK_BACKWARD_DATA = 1 };
+/* Device-side weight packing into the K-major [rows, k_pad] head / remainder layout of hd_conv_gemm's B operand (TMA maps from
+ * hd_make_weight_tmap).  w: fp32 [KH, Cin, Cout] (conv HWIO with KW = 1, or FC [in, out] with KH = 1).  elem_bytes 2 = fp16 head /
+ * 2^11-scaled remainder (impl 3), 4 = TF32 head / remainder in fp32 storage (impl 1).
+ *   HD_PACK_FORWARD:       dst[co, kh*Cin + ci] = W[kh, ci, co]  -- byte for byte nets.PackedConv + f16_split / tf32_split;
+ *   HD_PACK_BACKWARD_DATA: dst[ci, k'*Cout + co] = W[KH-1-k', ci, co]  (FC: W^T).
+ * Rows / columns past the matrix are zero.  rows % 64 == 0, k_pad % 32 (tf32) / % 64 (fp16) == 0, hi / lo 16-byte aligned. */
+int hd_pack_weight(const float *w, int KH, int Cin, int Cout, int mode, int elem_bytes, void *hi, void *lo, int rows, int k_pad, void *stream);
+/* Transpose with optional split: hi[r*out_ld + k] (and lo) = split(x[k*ld + r]) for r < cols, k < rows; 0 for r in [cols, out_rows) or
+ * k in [rows, out_cols).  mode 0 = plain fp32 (lo NULL), 1 = TF32 head / remainder, 2 = fp16 head / 2^11-scaled remainder.  Used for
+ * the dY^T operand of a weight-gradient GEMM (mode 1; pass column offsets in hi / lo to stack several products along K) and for the
+ * transposed inputs of FC weight gradients (mode 0). */
+int hd_transpose_split(const float *x, long long rows, int cols, long long ld, int mode, void *hi, void *lo, long long out_ld, int out_rows,
+                       long long out_cols, void *stream);
+/* Transposing im2col of x [B, T, C] for a KH x 1 conv over T with `pad` leading zero taps:
+ *   out[(kh*C + c)*out_ld + b*T + t] = a[b, t + kh - pad, c]  (0 outside the clip), columns [B*T, out_cols) = 0,
+ *   a = x, or with gain / offset [B, C] (hd_groupnorm_stats) a = x*gain + offset, then ReLU when relu != 0. */
+int hd_im2col_t(const float *x, int B, int T, int C, int KH, int pad, const float *gain, const float *offset, int relu, float *out,
+                long long out_ld, long long out_cols, void *stream);
+/* GroupNorm (+ ReLU) backward (tf.contrib.layers.group_norm, A7).  Recomputes mean / rstd per (clip, group) with the arithmetic of
+ * hd_groupnorm_stats; with z = x*gain + offset the forward's pre-ReLU value, g = dy * (z > 0) (relu != 0; TF's ReluGrad is 0 at 0),
+ * x^ = (x - mean)*rstd, g^ = g*gamma:  dx = rstd*(g^ - mean(g^) - x^*mean(g^ x^)) + addend (nullable), and per-clip partials
+ * dgamma_part[b, c] = sum_t g x^, dbeta_part[b, c] = sum_t g (reduce over clips with hd_col_sum).  Any T; dx must not alias x / dy. */
+int hd_groupnorm_relu_backward(const float *x, const float *gamma, const float *beta, const float *dy, const float *addend, float *dx,
+                               float *dgamma_part, float *dbeta_part, int B, int T, int C, int groups, float eps, int relu, void *stream);
+/* out[c] = sum over rows of x[r*ld + c], fixed order (bias gradients, GroupNorm affine gradients, mean_param). */
+int hd_col_sum(const float *x, long long rows, int cols, long long ld, float *out, void *stream);
+/* dx[i] = y[i] > 0 ? dy[i] : 0 (y = the ReLU's output; dx may alias dy). */
+int hd_relu_backward(const float *y, const float *dy, float *dx, long long n, void *stream);
+/* Short-K input gradient of an FC layer with D <= 96 outputs (the IEF fc3, D = 85 / 72):
+ * out[n, k] = (mask[n, k] > 0) * sum_j g[n*g_ld + j] * Wt[j, k], Wt = W^T [D, K] fp32, out / mask dense [N, K] (mask nullable). */
+int hd_fc_small_dgrad(const float *g, int g_ld, const float *Wt, int K, int D, const float *mask, float *out, int N, void *stream);
+/* out[r, c] = a[r, c] + b[r, c] at independent row strides (out may alias a or b): gradient accumulation of the IEF glue. */
+int hd_add_strided(const float *a, long long lda, const float *b, long long ldb, float *out, long long ldo, int rows, int cols, void *stream);
+
 /* ---- Mesh rendering (the visualiser of src/util/render/nmr_renderer.py:43-240: NMR with camera_mode='look_at',
  * perspective=False, anti_aliasing and fill_back on), one colour per mesh.  The model is R1-R8 of oracle/render_ref.py:
  *   x = s*(X + tx), y = -s*(Y + ty), z = Z - eye_z  (R1); a 2S x 2S sample grid whose sample (r, c) sits at image
