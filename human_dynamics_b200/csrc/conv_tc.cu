@@ -24,7 +24,8 @@
 // continuously across tiles, and the producers keep prefetching the next tile's chunks while the consumers run the
 // fused epilogue (scale/shift, residual, ReLU, fp32 output or its strided subsample, the next layer's fp16 pair)
 // straight from the accumulator fragments.  RES (pre-split input, residual row-aligned with the output, K <= 512): each
-// consumer warpgroup's 64 residual rows arrive by TMA in a shared-memory slot while the tile's main loop runs.
+// consumer warpgroup's 64 residual rows arrive by TMA in a shared-memory slot while the tile's main loop runs.  Pre-split
+// layers stage their outputs in shared memory (the fp32 output over the residual slot) and write them with TMA stores.
 //
 // Warp roles:
 //   warps 0-7    two consumer warpgroups: wgmma issue, drains, epilogue (warpgroup g owns tile rows 64 g .. 64 g + 63)
@@ -44,6 +45,8 @@ constexpr int BM = 128;
 constexpr int A_TILE_BYTES = BM * 128;      // 16 KiB: 128 rows x one 128-byte swizzle row (32 tf32 or 64 fp16 of K)
 constexpr int BOX_BYTES = 64 * 128;         // one 64-row weight box (hd_make_weight_tmap)
 constexpr int W_PROD = 8;                   // first producer warp
+// `stage` argument (pre-split layers): which outputs the epilogue stages in shared memory and writes by TMA (launch_tc)
+constexpr int STAGE_OUT = 1, STAGE_PAIR = 2;
 
 using namespace ptx;
 
@@ -58,14 +61,18 @@ struct Cfg {
   static constexpr int PROD_REGS = BN == 128 ? 40 : 104, CONS_REGS = BN == 128 ? 232 : 152;
   static_assert(256 * CONS_REGS + PROD_THREADS * PROD_REGS <= 65536, "setmaxnreg split beyond the register file");
   static constexpr int NACC = BN / 2;                           // fp32 registers of one m64nBN fragment per thread
-  // RES, BN = 128: the 64 KB residual tile does not fit beside three 64 KB stages.  Residual layers have K <= 512 (<= 8 chunks).
-  static constexpr int STAGES = BN == 128 ? (RES ? 2 : 3) : 4;
+  // RES: the residual slots do not fit beside three 64 KB stages (BN = 128) or four 48 KB ones plus the output staging (BN = 64).
+  // Residual layers have K <= 512 (<= 8 chunks).
+  static constexpr int STAGES = BN == 128 ? (RES ? 2 : 3) : (RES ? 3 : 4);
   static constexpr int BKE = HALF ? 64 : 32;                    // K elements per chunk (one 128-byte row)
   static constexpr int B_TILE_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
   static constexpr int RES_OFFSET = STAGES * STAGE_BYTES;
   static constexpr int RES_SLOT_BYTES = RES ? 64 * BN * 4 : 0; // one warpgroup's 64 rows x BN fp32 residual (BN / 32 TMA boxes)
-  static constexpr int BAR_OFFSET = RES_OFFSET + 2 * RES_SLOT_BYTES;
+  static constexpr int STG_OFFSET = RES_OFFSET + 2 * RES_SLOT_BYTES;
+  // ASPLIT: one warpgroup's output staging, two 64-row x 128-byte TMA boxes (64 columns of fp32, or of the fp16 head and remainder)
+  static constexpr int STG_BYTES = ASPLIT ? 2 * BOX_BYTES : 0;
+  static constexpr int BAR_OFFSET = STG_OFFSET + 2 * STG_BYTES;
   static constexpr int SMEM_BYTES = BAR_OFFSET + 128 + 1024;    // + alignment slack
   static_assert(SMEM_BYTES <= 232448, "dynamic shared memory beyond the 227 KB a CTA can opt into");
   static constexpr int PF = HALF ? 2 : 3;                       // producer prefetch ring depth (chunks in flight per thread)
@@ -80,7 +87,8 @@ struct RowState {       // R output rows of one producer thread: image index and
 template <bool SPLIT, int PCH, bool HALF, bool GATHER, bool ASPLIT, int BN, bool RES>
 __global__ void __launch_bounds__((Cfg<HALF, ASPLIT, BN, RES>::NUM_THREADS), 1)
 conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap_hi, const __grid_constant__ CUtensorMap tmap_lo,
-                    const __grid_constant__ CUtensorMap tmap_res) {
+                    const __grid_constant__ CUtensorMap tmap_res, const __grid_constant__ CUtensorMap tmap_out,
+                    const __grid_constant__ CUtensorMap tmap_out_hi, const __grid_constant__ CUtensorMap tmap_out_lo, const int stage) {
   using C = Cfg<HALF, ASPLIT, BN, RES>;
   constexpr int BKE = C::BKE, PF = C::PF, V = C::V, STAGES = C::STAGES, R = C::ROWS, RS = C::ROW_STEP, NA = C::NACC;
   extern __shared__ uint8_t smem_raw[];
@@ -444,8 +452,9 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(C::CONS_REGS));
     const int wg = warp >> 2;                             // rows 64 wg .. 64 wg + 63 of the tile
     const bool prof = p.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0;
-    long long t_wait = 0, t_epi = 0, t_start = prof && !RES ? clock64() : 0;
+    long long t_wait = 0, t_start = prof && !RES ? clock64() : 0;
     if (RES && prof) p.dbg[2] = clock64();    // start stamp in memory (RES, BN = 128: keeps the consumers within 232 registers spill-free)
+    if (prof) p.dbg[4] = 0;                   // epilogue clocks, summed in memory for the same reason
     const int hw = p.Ho * p.Wo;
     const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's fragment rows: frow, frow + 8
     const int fcol = 2 * (lane & 3);                            // and columns 8 j + fcol, + 1
@@ -456,8 +465,10 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     // 16-byte piece k at (k ^ (r & 7)) * 16), issued by the warpgroup's first thread as soon as the previous tile's epilogue has read
     // the slot, so the load overlaps the tile's main loop.  Boxes wholly past M or Cout are not loaded (their values are never read);
     // partial ones are zero-filled by TMA and count their full bytes.
-    const uint8_t *res_sm = smem + C::RES_OFFSET + wg * C::RES_SLOT_BYTES;
+    uint8_t *res_sm = smem + C::RES_OFFSET + wg * C::RES_SLOT_BYTES;
     const bool res_issuer = RES && (threadIdx.x & 127) == 0;
+    // ASPLIT: the same thread issues the warpgroup's output stores (bulk async-groups belong to the thread that commits them)
+    const bool stg_issuer = ASPLIT && (threadIdx.x & 127) == 0;
     auto load_res = [&](int ti) {
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
       const int r0 = (tile / tiles_n) * BM + 64 * wg, c0 = (tile % tiles_n) * BN;
@@ -470,8 +481,6 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     if (res_issuer && my_tiles > 0) load_res(0);
     int q = 0;
     for (int ti = 0; ti < my_tiles; ++ti) {
-      const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-      const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
 #pragma unroll
       for (int i = 0; i < NA; ++i) sums[i] = 0.f;
       for (int kc = 0; kc < num_k; ++kc, ++q) {
@@ -525,39 +534,156 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
 #pragma unroll
         for (int i = 0; i < NA; ++i) sums[i] += accx[i] * (HALF ? (1.0f / 2048.0f) : 1.0f);
       }
-      long long te0 = prof ? clock64() : 0;
+      if (prof) p.dbg[4] -= clock64();                   // the epilogue's clocks, summed in memory (see above)
+      const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
+      const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
       if (RES) mbar_wait(res_bar(wg), (uint32_t)ti & 1u);
-      // Epilogue from the fragments: per row, per pair of adjacent columns (8-byte fp32 / 4-byte fp16-pair stores; the four
-      // threads of a quad cover 8 contiguous columns of a row).  v = acc * scale + shift (+ residual) (ReLU) -> fp32 output
-      // (or its strided subsample), and the next layer's pre-activation relu?(v * s2 + b2) as an fp16 head / remainder pair.
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int m = m0 + frow + 8 * h;
-        if (m >= p.M) continue;
-        int n_img = 0, oy = 0, ox = 0;
+      // Epilogue from the fragments, per row and pair of adjacent columns c, c + 1 (the four threads of a quad cover 8 contiguous
+      // columns of a row): v = acc * scale + shift (+ residual) (ReLU) -> fp32 output (or its strided subsample), and the next
+      // layer's pre-activation relu?(v * s2 + b2) as an fp16 head / remainder pair.
+      auto row_geom = [&](int m, int &n_img, int &oy, int &ox) {
+        n_img = 0; oy = 0; ox = 0;
         if (p.out_sub || (!RES && p.res && !(p.res_stride == 1 && p.res_H == p.Ho && p.res_W == p.Wo))) {
           n_img = m / hw;
           const int r = m - n_img * hw;
           oy = r / p.Wo; ox = r - oy * p.Wo;
         }
-        // RES: this thread's residual row in the slot; its 8-byte pair of columns 8 j + fcol lies in box j / 4, piece 2 (j % 4) + fcol / 4
-        const uint8_t *rsrow = res_sm + (frow - 64 * wg + 8 * h) * 128 + 8 * (lane & 1);
-        const uint32_t rsw = (uint32_t)(lane >> 2);            // the row's swizzle: (frow + 8 h) & 7
-        const float *rrow = nullptr;
-        if (!RES && p.res) {
-          const size_t rr = (p.res_stride == 1 && p.res_H == p.Ho && p.res_W == p.Wo)
-                                ? (size_t)m
-                                : ((size_t)n_img * p.res_H + (size_t)oy * p.res_stride) * p.res_W + (size_t)ox * p.res_stride;
-          rrow = p.res + rr * p.res_ld;
-        }
-        float *orow = nullptr;
-        if (p.out) {
-          if (!p.out_sub) orow = p.out + (size_t)m * p.out_ld;
-          else if (oy % p.out_sub == 0 && ox % p.out_sub == 0) {
-            const int Hs = (p.Ho + p.out_sub - 1) / p.out_sub, Ws = (p.Wo + p.out_sub - 1) / p.out_sub;
-            orow = p.out + ((size_t)((size_t)n_img * Hs + oy / p.out_sub) * Ws + ox / p.out_sub) * p.out_ld;
+      };
+      auto res_row = [&](int m, int n_img, int oy, int ox) -> const float * {     // residual read from global memory (!RES)
+        if (RES || !p.res) return nullptr;
+        const size_t rr = (p.res_stride == 1 && p.res_H == p.Ho && p.res_W == p.Wo)
+                              ? (size_t)m
+                              : ((size_t)n_img * p.res_H + (size_t)oy * p.res_stride) * p.res_W + (size_t)ox * p.res_stride;
+        return p.res + rr * p.res_ld;
+      };
+      auto out_row = [&](int m, int n_img, int oy, int ox) -> float * {
+        if (!p.out) return nullptr;
+        if (!p.out_sub) return p.out + (size_t)m * p.out_ld;
+        if (oy % p.out_sub != 0 || ox % p.out_sub != 0) return nullptr;
+        const int Hs = (p.Ho + p.out_sub - 1) / p.out_sub, Ws = (p.Wo + p.out_sub - 1) / p.out_sub;
+        return p.out + ((size_t)((size_t)n_img * Hs + oy / p.out_sub) * Ws + ox / p.out_sub) * p.out_ld;
+      };
+      // vec_out (Cout % 4 == 0, 16-byte aligned rows and vectors: pairs are 8-byte aligned).  RES: rs is the residual pair in the slot.
+      auto value2 = [&](int c, const float2 *rs, const float *rrow, float &y0, float &y1) {
+        if (p.post_scale) { const float2 sc = __ldg(reinterpret_cast<const float2 *>(p.post_scale + c)); y0 *= sc.x; y1 *= sc.y; }
+        if (p.post_shift) { const float2 sh = __ldg(reinterpret_cast<const float2 *>(p.post_shift + c)); y0 += sh.x; y1 += sh.y; }
+        if (RES) { const float2 r = *rs; y0 += r.x; y1 += r.y; }
+        else if (rrow) { const float2 r = *reinterpret_cast<const float2 *>(rrow + c); y0 += r.x; y1 += r.y; }
+        if (p.post_relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+      };
+      // the next layer's A operand: second affine (+ReLU) = its pre-activation, split into fp16 head/remainder
+      auto pair2 = [&](int c, float a0, float a1, uint32_t &hh, uint32_t &ll) {
+        if (p.post2_scale) { const float2 sc = __ldg(reinterpret_cast<const float2 *>(p.post2_scale + c)); a0 *= sc.x; a1 *= sc.y; }
+        if (p.post2_shift) { const float2 sh = __ldg(reinterpret_cast<const float2 *>(p.post2_shift + c)); a0 += sh.x; a1 += sh.y; }
+        if (p.post2_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+        split_f16x2(a0, a1, hh, ll);
+      };
+      if constexpr (ASPLIT) {
+        // Staged: per 64-column pass, (1) v; the fp32 output goes into 32-column x 64-row boxes in the TMA box layout (row r at
+        // r * 128 B, its 16-byte piece k at (k ^ (r & 7)) * 16), over the residual pair just read (RES) or in the staging
+        // buffer, and v replaces the sums; (2) the pair from v into the staging buffer (head box, remainder box: 64 fp16
+        // columns each).  A filled buffer is published (proxy fence, warpgroup barrier), and the warpgroup's first thread
+        // writes it with TMA bulk-tensor stores, which clip rows >= M and columns >= Cout, and goes on without waiting; it
+        // waits for their reads only before the buffer is filled again.  The strided subsample and a pair pitch that is not a
+        // multiple of 16 bytes are stored from registers.
+        const bool st32 = (stage & STAGE_OUT) != 0, st2 = (stage & STAGE_PAIR) != 0;
+        uint8_t *stg = smem + C::STG_OFFSET + wg * C::STG_BYTES;
+        const uint32_t stg_a = smem_base + C::STG_OFFSET + wg * C::STG_BYTES;
+        const int r0 = m0 + 64 * wg;
+        const uint32_t rsw = (uint32_t)(lane >> 2);            // the swizzle of this thread's rows: (frow + 8 h) & 7
+        auto acquire = [&](bool after_out) {   // the staging buffer may be rewritten: its last stores have been read
+          if (stg_issuer) {
+            if (after_out) bulk_wait_read<1>();                // RES: the fp32 stores just issued read the slot, not the buffer
+            else bulk_wait_read<0>();
+          }
+          named_bar_sync(3 + wg, 128);
+        };
+#pragma unroll
+        for (int cc = 0; cc < BN / 64; ++cc) {
+          const int c0 = n0 + 64 * cc;
+          const bool issue = stg_issuer && r0 < p.M && c0 < p.Cout;
+          if (st32 && !RES) acquire(false);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int m = m0 + frow + 8 * h;
+            if (m >= p.M) continue;
+            int n_img, oy, ox;
+            row_geom(m, n_img, oy, ox);
+            const float *rrow = res_row(m, n_img, oy, ox);
+            float *orow = st32 ? nullptr : out_row(m, n_img, oy, ox);
+            uint8_t *brow = (RES ? res_sm + 2 * cc * BOX_BYTES : stg) + (frow - 64 * wg + 8 * h) * 128 + 8 * (lane & 1);
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * cc + jj;
+              const int c = n0 + 8 * j + fcol;
+              if (c >= p.Cout) continue;
+              // columns 8 j + fcol, + 1: box jj / 4 of the pass, piece 2 (jj % 4) + fcol / 4
+              const uint32_t piece = (uint32_t)(2 * (jj & 3) + ((lane & 3) >> 1)) ^ rsw;
+              float2 *f32 = reinterpret_cast<float2 *>(brow + (jj >> 2) * BOX_BYTES + piece * 16);
+              float y0 = sums[4 * j + 2 * h], y1 = sums[4 * j + 2 * h + 1];
+              value2(c, f32, rrow, y0, y1);
+              if (st32) *f32 = make_float2(y0, y1);
+              else if (orow) *reinterpret_cast<float2 *>(orow + c) = make_float2(y0, y1);
+              sums[4 * j + 2 * h] = y0; sums[4 * j + 2 * h + 1] = y1;
+            }
+          }
+          if (st32) {
+            fence_proxy_async();
+            named_bar_sync(3 + wg, 128);
+            if (issue) {
+              const uint32_t src = RES ? smem_base + C::RES_OFFSET + wg * C::RES_SLOT_BYTES + 2 * cc * BOX_BYTES : stg_a;
+              tma_store_2d(&tmap_out, src, c0, r0);
+              if (c0 + 32 < p.Cout) tma_store_2d(&tmap_out, src + BOX_BYTES, c0 + 32, r0);
+            }
+            if (stg_issuer) bulk_commit();
+          }
+          if (p.out_hi) {
+            if (st2) acquire(RES && st32);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int m = m0 + frow + 8 * h;
+              if (m >= p.M) continue;
+              __half *hrow = reinterpret_cast<__half *>(p.out_hi) + (size_t)m * p.out2_ld;
+              __half *lrow = reinterpret_cast<__half *>(p.out_lo) + (size_t)m * p.out2_ld;
+              uint8_t *brow = stg + (frow - 64 * wg + 8 * h) * 128 + 4 * (lane & 3);
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj) {
+                const int j = 8 * cc + jj;
+                const int c = n0 + 8 * j + fcol;
+                if (c >= p.Cout) continue;
+                uint32_t hh, ll;
+                pair2(c, sums[4 * j + 2 * h], sums[4 * j + 2 * h + 1], hh, ll);
+                if (st2) {       // columns 8 j + fcol, + 1 of the pass: piece jj of the 128-byte row
+                  uint32_t *hs = reinterpret_cast<uint32_t *>(brow + (((uint32_t)jj ^ rsw) * 16));
+                  hs[0] = hh;
+                  hs[BOX_BYTES / 4] = ll;
+                } else {
+                  *reinterpret_cast<uint32_t *>(hrow + c) = hh;
+                  *reinterpret_cast<uint32_t *>(lrow + c) = ll;
+                }
+              }
+            }
+            if (st2) {
+              fence_proxy_async();
+              named_bar_sync(3 + wg, 128);
+              if (issue) {
+                tma_store_2d(&tmap_out_hi, stg_a, c0, r0);
+                tma_store_2d(&tmap_out_lo, stg_a + BOX_BYTES, c0, r0);
+              }
+              if (stg_issuer) bulk_commit();
+            }
           }
         }
+      } else {
+      // register-staged producers: every output from registers
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = m0 + frow + 8 * h;
+        if (m >= p.M) continue;
+        int n_img, oy, ox;
+        row_geom(m, n_img, oy, ox);
+        const float *rrow = res_row(m, n_img, oy, ox);
+        float *orow = out_row(m, n_img, oy, ox);
         __half *hrow = p.out_hi ? reinterpret_cast<__half *>(p.out_hi) + (size_t)m * p.out2_ld : nullptr;
         __half *lrow = p.out_hi ? reinterpret_cast<__half *>(p.out_lo) + (size_t)m * p.out2_ld : nullptr;
 #pragma unroll
@@ -566,23 +692,12 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           if (c >= p.Cout) continue;
           const bool two = c + 1 < p.Cout;
           float y[2] = {sums[4 * j + 2 * h], sums[4 * j + 2 * h + 1]};
-          if (p.vec_out) {                              // Cout % 4 == 0, 16-byte aligned rows and vectors: pairs are 8-byte aligned
-            if (p.post_scale) { const float2 sc = __ldg(reinterpret_cast<const float2 *>(p.post_scale + c)); y[0] *= sc.x; y[1] *= sc.y; }
-            if (p.post_shift) { const float2 sh = __ldg(reinterpret_cast<const float2 *>(p.post_shift + c)); y[0] += sh.x; y[1] += sh.y; }
-            if (RES) {
-              const uint32_t piece = (uint32_t)(2 * (j & 3) + ((lane & 3) >> 1)) ^ rsw;
-              const float2 r = *reinterpret_cast<const float2 *>(rsrow + (j >> 2) * (64 * 128) + piece * 16);
-              y[0] += r.x; y[1] += r.y;
-            } else if (rrow) { const float2 r = *reinterpret_cast<const float2 *>(rrow + c); y[0] += r.x; y[1] += r.y; }
-            if (p.post_relu) { y[0] = fmaxf(y[0], 0.f); y[1] = fmaxf(y[1], 0.f); }
+          if (p.vec_out) {
+            value2(c, nullptr, rrow, y[0], y[1]);
             if (orow) *reinterpret_cast<float2 *>(orow + c) = make_float2(y[0], y[1]);
-            if (hrow) {       // the next layer's A operand: second affine (+ReLU) = its pre-activation, split into fp16 head/remainder
-              float a0 = y[0], a1 = y[1];
-              if (p.post2_scale) { const float2 sc = __ldg(reinterpret_cast<const float2 *>(p.post2_scale + c)); a0 *= sc.x; a1 *= sc.y; }
-              if (p.post2_shift) { const float2 sh = __ldg(reinterpret_cast<const float2 *>(p.post2_shift + c)); a0 += sh.x; a1 += sh.y; }
-              if (p.post2_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+            if (hrow) {
               uint32_t hh, ll;
-              split_f16x2(a0, a1, hh, ll);
+              pair2(c, y[0], y[1], hh, ll);
               *reinterpret_cast<uint32_t *>(hrow + c) = hh;
               *reinterpret_cast<uint32_t *>(lrow + c) = ll;
             }
@@ -600,13 +715,21 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           }
         }
       }
+      }
       if (RES && ti + 1 < my_tiles) {
         named_bar_sync(1 + wg, 128);                       // every thread of the warpgroup has read the slot
-        if (res_issuer) load_res(ti + 1);
+        if (res_issuer) {
+          if (stage & STAGE_OUT) {                         // the slot's fp32 stores have read it (the pair's may still run)
+            if (stage & STAGE_PAIR) bulk_wait_read<1>();
+            else bulk_wait_read<0>();
+          }
+          load_res(ti + 1);
+        }
       }
-      if (prof) t_epi += clock64() - te0;
+      if (prof) p.dbg[4] += clock64();
     }
-    if (prof) { p.dbg[2] = clock64() - (RES ? p.dbg[2] : t_start); p.dbg[3] = t_wait; p.dbg[4] = t_epi; }
+    if (stg_issuer) bulk_wait_all();                       // the last stores have completed before the CTA exits
+    if (prof) { p.dbg[2] = clock64() - (RES ? p.dbg[2] : t_start); p.dbg[3] = t_wait; }
   }
 }
 
@@ -629,6 +752,27 @@ EncodeTiledFn get_encode_fn() {
 }
 
 constexpr int kMaxDevices = 64;
+
+// Map over a row-major [rows, cols] activation matrix (row pitch ld_bytes) with the box of one warpgroup's epilogue: 128 bytes of
+// columns x 64 rows, 128-byte swizzle.  gdim = {cols, rows}: TMA clips a partial box and never touches the pitch padding.
+int encode_epilogue_map(CUtensorMap *tm, bool fp16, const void *base, int cols, int rows, long long ld_bytes, const char *what) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) { set_last_error_text("cuTensorMapEncodeTiled unavailable (no CUDA driver?)"); return HD_ERR_UNSUPPORTED; }
+  const cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t gstride[1] = {(cuuint64_t)ld_bytes};
+  const cuuint32_t box[2] = {fp16 ? 64u : 32u, 64u};
+  const cuuint32_t estr[2] = {1u, 1u};
+  CUresult r = fn(tm, fp16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(base), gdim, gstride,
+                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    char msg[96];
+    snprintf(msg, sizeof(msg), "cuTensorMapEncodeTiled (%s) failed with CUresult %d", what, (int)r);
+    set_last_error_text(msg);
+    return HD_ERR_CUDA;
+  }
+  return HD_OK;
+}
 
 template <bool SPLIT, int PCH, bool HALF, bool GATHER = false, bool ASPLIT = false, int BN = 64, bool RES = false>
 int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
@@ -653,31 +797,33 @@ int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
   const void *mlo = d->tmap_hi_n64 ? d->tmap_lo_n64 : d->tmap_lo;
   memcpy(&thi, mhi, sizeof(CUtensorMap));
   memcpy(&tlo, mlo ? mlo : mhi, sizeof(CUtensorMap));     // mlo is null only for 1xTF32, which never loads it (launch_conv_tc)
-  // RES: the residual map is encoded here from p.res on every launch, never taken from the descriptor's activation maps, so it
-  // always describes the buffer this launch reads.  Box: 32 fp32 columns (one 128-byte swizzle row) x 64 rows (one warpgroup).
-  alignas(64) CUtensorMap tres;
-  if (RES) {
-    EncodeTiledFn fn = get_encode_fn();
-    if (!fn) { set_last_error_text("cuTensorMapEncodeTiled unavailable (no CUDA driver?)"); return HD_ERR_UNSUPPORTED; }
-    const cuuint64_t gdim[2] = {(cuuint64_t)p.Cout, (cuuint64_t)p.M};
-    const cuuint64_t gstride[1] = {(cuuint64_t)p.res_ld * 4u};
-    const cuuint32_t box[2] = {32u, 64u};
-    const cuuint32_t estr[2] = {1u, 1u};
-    CUresult r = fn(&tres, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(p.res), gdim, gstride, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      char msg[96];
-      snprintf(msg, sizeof(msg), "cuTensorMapEncodeTiled (residual) failed with CUresult %d", (int)r);
-      set_last_error_text(msg);
-      return HD_ERR_CUDA;
-    }
-  } else {
-    memcpy(&tres, &thi, sizeof(CUtensorMap));             // not read
+  // The residual and output maps are encoded here from p.res / p.out / p.out_hi / p.out_lo on every launch, never taken from the
+  // descriptor's activation maps, so they always describe the buffers this launch reads and writes.  Maps not used stay copies
+  // of the weight map.
+  alignas(64) CUtensorMap tres, tout, tohi, tolo;
+  memcpy(&tres, &thi, sizeof(CUtensorMap));
+  memcpy(&tout, &thi, sizeof(CUtensorMap));
+  memcpy(&tohi, &thi, sizeof(CUtensorMap));
+  memcpy(&tolo, &thi, sizeof(CUtensorMap));
+  int rc = HD_OK;
+  if (RES) rc = encode_epilogue_map(&tres, false, p.res, p.Cout, p.M, p.res_ld * 4, "residual");
+  // Pre-split layers stage outputs in shared memory for TMA stores, except those TMA cannot write: the strided subsample, and a
+  // pair whose row pitch is not a multiple of 16 bytes (vec_out, checked by launch_conv_tc, gives aligned bases and fp32 pitches).
+  int stage = 0;
+  if (ASPLIT && p.out && !p.out_sub) {
+    stage |= STAGE_OUT;
+    if (rc == HD_OK) rc = encode_epilogue_map(&tout, false, p.out, p.Cout, p.M, p.out_ld * 4, "output");
   }
+  if (ASPLIT && p.out_hi && p.out2_ld % 8 == 0) {
+    stage |= STAGE_PAIR;
+    if (rc == HD_OK) rc = encode_epilogue_map(&tohi, true, p.out_hi, p.Cout, p.M, p.out2_ld * 2, "output head");
+    if (rc == HD_OK) rc = encode_epilogue_map(&tolo, true, p.out_lo, p.Cout, p.M, p.out2_ld * 2, "output remainder");
+  }
+  if (rc != HD_OK) return rc;
   const int num_tiles = ceil_div(p.M, BM) * ceil_div(p.Cout, BN);
   dim3 grid(num_tiles < num_sms[dev] ? num_tiles : num_sms[dev]);     // persistent: one CTA per SM walks the tile list
-  conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES><<<grid, C::NUM_THREADS, C::SMEM_BYTES, st>>>(p, thi, tlo, tres);
+  conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES>
+      <<<grid, C::NUM_THREADS, C::SMEM_BYTES, st>>>(p, thi, tlo, tres, tout, tohi, tolo, stage);
   return check_launch("conv_gemm_tc_kernel");
 }
 

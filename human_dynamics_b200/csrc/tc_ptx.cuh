@@ -47,6 +47,9 @@ static __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap *tmap, 
 static __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 static __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+static __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// generic-proxy shared-memory writes -> visible to the async proxy (a following TMA store or wgmma)
+static __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 static __device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 // One lane of a CONVERGED warp (elect.sync).  Code guarded by this predicate is known to the compiler to run in a single thread, so
 // warp-uniform instructions (TMA) are emitted once, not inside a per-active-lane ELECT loop as under `lane == 0`.

@@ -81,9 +81,9 @@ typedef struct {
   const float *post2_scale, *post2_shift;  int post2_relu;
   /* Activation tensor maps (impl 3, pre-split input, Cout % 32 == 0, residual row == output row): HOST pointers to 128-byte
    * CUtensorMap blobs from hd_make_act_tmap over `res`, `out`, `out_hi`, `out_lo` (each required iff that pointer is set).
-   * The sm_90a kernel does not read them: it writes every output from the accumulator registers, and results do not depend on
-   * the maps or on HD_CONV_NO_TMA_EPILOGUE in `flags`.  They are kept only for ABI compatibility: out_subsample (below) is still
-   * accepted exactly when they are given and the flag is unset, as it was for the earlier TMA epilogue. */
+   * The sm_90a kernel does not read them: it encodes its own residual and output maps from `res`, `out`, `out_hi` and `out_lo`
+   * on every launch, and results do not depend on these maps or on HD_CONV_NO_TMA_EPILOGUE in `flags`.  They are kept only for
+   * ABI compatibility: out_subsample (below) is still accepted exactly when they are given and the flag is unset. */
   const void *tmap_res, *tmap_out, *tmap_out_hi, *tmap_out_lo;
   int flags;
   /* optional: weight maps to use instead of tmap_hi / tmap_lo (64-row box; the kernel loads a 64- or 128-wide N tile as one or
