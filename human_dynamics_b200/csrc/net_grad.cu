@@ -9,13 +9,13 @@
 
 namespace {
 
-// Round to the nearest TF32 value (low 13 mantissa bits zero): the same bit trick as nets.py:tf32_split.
+// Round to the nearest TF32 value (low 13 mantissa bits zero); oracle/pack_ref.py:tf32_split restates it in numpy.
 __device__ __forceinline__ float rn_tf32(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
 
 // One element of a split operand: mode 0 = plain fp32 (hi only), 1 = TF32 head / remainder (fp32 storage), 2 = fp16 head /
-// 2^11-scaled remainder (the arithmetic of nets.py:f16_split, numpy's round-to-nearest-even conversions).
+// 2^11-scaled remainder (round-to-nearest-even conversions; oracle/pack_ref.py:f16_split restates it in numpy).
 __device__ __forceinline__ void store_split(float v, int mode, void *hi, void *lo, size_t o) {
   if (mode == 2) {
     const __half h = __float2half_rn(v);

@@ -1,10 +1,10 @@
 // Network-level entry points (SURVEY.md 8b): slim resnet_v2_50, f_movie and the IEF regressor as library-owned layer plans.
 //
 // Host-only code.  A plan packs the TF-named weights once (BatchNorm folded in double precision, K-major fp16 head / 2^11-scaled
-// remainder split, TMA descriptors), owns its activation buffers, and `*_forward` is a fixed sequence of the per-layer entries of
-// this library (hd_conv_gemm and friends) on the caller's stream: no allocation, no synchronisation.  The sequence, buffers and
-// descriptors are the same as the Python host plans (human_dynamics_b200/nets.py: ResNetPlan in split mode, FMoviePlan /
-// IEFPlan fast paths), so the results are bit-identical to them (tests/test_gpu_cplan.py).
+// remainder written on the device by hd_pack_weight, TMA descriptors), owns its activation buffers, and `*_forward` is a fixed
+// sequence of the per-layer entries of this library (hd_conv_gemm and friends) on the caller's stream: no allocation, no
+// synchronisation.  The sequence, buffers and descriptors are the same as the Python host plans (human_dynamics_b200/nets.py:
+// ResNetPlan in split mode, FMoviePlan / IEFPlan fast paths), so the results are bit-identical to them (tests/test_gpu_cplan.py).
 //
 // Reference functions replaced (graph-building Python + sess.run in the reference):
 //   hd_resnet50_forward  encoder_resnet            src/models.py:50-77  (slim resnet_v2_50 [TF-ext], global pool, squeeze)
@@ -12,8 +12,6 @@
 //   hd_ief_forward       call_hmr_ief / hmr_ief    src/models.py:299-415 (+ encoder_fc3_dropout :80-116), use_optcam=True,
 //                                                   use_delta_from_pred=True as wired by tester.py:196-207
 #include "common.cuh"
-
-#include <cuda_fp16.h>
 
 #include <algorithm>
 #include <cmath>
@@ -121,20 +119,25 @@ struct Builder {
     return true;
   }
 
-  // K-major [rows_pad, K] fp16 head / 2^11-scaled remainder (nets.py f16_split) + TMA descriptors
-  bool pack_nk(PackedConv &c, const std::vector<float> &w_nk, int rows_pad, int box) {
-    std::vector<__half> hi(w_nk.size()), lo(w_nk.size());
-    for (size_t i = 0; i < w_nk.size(); ++i) {
-      const __half h = __float2half_rn(w_nk[i]);
-      hi[i] = h;
-      lo[i] = __float2half_rn((w_nk[i] - __half2float(h)) * 2048.0f);
-    }
-    c.w_hi = upload(hi); c.w_lo = upload(lo);
+  // K-major [roundup64(Cout), K_pad] fp16 head / 2^11-scaled remainder of the device weight w [KH, Cin, Cout] (hd_pack_weight on the
+  // default stream; sync() completes it) + TMA descriptors (box 64 rows: the kernel loads a 64/128-wide N tile as one or two, conv_tc.cu)
+  bool pack(PackedConv &c, const float *w, int KH, int Cin) {
+    const int rows = (c.Cout + 63) / 64 * 64;
+    c.w_hi = dev_alloc((size_t)rows * c.K_pad * 2); c.w_lo = dev_alloc((size_t)rows * c.K_pad * 2);
     if (!c.w_hi || !c.w_lo) return false;
     c.tmap_hi = new_map(true); c.tmap_lo = new_map(true);
-    int r = hd_make_weight_tmap(c.w_hi, rows_pad, c.K_pad, box, 2, c.tmap_hi);
-    if (!r) r = hd_make_weight_tmap(c.w_lo, rows_pad, c.K_pad, box, 2, c.tmap_lo);
+    int r = hd_pack_weight(w, KH, Cin, c.Cout, HD_PACK_FORWARD, 2, c.w_hi, c.w_lo, rows, c.K_pad, nullptr);
+    if (!r) r = hd_make_weight_tmap(c.w_hi, rows, c.K_pad, 64, 2, c.tmap_hi);
+    if (!r) r = hd_make_weight_tmap(c.w_lo, rows, c.K_pad, 64, 2, c.tmap_lo);
     if (r) { rc = rc ? rc : r; return false; }
+    return true;
+  }
+
+  // waits for the packing queued by pack(): a plan's weights are then ready on any stream
+  bool sync() {
+    if (rc != HD_OK) return false;
+    const cudaError_t e = cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) { hd::set_last_error("cudaStreamSynchronize", e); rc = HD_ERR_CUDA; return false; }
     return true;
   }
 
@@ -152,12 +155,7 @@ struct Builder {
     if (!c.w_kn || (scale && !c.post_scale) || (shift && !c.post_shift)) return false;
     if (!tc) return true;
     if (Cin % 64 != 0) return fail(HD_ERR_UNSUPPORTED, "layer '" + wname + "': Cin % 64 != 0 has no fp16 tensor-core packing");
-    const int box = 64;                               // the N tile of the tensor-core kernel (conv_tc.cu)
-    const int rows = (Cout + box - 1) / box * box;
-    std::vector<float> w_nk((size_t)rows * c.K, 0.0f);
-    for (int k = 0; k < c.K; ++k)
-      for (int co = 0; co < Cout; ++co) w_nk[(size_t)co * c.K + k] = w[(size_t)k * Cout + co];
-    return pack_nk(c, w_nk, rows, box);
+    return pack(c, c.w_kn, KH * KW, Cin);
   }
 
   bool bias_vec(const std::string &name, int C, std::vector<float> &v) {
@@ -311,19 +309,19 @@ int hd_resnet50_create(hd_weight_fn get, void *user, int n_frames, int size, hd_
   const int n = n_frames;
 
   // ---- pack (nets.py PackedResNet) ----
-  PackedConv conv1;                        // PackedConv1Planes: [co, ky(8), kx(8), c(4)] with zero weights in the padding taps
+  PackedConv conv1;                        // PackedConv1Planes: HWIO [ky(8), kx(8), c(4), co] with zero weights in the padding taps
   {
     const float *w = b.weight(p + "/conv1/weights", 7 * 7 * 3 * 64);
     std::vector<float> bias;
     if (w && b.bias_vec(p + "/conv1/biases", 64, bias)) {
       conv1.Cout = 64; conv1.K = conv1.K_pad = 256;
-      std::vector<float> w_nk((size_t)64 * 256, 0.0f);
+      std::vector<float> wp((size_t)256 * 64, 0.0f);
       for (int ky = 0; ky < 7; ++ky)
         for (int kx = 0; kx < 7; ++kx)
-          for (int c = 0; c < 3; ++c)
-            for (int co = 0; co < 64; ++co) w_nk[(size_t)co * 256 + (ky * 8 + kx) * 4 + c] = w[((ky * 7 + kx) * 3 + c) * 64 + co];
+          for (int c = 0; c < 3; ++c) memcpy(&wp[(size_t)((ky * 8 + kx) * 4 + c) * 64], w + ((ky * 7 + kx) * 3 + c) * 64, 64 * sizeof(float));
       conv1.post_shift = (float *)b.upload(bias);
-      b.pack_nk(conv1, w_nk, 64, 64);
+      const float *wd = (const float *)b.upload(wp);
+      if (conv1.post_shift && wd) b.pack(conv1, wd, 8, 32);
     }
   }
   std::vector<Unit> units;
@@ -358,6 +356,7 @@ int hd_resnet50_create(hd_weight_fn get, void *user, int n_frames, int size, hd_
     std::vector<float> s, sh;
     if (b.fold_bn(p + "/postnorm", d_in, s, sh)) { post_scale = (float *)b.upload(s); post_shift = (float *)b.upload(sh); }
   }
+  b.sync();
   if (b.rc != HD_OK) { const int r = b.rc; hd_net_destroy(net); return r; }
 
   // ---- plan (nets.py ResNetPlan, split mode, root + all units + tail) ----
@@ -493,6 +492,7 @@ int hd_fmovie_create(hd_weight_fn get, void *user, int B, int T, int num_conv_la
       if (!b.make_conv(convs[2 * i + k - 1], cv + "/weights", 3, 1, C, C, 1, 1, 0, nullptr, &bias, 0)) break;
     }
   }
+  b.sync();
   if (b.rc != HD_OK) { const int r = b.rc; hd_net_destroy(net); return r; }
   *out_net = net;
   return HD_OK;
@@ -574,6 +574,7 @@ int hd_ief_create(hd_weight_fn get, void *user, int N, const int *delta_t, int n
     auto view = [net, i]() { return net->out1 + (size_t)i * 85 + 3; };
     head(sc, 72, [view]() { return (const float *)view(); }, D * 85, view, D * 85);
   }
+  b.sync();
   if (b.rc != HD_OK) { const int r = b.rc; hd_net_destroy(net); return r; }
   *out_net = net;
   return HD_OK;

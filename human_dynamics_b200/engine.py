@@ -14,7 +14,7 @@ import torch
 
 from . import _lib
 from .config import HMMRConfig
-from .nets import FMoviePlan, IEFPlan, PackedConv, PackedFMovie, PackedIEF, PackedResNet, ResNetPlan
+from .nets import FMoviePlan, IEFPlan, PackedConv, PackedFMovie, PackedIEF, PackedResNet, ResNetPlan, sync_packing
 from .smpl import SMPLConstants
 from ._lib import current_stream
 
@@ -101,6 +101,7 @@ class PackedHal(object):
         self.fc1 = PackedConv(w[name + '/fc1/weights'], device, post_shift=w[name + '/fc1/biases'], post_relu=True, tc=tc)
         self.fc2 = PackedConv(w[name + '/fc2/weights'], device, post_shift=w[name + '/fc2/biases'], post_relu=True, tc=tc)
         self.fc3 = PackedConv(w[name + '/fc3/weights'], device, post_shift=w[name + '/fc3/biases'], tc=tc)
+        sync_packing(device)
 
 
 class HMMREngine(object):

@@ -22,7 +22,37 @@ GN_GROUPS = 32
 
 
 def _dev(a, device, dtype=np.float32):
+    if isinstance(a, torch.Tensor):           # already on the device (TemporalModel's parameters): used in place
+        return a
     return torch.from_numpy(np.ascontiguousarray(a, dtype=dtype)).to(device)
+
+
+def pack_weight(src, KH, Cin, Cout, hi, lo, stream):
+    """hd_pack_weight (forward): the fp32 weight src [KH, Cin, Cout] on the device -> K-major head / remainder hi, lo [rows, k_pad]
+    (fp16 tensors: fp16 head + 2^11-scaled remainder; fp32 tensors: TF32 pair), zero past the matrix.  Runs on `stream`."""
+    check(lib.hd_pack_weight(C.c_void_p(src.data_ptr()), KH, Cin, Cout, _lib.HD_PACK_FORWARD, hi.element_size(), C.c_void_p(hi.data_ptr()),
+                             C.c_void_p(lo.data_ptr()), hi.shape[0], hi.shape[1], stream), 'hd_pack_weight')
+
+
+def weight_tmap(t):
+    """128-byte TMA descriptor of a packed [rows, k_pad] weight half (box 64 rows: the kernel loads a 64- or 128-wide N tile as one or
+    two boxes, conv_tc.cu)."""
+    m = (C.c_ubyte * 128)()
+    check(lib.hd_make_weight_tmap(C.c_void_p(t.data_ptr()), t.shape[0], t.shape[1], 64, t.element_size(), C.cast(m, C.c_void_p)),
+          'hd_make_weight_tmap')
+    return m
+
+
+def _packs_on(device):
+    """Packing is a kernel launch, so only a CUDA device runs it.  Host-side plan logic on another device (the CPU wiring tests) gets
+    its pack tensors and descriptors, but the packs stay unwritten."""
+    return torch.device(device).type == 'cuda'
+
+
+def sync_packing(device):
+    """Wait for the packing queued on `device`'s current stream: a constructor's weights are then complete on any stream."""
+    if _packs_on(device):
+        torch.cuda.current_stream(device).synchronize()
 
 
 def fold_bn(w, prefix):
@@ -35,44 +65,24 @@ def fold_bn(w, prefix):
     return s.astype(np.float32), (b - m * s).astype(np.float32)
 
 
-def tf32_split(w):
-    """w (float32) -> (hi, lo), both exactly representable in TF32 (low 13 mantissa bits zero, which is all the
-    tensor core reads): hi = w rounded to nearest TF32, lo = (w - hi) rounded to nearest TF32.  Rounding (not
-    truncating) keeps the representation error zero-mean, so it does not build up over the 53 layers."""
-    def rn_tf32(x):
-        b = np.ascontiguousarray(x, np.float32).view(np.uint32)
-        return ((b + np.uint32(0x1000)) & np.uint32(0xFFFFE000)).view(np.float32)
-    w = np.ascontiguousarray(w, np.float32)
-    hi = rn_tf32(w)
-    lo = rn_tf32((w - hi).astype(np.float32))
-    return hi, lo
-
-
-def f16_split(w):
-    """w (float32) -> (hi, lo) float16: hi = RN_f16(w), lo = RN_f16((w - hi) * 2^11).  Same 11+11 significant bits as the
-    TF32 split at twice the tensor-core rate; the 2^11 scale keeps the remainder of small weights out of the fp16
-    subnormal range (the kernel accumulates the scaled cross terms separately and rescales once)."""
-    w = np.ascontiguousarray(w, np.float32)
-    hi = w.astype(np.float16)
-    lo = ((w - hi.astype(np.float32)) * np.float32(2048.0)).astype(np.float16)
-    return hi, lo
-
-
 class PackedConv(object):
-    """Device-resident weights (+ epilogue vectors) of one conv / FC layer."""
+    """Device-resident weights (+ epilogue vectors) of one conv / FC layer.
+
+    w_hwio: TF HWIO (FC: [in, out]) float32, a host array or a contiguous device tensor whose storage the layer then reads in place
+    (as post_scale / post_shift may be).  The tensor-core packs (K-major head / remainder, rows padded to 64; DESIGN.md 3) are written
+    from it on the device by hd_pack_weight, on the current stream."""
 
     def __init__(self, w_hwio, device, post_scale=None, post_shift=None, post_relu=False, stride=1, pad=(0, 0),
                  tc=False):
-        w_hwio = np.asarray(w_hwio, np.float32)
-        if w_hwio.ndim == 2:
-            w_hwio = w_hwio[None, None]
-        self.KH, self.KW, self.Cin, self.Cout = w_hwio.shape
+        if not isinstance(w_hwio, torch.Tensor):
+            w_hwio = np.asarray(w_hwio, np.float32)
+        shape = tuple(w_hwio.shape)
+        self.KH, self.KW, self.Cin, self.Cout = (1, 1) + shape if len(shape) == 2 else shape
         self.K = self.KH * self.KW * self.Cin
         self.stride = stride
         self.pad_t, self.pad_l = pad
         self.device = device
-        w_kn = w_hwio.reshape(self.K, self.Cout)
-        self.w_kn = _dev(w_kn, device)
+        self.w_kn = _dev(w_hwio.reshape(self.K, self.Cout), device)
         self.post_scale = _dev(post_scale, device) if post_scale is not None else None
         self.post_shift = _dev(post_shift, device) if post_shift is not None else None
         self.post_relu = bool(post_relu)
@@ -87,32 +97,26 @@ class PackedConv(object):
             seg = self.KW * self.Cin
             segp = (seg + 7) // 8 * 8                        # gather layout: each kernel row's KW*Cin floats padded to x8
             self.K_pad = (self.KH * segp + 63) // 64 * 64 if gather else self.K
-            box = 64                                         # the TMA box the kernel loads its 64/128-wide N tile in (conv_tc.cu)
-            rows = (self.Cout + box - 1) // box * box
-            w_nk = np.zeros((rows, self.K_pad), np.float32)
             if gather:                                       # K index = ky*segp + (kx*Cin + ci)   (conv_tc.cu GATHER producer)
-                wg = w_hwio.reshape(self.KH, seg, self.Cout)
-                for ky in range(self.KH):
-                    w_nk[:self.Cout, ky * segp:ky * segp + seg] = wg[ky].T
+                src = torch.zeros((self.KH, segp, self.Cout), dtype=torch.float32, device=device)
+                src[:, :seg] = self.w_kn.view(self.KH, seg, self.Cout)
+                self.pack_src = (src, self.KH, segp)
             else:
-                w_nk[:self.Cout, :self.K] = w_kn.T
-            if want == 'f16':
-                hi, lo = f16_split(w_nk)
-                self.w_nk_hi = torch.from_numpy(hi).to(device)
-                self.w_nk_lo = torch.from_numpy(lo).to(device)
-                eb = 2
-            else:
-                hi, lo = tf32_split(w_nk)
-                self.w_nk_hi = _dev(hi, device)
-                self.w_nk_lo = _dev(lo, device)
-                eb = 4
-            self.tmap_hi = (C.c_ubyte * 128)()
-            self.tmap_lo = (C.c_ubyte * 128)()
-            check(lib.hd_make_weight_tmap(C.c_void_p(self.w_nk_hi.data_ptr()), rows, self.K_pad, box, eb, C.cast(self.tmap_hi, C.c_void_p)),
-                  'hd_make_weight_tmap')
-            check(lib.hd_make_weight_tmap(C.c_void_p(self.w_nk_lo.data_ptr()), rows, self.K_pad, box, eb, C.cast(self.tmap_lo, C.c_void_p)),
-                  'hd_make_weight_tmap')
+                self.pack_src = (self.w_kn, self.KH * self.KW, self.Cin)
+            rows = (self.Cout + 63) // 64 * 64
+            dt = torch.float16 if want == 'f16' else torch.float32
+            self.w_nk_hi = torch.empty((rows, self.K_pad), dtype=dt, device=device)
+            self.w_nk_lo = torch.empty((rows, self.K_pad), dtype=dt, device=device)
+            if _packs_on(device):
+                self.repack(current_stream())
+            self.tmap_hi, self.tmap_lo = weight_tmap(self.w_nk_hi), weight_tmap(self.w_nk_lo)
             self.tc = want
+
+    def repack(self, stream):
+        """Rewrite w_nk_hi / w_nk_lo on `stream` from the fp32 source `pack_src` (w_kn; for the gather layout its zero-padded copy
+        [KH, segp, Cout] made at construction)."""
+        src, KH, Cin = self.pack_src
+        pack_weight(src, KH, Cin, self.Cout, self.w_nk_hi, self.w_nk_lo, stream)
 
     def bind(self, inp, n_img, H, W, out, in_ld=None, out_ld=None, pre=None, res=None, res_geom=None, impl='auto',
              inp_split=None, out_split=None, post2=None, out_subsample=0):
@@ -267,16 +271,14 @@ class PackedConv1Planes(object):
         assert w.shape == (7, 7, 3, 64), w.shape
         self.device = device
         self.Cout, self.K = 64, 256
-        w_nk = np.zeros((64, 8, 8, 4), np.float32)                 # [co, ky, kx, c]
-        w_nk[:, :7, :7, :3] = w.transpose(3, 0, 1, 2)
-        hi, lo = f16_split(w_nk.reshape(64, 256))
-        self.w_nk_hi = torch.from_numpy(hi).to(device)
-        self.w_nk_lo = torch.from_numpy(lo).to(device)
+        wp = np.zeros((8, 8, 4, 64), np.float32)                   # [ky, kx, c, co]: K index ky*32 + kx*4 + c
+        wp[:7, :7, :3] = w
+        self.w_nk_hi = torch.empty((64, 256), dtype=torch.float16, device=device)
+        self.w_nk_lo = torch.empty((64, 256), dtype=torch.float16, device=device)
+        if _packs_on(device):
+            pack_weight(_dev(wp, device), 8, 32, 64, self.w_nk_hi, self.w_nk_lo, current_stream())
         self.bias = _dev(bias, device)
-        self.tmap_hi = (C.c_ubyte * 128)()
-        self.tmap_lo = (C.c_ubyte * 128)()
-        for t, m in ((self.w_nk_hi, self.tmap_hi), (self.w_nk_lo, self.tmap_lo)):
-            check(lib.hd_make_weight_tmap(C.c_void_p(t.data_ptr()), 64, 256, 64, 2, C.cast(m, C.c_void_p)), 'hd_make_weight_tmap')
+        self.tmap_hi, self.tmap_lo = weight_tmap(self.w_nk_hi), weight_tmap(self.w_nk_lo)
 
     @staticmethod
     def plane_width(size):
@@ -345,6 +347,7 @@ class PackedResNet(object):
         s, b = fold_bn(w, p + '/postnorm')
         self.post = (_dev(s, device), _dev(b, device))
         self.out_dim = d_in
+        sync_packing(device)
 
 
 class ResNetPlan(object):
@@ -567,6 +570,7 @@ class PackedFMovie(object):
                                                post_shift=w['AZ_FC_block2_conv%d%s/biases' % (k, name)], pad=(1, 0), tc=tc)
             self.blocks.append(blk)
         self.C = self.blocks[0]['conv1'].Cin if self.blocks else 2048
+        sync_packing(device)
 
 
 class FMoviePlan(object):
@@ -667,6 +671,7 @@ class PackedIEF(object):
             sc = scope + ('_future%d' % dt if dt > 0 else '_past%d' % abs(dt))
             self.deltas[dt] = PackedIEFHead(w, sc, device, tc=tc)
         self.mean_param = _dev(np.asarray(w['mean_param'], np.float32).reshape(1, 85), device)
+        sync_packing(device)
 
 
 class IEFPlan(object):

@@ -148,13 +148,15 @@ class SMPLConstants(object):
         self.blend = None
         self._tc_bufs = {}
         if tc:
-            from .nets import PackedConv
+            from .nets import PackedConv, sync_packing
             self.vp_ld = (V * 3 + 3) // 4 * 4
             wb = np.zeros((256, self.vp_ld), np.float32)
             wb[:217, :V * 3] = dirs
             bias = np.zeros(self.vp_ld, np.float32)
             bias[:V * 3] = v_template.reshape(-1)
-            self.blend = PackedConv(wb, dev, post_shift=bias, tc='tc3h')
+            with torch.cuda.device(dev):                       # packed on dev's current stream
+                self.blend = PackedConv(wb, dev, post_shift=bias, tc='tc3h')
+                sync_packing(dev)
             # dense skinning weights as the A operand of the tensor-core skinning GEMM: [roundup128(V), 32] fp16 head + unscaled remainder
             wd = np.zeros(((V + 127) // 128 * 128, 32), np.float32)
             wd[:V, :24] = weights
@@ -256,7 +258,7 @@ class SMPLConstants(object):
         if self._grad is None:
             if self.blend is None:
                 raise _lib.HDError('the SMPL backward recomputes v_posed on the tensor-core blend: build SMPLConstants with tc=True')
-            from .nets import PackedConv
+            from .nets import PackedConv, sync_packing
             weights, kreg, dirs = self._grad_src
             V, dev = self.num_verts, self.device
             pk = pack_grad_arrays(weights, kreg)
@@ -270,7 +272,9 @@ class SMPLConstants(object):
             # Gradients carry the loss's arbitrary scale, so they never go through the fp16 head / remainder split.
             wt = np.zeros((self.vp_ld, _lib.SMPL_GRAD_CLD), np.float32)
             wt[:V * 3, :217] = dirs.T
-            gemm = PackedConv(wt, dev, tc='tc3')
+            with torch.cuda.device(dev):
+                gemm = PackedConv(wt, dev, tc='tc3')
+                sync_packing(dev)
             if gemm.tc != 'tf32':
                 raise _lib.HDError('dirs^T did not get the TF32 tensor-core packing (vp_ld %% 32 != 0?)')
             self._grad = (g, keep, gemm)

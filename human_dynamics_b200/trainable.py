@@ -28,7 +28,7 @@ from torch.autograd.function import once_differentiable
 
 from . import _lib
 from ._lib import lib, check, fptr, current_stream, ConvDesc
-from .nets import FAST_HEADS, GN_EPS, GN_GROUPS, PackedConv
+from .nets import FAST_HEADS, GN_EPS, GN_GROUPS, PackedConv, sync_packing, weight_tmap
 
 F32 = torch.float32
 
@@ -41,57 +41,33 @@ def _round(x, m):
     return (x + m - 1) // m * m
 
 
-def _tmap(t, rows, k_pad, eb):
-    m = (C.c_ubyte * 128)()
-    check(lib.hd_make_weight_tmap(_vp(t), rows, k_pad, 64, eb, C.cast(m, C.c_void_p)), 'hd_make_weight_tmap')
-    return m
+class BackwardDataPack(object):
+    """The transposed, tap-flipped weight of a KH x 1 conv (FC: KH = 1) whose conv is dX, written on the device from the fp32 weight
+    [KH, Cin, Cout] by hd_pack_weight(HD_PACK_BACKWARD_DATA): TF32 head / remainder [roundup64(Cin), KH*Cout] for impl tc3."""
 
-
-class DevicePackedConv(PackedConv):
-    """A PackedConv whose K-major head / remainder packs are written on the device from an fp32 weight tensor (hd_pack_weight),
-    so a training step never round-trips the weights through the host.
-
-    mode HD_PACK_FORWARD: the layer itself, fp16 packing (impl tc3h), exactly what PackedConv(tc='f16') holds; w_kn / post_shift point
-    at the parameter storage.  mode HD_PACK_BACKWARD_DATA: the transposed, tap-flipped layer whose conv is dX (TF32 packing, impl tc3)."""
-
-    def __init__(self, weight, KH, Cin, Cout, mode=_lib.HD_PACK_FORWARD, bias=None, post_relu=False, pad=0):
-        fwd = mode == _lib.HD_PACK_FORWARD
-        self.src, self.mode, self.src_shape = weight, mode, (KH, Cin, Cout)
-        self.KH, self.KW = KH, 1
-        self.Cin, self.Cout = (Cin, Cout) if fwd else (Cout, Cin)
-        self.K = self.K_pad = KH * self.Cin
-        self.stride, self.pad_t, self.pad_l = 1, pad, 0
-        self.device = weight.device
-        self.w_kn = weight
-        self.post_scale = None
-        self.post_shift = bias
-        self.post_relu = bool(post_relu)
-        self.gather = False
-        self.tc = 'f16' if fwd else 'tf32'
-        self.eb = 2 if fwd else 4
-        if self.K % (32 if self.eb == 4 else 64) != 0:
-            raise _lib.HDError('DevicePackedConv: K = %d does not fit the tensor-core packing' % self.K)
-        self.rows = _round(self.Cout, 64)
-        dt = torch.float16 if fwd else F32
-        self.w_nk_hi = torch.empty((self.rows, self.K), dtype=dt, device=self.device)
-        self.w_nk_lo = torch.empty((self.rows, self.K), dtype=dt, device=self.device)
-        self.tmap_hi = _tmap(self.w_nk_hi, self.rows, self.K, self.eb)
-        self.tmap_lo = _tmap(self.w_nk_lo, self.rows, self.K, self.eb)
+    def __init__(self, weight, KH, Cin, Cout):
+        self.src, self.src_shape = weight, (KH, Cin, Cout)
+        self.Cout, self.K = Cin, KH * Cout
+        if self.K % 32 != 0:
+            raise _lib.HDError('BackwardDataPack: K = %d does not fit the TF32 packing' % self.K)
+        self.w_nk_hi = torch.empty((_round(Cin, 64), self.K), dtype=F32, device=weight.device)
+        self.w_nk_lo = torch.empty_like(self.w_nk_hi)
+        self.tmap_hi, self.tmap_lo = weight_tmap(self.w_nk_hi), weight_tmap(self.w_nk_lo)
 
     def repack(self, stream):
         KH, Cin, Cout = self.src_shape
-        check(lib.hd_pack_weight(fptr(self.src), KH, Cin, Cout, self.mode, self.eb, _vp(self.w_nk_hi), _vp(self.w_nk_lo), self.rows, self.K,
-                                 stream), 'hd_pack_weight')
+        check(lib.hd_pack_weight(fptr(self.src), KH, Cin, Cout, _lib.HD_PACK_BACKWARD_DATA, 4, _vp(self.w_nk_hi), _vp(self.w_nk_lo),
+                                 self.w_nk_hi.shape[0], self.K, stream), 'hd_pack_weight')
 
 
 def _tf32_gemm(a, M, K, a_ld, b, out, out_ld, res=None, T=1, KH=1, pad=0, stream=None):
-    """out[M', Cout] = (implicit conv of) a . B on the 3xTF32 tensor-core kernel.  b: a DevicePackedConv (backward-data pack) or an
-    operand tuple (hi, lo, tmap_hi, tmap_lo, Cout) from _bt_operand.  T / KH / pad > 1: a KH x 1 conv over T of M = B clips."""
+    """out[M', Cout] = (implicit conv of) a . B on the 3xTF32 tensor-core kernel.  b: a BackwardDataPack or an operand tuple
+    (hi, lo, tmap_hi, tmap_lo, Cout) from _bt_operand.  T / KH / pad > 1: a KH x 1 conv over T of M = B clips."""
     d = ConvDesc()
     d.in_, d.in_ld = a.data_ptr(), a_ld
     d.n_img, d.H, d.W, d.Cin = M, T, 1, K
     d.Ho, d.Wo, d.KH, d.KW, d.stride, d.pad_t, d.pad_l = T, 1, KH, 1, 1, pad, 0
-    if isinstance(b, DevicePackedConv):
+    if isinstance(b, BackwardDataPack):
         hi, lo, th, tl, Cout = b.w_nk_hi, b.w_nk_lo, b.tmap_hi, b.tmap_lo, b.Cout
     else:
         hi, lo, th, tl, Cout = b
@@ -113,7 +89,7 @@ def _bt_operand(pieces, cols, k_pad, st):
     hi = torch.empty((rows, k_pad), dtype=F32, device=pieces[0][0].device)
     lo = torch.empty_like(hi)
     _stack_t(pieces, cols, k_pad, 1, hi, lo, rows, st)
-    return (hi, lo, _tmap(hi, rows, k_pad, 4), _tmap(lo, rows, k_pad, 4), cols), (hi, lo)
+    return (hi, lo, weight_tmap(hi), weight_tmap(lo), cols), (hi, lo)
 
 
 def _stack_t(pieces, cols, k_pad, mode, hi, lo, out_rows, st):
@@ -509,7 +485,6 @@ class TemporalModel(nn.Module):
             self._params[n] = nn.Parameter(torch.from_numpy(np.ascontiguousarray(a)).to(self.device))
         with torch.cuda.device(self.device):
             self._build()
-        self._seen = {}
         self._bwd_seen = {}
 
     # ---------------------------------------------------------------- packing
@@ -528,8 +503,8 @@ class TemporalModel(nn.Module):
                 bwd = []
                 for k, wn, bn in ((1, n[2], n[3]), (2, n[6], n[7])):
                     Cc = P(wn).shape[2]
-                    blk['conv%d' % k] = DevicePackedConv(P(wn).data, 3, Cc, Cc, bias=P(bn).data, pad=1)
-                    bwd.append(DevicePackedConv(P(wn).data, 3, Cc, Cc, mode=_lib.HD_PACK_BACKWARD_DATA, pad=1))
+                    blk['conv%d' % k] = PackedConv(P(wn).data, self.device, post_shift=P(bn).data, pad=(1, 0), tc='auto')
+                    bwd.append(BackwardDataPack(P(wn).data, 3, Cc, Cc))
                     self._fwd_packs.append((wn, blk['conv%d' % k]))
                     self._bwd_packs.append((wn, bwd[-1]))
                 self.fm_blocks.append(blk)
@@ -541,10 +516,10 @@ class TemporalModel(nn.Module):
             d = W3.shape[1]
             feat = W1.shape[0] - d
             h = {'d': d, 'feat': feat, 'p': [P(x) for x in n], 'W1t': W1[feat:], 'W3': W3, 'b3': b3,
-                 'fc1_phi': DevicePackedConv(W1, 1, feat, 1024, bias=b1),
-                 'fc1_bwd': DevicePackedConv(W1, 1, feat, 1024, mode=_lib.HD_PACK_BACKWARD_DATA),
-                 'fc2': DevicePackedConv(W2, 1, 1024, 1024, bias=b2, post_relu=True),
-                 'fc2_bwd': DevicePackedConv(W2, 1, 1024, 1024, mode=_lib.HD_PACK_BACKWARD_DATA),
+                 'fc1_phi': PackedConv(W1[:feat], self.device, post_shift=b1, tc='auto'),
+                 'fc1_bwd': BackwardDataPack(W1, 1, feat, 1024),
+                 'fc2': PackedConv(W2, self.device, post_shift=b2, post_relu=True, tc='auto'),
+                 'fc2_bwd': BackwardDataPack(W2, 1, 1024, 1024),
                  'W3t': torch.empty((d, 1024), dtype=F32, device=self.device),       # fc3^T  (input gradient of fc3)
                  'W1tT': torch.empty((1024, d), dtype=F32, device=self.device)}      # fc1's theta rows, transposed
             self._fwd_packs += [(n[0], h['fc1_phi']), (n[2], h['fc2'])]
@@ -556,10 +531,13 @@ class TemporalModel(nn.Module):
             self.hal = {}
             for i in (1, 2, 3):
                 wn, bn = HAL_NAMES[2 * i - 2], HAL_NAMES[2 * i - 1]
-                self.hal['fc%d' % i] = DevicePackedConv(P(wn).data, 1, 2048, 2048, bias=P(bn).data, post_relu=i < 3)
-                self.hal['fc%d_bwd' % i] = DevicePackedConv(P(wn).data, 1, 2048, 2048, mode=_lib.HD_PACK_BACKWARD_DATA)
+                self.hal['fc%d' % i] = PackedConv(P(wn).data, self.device, post_shift=P(bn).data, post_relu=i < 3, tc='auto')
+                self.hal['fc%d_bwd' % i] = BackwardDataPack(P(wn).data, 1, 2048, 2048)
                 self._fwd_packs.append((wn, self.hal['fc%d' % i]))
                 self._bwd_packs.append((wn, self.hal['fc%d_bwd' % i]))
+        # the forward packs were written by their constructors: complete them, and repack only what changes from here on
+        sync_packing(self.device)
+        self._seen = {n: self.param(n)._version for n, _ in self._fwd_packs}
 
     def _repack(self, packs, seen):
         st = current_stream()

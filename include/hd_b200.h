@@ -339,9 +339,11 @@ int hd_orth_proj_backward(const float *X, const float *cam, const float *dout, f
  * Deterministic: no floating-point atomics, every reduction in a fixed order; an input gradient's row depends only on that row. */
 enum { HD_PACK_FORWARD = 0, HD_PACK_BACKWARD_DATA = 1 };
 /* Device-side weight packing into the K-major [rows, k_pad] head / remainder layout of hd_conv_gemm's B operand (TMA maps from
- * hd_make_weight_tmap).  w: fp32 [KH, Cin, Cout] (conv HWIO with KW = 1, or FC [in, out] with KH = 1).  elem_bytes 2 = fp16 head /
- * 2^11-scaled remainder (impl 3), 4 = TF32 head / remainder in fp32 storage (impl 1).
- *   HD_PACK_FORWARD:       dst[co, kh*Cin + ci] = W[kh, ci, co]  -- byte for byte nets.PackedConv + f16_split / tf32_split;
+ * hd_make_weight_tmap); the only writer of that layout.  w: fp32 [KH, Cin, Cout]: an FC [in, out] with KH = 1, or, in forward mode, any
+ * HWIO conv with KH*KW passed as KH (backward-data mode: KW = 1).  elem_bytes 2 = fp16 head / 2^11-scaled remainder (impl 3), 4 = TF32
+ * head / remainder in fp32 storage (impl 1).
+ *   HD_PACK_FORWARD:       dst[co, kh*Cin + ci] = W[kh, ci, co]  (hi = RN_f16(w), lo = RN_f16((w - hi) * 2^11); TF32: hi = RN_tf32(w),
+ *                          lo = RN_tf32(w - hi));
  *   HD_PACK_BACKWARD_DATA: dst[ci, k'*Cout + co] = W[KH-1-k', ci, co]  (FC: W^T).
  * Rows / columns past the matrix are zero.  rows % 64 == 0, k_pad % 32 (tf32) / % 64 (fp16) == 0, hi / lo 16-byte aligned. */
 int hd_pack_weight(const float *w, int KH, int Cin, int Cout, int mode, int elem_bytes, void *hi, void *lo, int rows, int k_pad, void *stream);

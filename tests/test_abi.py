@@ -107,7 +107,7 @@ def test_host_logic_without_gpu():
     with pytest.raises(Exception):
         Tester(HMMRConfig(load_path='/nonexistent/model.npz'))
     # TF-style SAME / conv2d_same output sizes used by the plans
-    from human_dynamics_b200.nets import f16_split, tf32_split
+    from oracle.pack_ref import f16_split, tf32_split
     import numpy as np
     w = np.random.RandomState(0).normal(0, 0.05, size=(7, 5)).astype(np.float32)
     hi, lo = f16_split(w)

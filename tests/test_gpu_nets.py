@@ -458,3 +458,33 @@ def test_subsample_is_strided_slice(n, H, C, s):
     torch.cuda.synchronize()
     assert torch.equal(out, x[:, ::s, ::s, :].contiguous())
     assert float(guard.abs().sum()) == 0.0
+
+
+def test_weight_packing_layouts_and_split_precision():
+    """What the tensor-core kernels are fed, as hd_pack_weight writes it on the device: K-major [Cout_pad, K] with K = (ky, kx, ci) (TF
+    HWIO flattened), each weight as an fp16 head + 2^11-scaled fp16 remainder that together carry >= 21 significant bits; conv1's 7x7x3
+    filter re-laid as 8 x 8 x 4 taps with zero weights on the padding taps."""
+    from human_dynamics_b200 import nets
+    rng = np.random.RandomState(3)
+    w = (rng.normal(0, 1, size=(3, 3, 64, 96)) / 24).astype(np.float32)
+    pc = nets.PackedConv(w, torch.device('cuda'), tc='auto')
+    assert pc.tc == 'f16' and (pc.K, pc.K_pad, pc.Cout) == (576, 576, 96)
+    torch.cuda.synchronize()
+    hi, lo = pc.w_nk_hi.cpu().numpy(), pc.w_nk_lo.cpu().numpy()
+    assert hi.shape == lo.shape == (128, 576) and hi.dtype == lo.dtype == np.float16          # rows padded to the 128-wide N tile
+    assert not hi[96:].any() and not lo[96:].any()
+    rec = hi[:96].astype(np.float64) + lo[:96].astype(np.float64) / 2048.0
+    ref = w.reshape(576, 96).T.astype(np.float64)                                            # [co, (ky, kx, ci)]
+    assert np.abs(rec - ref).max() <= np.abs(ref).max() * 2.0 ** -21
+    assert np.array_equal(hi[:96], ref.astype(np.float16))                                   # head = RN_f16(w)
+    assert np.array_equal(pc.w_kn.cpu().numpy(), w.reshape(576, 96))                         # exact-FP32 path keeps TF's [K, Cout]
+    small = nets.PackedConv(w[:, :, :, :64], torch.device('cuda'), tc='auto')
+    assert small.w_nk_hi.shape == (64, 576)                                                  # Cout <= 64: 64-wide tile, no padding rows
+    # conv1 planes
+    w1 = rng.normal(0, 0.1, size=(7, 7, 3, 64)).astype(np.float32)
+    p1 = nets.PackedConv1Planes(w1, np.zeros(64, np.float32), torch.device('cuda'))
+    torch.cuda.synchronize()
+    t = (p1.w_nk_hi.cpu().numpy().astype(np.float64) + p1.w_nk_lo.cpu().numpy().astype(np.float64) / 2048.0).reshape(64, 8, 8, 4)
+    assert not t[:, 7].any() and not t[:, :, 7].any() and not t[:, :, :, 3].any()            # phantom kernel row / pixel / channel
+    assert np.abs(t[:, :7, :7, :3] - w1.transpose(3, 0, 1, 2)).max() <= np.abs(w1).max() * 2.0 ** -21
+    assert p1.plane_width(224) == 232 and p1.plane_width(64) == 72

@@ -138,26 +138,57 @@ def test_grads_match_oracle(weights, model, BT, scale):
     assert len(relaxed) <= len(names) // 4, relaxed
 
 
-def test_device_packing_equals_host_packing(weights):
-    import ctypes as C
-    from human_dynamics_b200 import _lib
-    from human_dynamics_b200.nets import PackedConv
-    from human_dynamics_b200.trainable import DevicePackedConv
-    for name, KH in (('AZ_FC_block2_conv1block_0/weights', 3), ('single_view_ief/3D_module/fc2/weights', 1), ('fc2_res/fc3/weights', 1)):
-        w = np.asarray(weights[name], np.float32)
-        Cin, Cout = w.shape[-2], w.shape[-1]
-        t = torch.from_numpy(np.ascontiguousarray(w)).cuda()
-        dp = DevicePackedConv(t, KH, Cin, Cout)
-        dp.repack(_lib.current_stream())
-        hp = PackedConv(w, 'cuda', tc='f16')
-        assert torch.equal(dp.w_nk_hi.view(torch.int16), hp.w_nk_hi.view(torch.int16))
-        assert torch.equal(dp.w_nk_lo.view(torch.int16), hp.w_nk_lo.view(torch.int16))
-        hp32 = PackedConv(w, 'cuda', tc='tc3')
-        hi, lo = torch.empty_like(hp32.w_nk_hi), torch.empty_like(hp32.w_nk_lo)
-        _lib.check(_lib.lib.hd_pack_weight(_lib.fptr(t), KH, Cin, Cout, 0, 4, C.c_void_p(hi.data_ptr()), C.c_void_p(lo.data_ptr()),
-                                           hi.shape[0], hi.shape[1], _lib.current_stream()))
-        assert torch.equal(hi.view(torch.int32), hp32.w_nk_hi.view(torch.int32))
-        assert torch.equal(lo.view(torch.int32), hp32.w_nk_lo.view(torch.int32))
+def test_device_packing_equals_host_packing(engine, model, weights):
+    """Every tensor-core pack of an engine (ResNet units, the gather and the plane conv1, f_movie, the IEF heads, fc2_res, the SMPL blend
+    and dc GEMMs), of the temporal model's forward, and a tc3 / tc1 TF32 pack, as hd_pack_weight writes them on the device, equal the
+    numpy restatement (oracle/pack_ref.py) byte for byte."""
+    from oracle import pack_ref
+    from human_dynamics_b200.nets import RESNET_BLOCKS, PackedConv
+
+    def same(hi, lo, w_nk, kind):
+        rh, rl = pack_ref.split(w_nk, kind)
+        bits = np.uint16 if kind == 'f16' else np.uint32
+        assert np.array_equal(hi.cpu().numpy().view(bits), rh.view(bits)) and np.array_equal(lo.cpu().numpy().view(bits), rl.view(bits))
+
+    layers = []                                            # (PackedConv, its TF HWIO source or None for its own fp32 copy, expected packing)
+    p = 'resnet_v2_50'
+    layers.append((engine.resnet.conv1, weights[p + '/conv1/weights'], 'f16'))
+    assert engine.resnet.conv1.gather
+    i = 0
+    for b, (_, units, _) in enumerate(RESNET_BLOCKS, start=1):
+        for u in range(1, units + 1):
+            unit = engine.resnet.units[i]
+            for k in ('shortcut', 'conv1', 'conv2', 'conv3'):
+                if k in unit:
+                    layers.append((unit[k], weights['%s/block%d/unit_%d/bottleneck_v2/%s/weights' % (p, b, u, k)], 'f16'))
+            i += 1
+    for i, blk in enumerate(engine.fmovie.blocks):
+        for k in (1, 2):
+            layers.append((blk['conv%d' % k], weights['AZ_FC_block2_conv%dblock_%d/weights' % (k, i)], 'f16'))
+    for dt, head in [(0, engine.ief.main)] + sorted(engine.ief.deltas.items()):
+        q = ('single_view_ief' if dt == 0 else 'single_view_ief_%s%d' % ('future' if dt > 0 else 'past', abs(dt))) + '/3D_module'
+        layers += [(head.fc1_phi, weights[q + '/fc1/weights'][:2048], 'f16'), (head.fc2, weights[q + '/fc2/weights'], 'f16'),
+                   (head.fc3, weights[q + '/fc3/weights'], 'f16')]
+    for k in (1, 2, 3):
+        layers.append((getattr(engine.hal, 'fc%d' % k), weights['fc2_res/fc%d/weights' % k], 'f16'))
+    layers += [(engine.smpl.blend, None, 'f16'), (engine.smpl.grad_state()[2], None, 'tf32')]
+    for tc in ('tc3', 'tc1'):
+        layers.append((PackedConv(weights['single_view_ief/3D_module/fc2/weights'], torch.device('cuda'), tc=tc), None, 'tf32'))
+    for blk in model.fm_blocks:
+        layers += [(blk['conv1'], None, 'f16'), (blk['conv2'], None, 'f16')]
+    for h in model.ief.values():
+        layers += [(h['fc1_phi'], None, 'f16'), (h['fc2'], None, 'f16')]
+    layers += [(model.hal['fc%d' % k], None, 'f16') for k in (1, 2, 3)]
+    assert len(layers) == 1 + 52 + 6 + 9 + 3 + 2 + 2 + 6 + 6 + 3
+    torch.cuda.synchronize()
+    for pc, src, kind in layers:
+        assert pc.tc == kind
+        w = pc.w_kn.cpu().numpy().reshape(pc.KH, pc.KW, pc.Cin, pc.Cout)
+        if src is not None:
+            assert np.array_equal(w, np.asarray(src, np.float32).reshape(w.shape))
+        same(pc.w_nk_hi, pc.w_nk_lo, pack_ref.nk_layout(w, pc.gather), kind)
+    planes = engine.resnet.conv1_planes
+    same(planes.w_nk_hi, planes.w_nk_lo, pack_ref.conv1_planes_layout(weights[p + '/conv1/weights']), 'f16')
 
 
 def test_step_then_forward_equals_fresh_model(weights):
