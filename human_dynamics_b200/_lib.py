@@ -138,6 +138,11 @@ SIGNATURES = {
     'hd_relu_backward': (_i, [_vp, _vp, _vp, _ll, _vp]),
     'hd_fc_small_dgrad': (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp]),
     'hd_add_strided': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _vp]),
+    'hd_dpose_workspace_bytes': (_sz, [_i]),
+    'hd_dpose_trunk_forward': (_i, [_vp] * 10 + [_i, _vp]),
+    'hd_dpose_out_forward': (_i, [_vp] * 4 + [_i, _vp]),
+    'hd_dpose_trunk_backward': (_i, [_vp] * 11 + [_sz, _i, _vp]),
+    'hd_dpose_grad_reduce': (_i, [_vp, _sz, _i, _vp, _vp]),
     'hd_render_workspace_bytes': (_sz, [_i, _i, _i]),
     'hd_render_mesh': (_i, [_vp, _ll, _i, _i, _vp, _i, _vp, _i, C.POINTER(RenderParams), _vp, _i, _vp, _vp, _vp, _sz, _vp]),
 }

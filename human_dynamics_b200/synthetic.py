@@ -210,6 +210,26 @@ def make_hal_weights(seed: int = 6, C: int = 2048, out: dict | None = None) -> d
     return w
 
 
+DPOSE_LAYERS = [('D_conv1', (1, 1, 9, 32)), ('D_conv2', (1, 1, 32, 32))] + \
+    [('pose_out_j%d' % j, (32, 1)) for j in range(23)] + \
+    [('D_alljoints_fc1', (736, 1024)), ('D_alljoints_fc2', (1024, 1024)), ('D_alljoints_out', (1024, 1))]
+
+
+def make_dpose_weights(seed: int = 0, bias_scale: float = 0.0) -> dict:
+    """D_pose variables (discriminators.py), in the order the reference creates them: slim's default initialisation, Xavier-uniform
+    weights (fan_in = kh*kw*cin, fan_out = kh*kw*cout) and zero biases; bias_scale > 0 draws the biases from U(-bias_scale, bias_scale)
+    instead, so tests exercise them."""
+    rng = np.random.RandomState(seed)
+    w = {}
+    for name, shape in DPOSE_LAYERS:
+        fan_in, fan_out = int(np.prod(shape[:-1])), int(np.prod(shape[:-2])) * shape[-1]
+        limit = np.sqrt(6.0 / (fan_in + fan_out))
+        w['D_pose/%s/weights' % name] = rng.uniform(-limit, limit, size=shape).astype(np.float32)
+        b = rng.uniform(-bias_scale, bias_scale, size=shape[-1]) if bias_scale > 0 else np.zeros(shape[-1])
+        w['D_pose/%s/biases' % name] = b.astype(np.float32)
+    return w
+
+
 def make_synthetic_weights(seed: int = 1, num_conv_layers: int = 3, delta_t_values=(-5, 5),
                            with_hal: bool = False) -> dict:
     """Full HMMR inference weight dict (TF variable names)."""

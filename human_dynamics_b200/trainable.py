@@ -60,6 +60,31 @@ class BackwardDataPack(object):
                                  self.w_nk_hi.shape[0], self.K, stream), 'hd_pack_weight')
 
 
+class TransposedCopy(object):
+    """dst = src^T in fp32 on the device (src [rows, cols] row-major, dst [cols, rows]): a small layer's input-gradient operand."""
+
+    def __init__(self, src, dst):
+        self.src, self.dst = src, dst
+
+    def repack(self, stream):
+        src, dst = self.src, self.dst
+        check(lib.hd_transpose_split(fptr(src), src.shape[0], src.shape[1], src.shape[1], 0, _vp(dst), None, dst.shape[1], dst.shape[0],
+                                     dst.shape[1], stream), 'hd_transpose_split')
+
+
+def repack_stale(packs, seen, param):
+    """Repack on the current stream every (name, pack) of `packs` whose parameter param(name) was changed in place (optimizer.step(),
+    copy_) since `seen` recorded its version counter, and record the new versions.  Returns the number of stale parameters."""
+    st = current_stream()
+    stale = {n for n, _ in packs if seen.get(n) != param(n)._version}
+    for n, pk in packs:
+        if n in stale:
+            pk.repack(st)
+    for n in stale:
+        seen[n] = param(n)._version
+    return len(stale)
+
+
 def _tf32_gemm(a, M, K, a_ld, b, out, out_ld, res=None, T=1, KH=1, pad=0, stream=None):
     """out[M', Cout] = (implicit conv of) a . B on the 3xTF32 tensor-core kernel.  b: a BackwardDataPack or an operand tuple
     (hi, lo, tmap_hi, tmap_lo, Cout) from _bt_operand.  T / KH / pad > 1: a KH x 1 conv over T of M = B clips."""
@@ -523,7 +548,8 @@ class TemporalModel(nn.Module):
                  'W3t': torch.empty((d, 1024), dtype=F32, device=self.device),       # fc3^T  (input gradient of fc3)
                  'W1tT': torch.empty((1024, d), dtype=F32, device=self.device)}      # fc1's theta rows, transposed
             self._fwd_packs += [(n[0], h['fc1_phi']), (n[2], h['fc2'])]
-            self._bwd_packs += [(n[0], h['fc1_bwd']), (n[2], h['fc2_bwd']), (n[4], ('W3t', h)), (n[0], ('W1tT', h))]
+            self._bwd_packs += [(n[0], h['fc1_bwd']), (n[2], h['fc2_bwd']), (n[4], TransposedCopy(W3, h['W3t'])),
+                                (n[0], TransposedCopy(h['W1t'], h['W1tT']))]
             self.ief['main' if dt == 0 else dt] = h
         self._zeros = torch.zeros(96, dtype=F32, device=self.device)
         self.hal = None
@@ -540,22 +566,7 @@ class TemporalModel(nn.Module):
         self._seen = {n: self.param(n)._version for n, _ in self._fwd_packs}
 
     def _repack(self, packs, seen):
-        st = current_stream()
-        stale = {n for n, _ in packs if seen.get(n) != self.param(n)._version}
-        for n, pk in packs:
-            if n not in stale:
-                continue
-            if isinstance(pk, tuple):
-                which, h = pk
-                src = h['W3'] if which == 'W3t' else h['W1t']
-                dst = h[which]
-                check(lib.hd_transpose_split(fptr(src), src.shape[0], src.shape[1], src.shape[1], 0, _vp(dst), None, dst.shape[1],
-                                             dst.shape[0], dst.shape[1], st), 'hd_transpose_split')
-            else:
-                pk.repack(st)
-        for n in stale:
-            seen[n] = self.param(n)._version
-        return len(stale)
+        return repack_stale(packs, seen, self.param)
 
     def sync_packs(self):
         """Repack every forward weight whose parameter changed since it was last packed (called by each forward).  Returns the count."""

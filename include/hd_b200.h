@@ -374,6 +374,29 @@ int hd_fc_small_dgrad(const float *g, int g_ld, const float *Wt, int K, int D, c
 /* out[r, c] = a[r, c] + b[r, c] at independent row strides (out may alias a or b): gradient accumulation of the IEF glue. */
 int hd_add_strided(const float *a, long long lda, const float *b, long long ldb, float *out, long long ldo, int rows, int cols, void *stream);
 
+/* ---- Adversarial pose prior D_pose (src/discriminators.py; csrc/dpose.cu) ----
+ * Input x [N, 23, 9]: the rotation matrices of the 23 non-root joints.  Variables (TF HWIO / [in, out], fp32):  D_conv1 W1 [9, 32], b1;
+ * D_conv2 W2 [32, 32], b2; the heads pose_out_j0..22 stacked as wj [23, 32], bj [23]; D_alljoints_fc1 [736, 1024], fc2 [1024, 1024]
+ * (both on hd_conv_gemm); D_alljoints_out w_out [1024], b_out [1].  Output logits [N, 24] (row stride 24):
+ *   h1 = relu(x W1 + b1), h2 = relu(h1 W2 + b2)  [N, 23, 32]        hd_dpose_trunk_forward (also logits[:, j] = h2[:, j] . wj[j] + bj[j])
+ *   f1 = relu(h2 [N, 736] . Wfc1 + bfc1), f2 = relu(f1 . Wfc2 + bfc2)  hd_conv_gemm (h2 is its input as written, in_ld 736)
+ *   logits[:, 23] = f2 . w_out + b_out                             hd_dpose_out_forward
+ * Backward of an upstream g [N, 24]: df2 = g[:, 23] w_out^T * (f2 > 0) (hd_fc_small_dgrad, D = 1), df1 and dflat [N, 736] by hd_conv_gemm
+ * (3xTF32) dX with hd_relu_backward between them, then hd_dpose_trunk_backward: dx [N, 23, 9] (nullable) and, with a workspace of
+ * hd_dpose_workspace_bytes(N), per-block partial sums that hd_dpose_grad_reduce sums into the packed gradient grad[HD_DPOSE_GRAD_FLOATS]:
+ *   dW1 [9,32] @0 | db1 @288 | dW2 [32,32] @320 | db2 @1344 | dwj [23,32] @1376 | dbj @2112 | dw_out [1024] @2135 | db_out @3159.
+ * Deterministic: a row's logits / dx depend on that row only; weight sums use a fixed partition and order, no atomics.
+ * HD_ERR_INVALID: a null pointer, N <= 0, a workspace smaller than hd_dpose_workspace_bytes(N), or unaligned h / w_out (16 bytes). */
+enum { HD_DPOSE_JOINTS = 23, HD_DPOSE_GRAD_FLOATS = 3160 };
+size_t hd_dpose_workspace_bytes(int N);
+int hd_dpose_trunk_forward(const float *x, const float *W1, const float *b1, const float *W2, const float *b2, const float *wj,
+                           const float *bj, float *h1, float *h2, float *logits, int N, void *stream);
+int hd_dpose_out_forward(const float *h, const float *w_out, const float *b_out, float *logits, int N, void *stream);
+/* dflat = d flatten(h2) from fc1's dX; hf = f2 (read with ws); x is read with ws, W1 with dx. */
+int hd_dpose_trunk_backward(const float *x, const float *h1, const float *h2, const float *dflat, const float *g, const float *hf,
+                            const float *W1, const float *W2, const float *wj, float *dx, void *ws, size_t ws_bytes, int N, void *stream);
+int hd_dpose_grad_reduce(const void *ws, size_t ws_bytes, int N, float *grad, void *stream);
+
 /* ---- Mesh rendering (the visualiser of src/util/render/nmr_renderer.py:43-240: NMR with camera_mode='look_at',
  * perspective=False, anti_aliasing and fill_back on), one colour per mesh.  The model is R1-R8 of oracle/render_ref.py:
  *   x = s*(X + tx), y = -s*(Y + ty), z = Z - eye_z  (R1); a 2S x 2S sample grid whose sample (r, c) sits at image
