@@ -78,6 +78,28 @@ class RenderParams(C.Structure):
     ]
 
 
+HD_LOSS_KP_L1, HD_LOSS_MSE_ROWS = 0, 1
+HD_LOSS_KP_CAMERA, HD_LOSS_KP_OPTCAM, HD_LOSS_KP_RAW = 0, 1, 2
+HD_LOSS_MAX_TERMS, HD_LOSS_MAX_GRADS = 64, 16
+
+
+class LossTerm(C.Structure):
+    """Mirror of hd_loss_term."""
+    _fields_ = [
+        ('kind', C.c_int), ('proj', C.c_int), ('B', C.c_int), ('Tw', C.c_int), ('p_t0', C.c_int), ('q_t0', C.c_int),
+        ('p_T', C.c_int), ('q_T', C.c_int), ('K', C.c_int), ('D', C.c_int),
+        ('p', C.c_void_p), ('p_clip', C.c_longlong), ('p_frame', C.c_longlong),
+        ('q', C.c_void_p), ('q_clip', C.c_longlong), ('q_frame', C.c_longlong),
+        ('cam', C.c_void_p), ('cam_clip', C.c_longlong), ('cam_frame', C.c_longlong),
+        ('w', C.c_void_p), ('cam_out', C.c_void_p), ('scale', C.c_float),
+    ]
+
+
+class LossGrad(C.Structure):
+    """Mirror of hd_loss_grad."""
+    _fields_ = [('src', C.c_void_p), ('grad', C.c_void_p), ('numel', C.c_longlong)]
+
+
 # name -> (restype, argtypes); must list every symbol include/hd_b200.h declares.
 _vp, _i, _ll, _f, _sz = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_size_t
 SIGNATURES = {
@@ -143,6 +165,9 @@ SIGNATURES = {
     'hd_dpose_out_forward': (_i, [_vp] * 4 + [_i, _vp]),
     'hd_dpose_trunk_backward': (_i, [_vp] * 11 + [_sz, _i, _vp]),
     'hd_dpose_grad_reduce': (_i, [_vp, _sz, _i, _vp, _vp]),
+    'hd_loss_workspace_bytes': (_sz, [_vp, _i]),
+    'hd_loss_forward': (_i, [_vp, _i, _vp, _vp, _sz, _vp]),
+    'hd_loss_backward': (_i, [_vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
     'hd_render_workspace_bytes': (_sz, [_i, _i, _i]),
     'hd_render_mesh': (_i, [_vp, _ll, _i, _i, _vp, _i, _vp, _i, C.POINTER(RenderParams), _vp, _i, _vp, _vp, _vp, _sz, _vp]),
 }

@@ -255,3 +255,44 @@ def make_smpl_inputs(n: int, seed: int = 0, zero_pose: bool = False):
     beta = rng.normal(0, 1.0, size=(n, 10)).astype(np.float32)
     theta = np.zeros((n, 72), np.float32) if zero_pose else rng.normal(0, 0.3, size=(n, 72)).astype(np.float32)
     return beta, theta
+
+
+def make_loss_inputs(obj, seed: int = 0, flip_frame: bool = True, dtype=np.float32) -> dict:
+    """Seeded inputs of an objective.Objective (numpy, its `shapes()`): cameras with scale in [0.6, 1.4], keypoint visibility mixing
+    0, 1 and 0.5, the has_3d patterns [joints, smpl] cycling through (1, 0), (0, 1), (0, 0), (1, 1), and, with `flip_frame`, one frame
+    of the first delta set whose prediction is the label mirrored (its optimal scale falls to the 0.7 clip)."""
+    from .objective import Objective
+    assert isinstance(obj, Objective)
+    rng = np.random.RandomState(seed)
+    S, B, T, K = len(obj.sets), obj.B, obj.T, obj.K
+    out = {}
+    om = rng.normal(0, 0.3, size=(S, B, T, 85))
+    om[..., 0] = rng.uniform(0.6, 1.4, size=(S, B, T))
+    out['omega'] = om
+    # labels move slowly in time and the predictions are scaled, shifted, noisy copies, so that the optimal cameras of every window
+    # are mostly inside the scale clip
+    lab = rng.normal(0, 0.5, size=(B, 1, K, 3)) + rng.normal(0, 0.05, size=(B, T, K, 3))
+    js = rng.normal(0, 0.5, size=(S, B, T, K, 3))
+    js[..., :2] = lab[None, ..., :2] / rng.uniform(0.8, 1.6, size=(S, B, T, 1, 1)) + rng.normal(0, 0.1, size=(S, B, T, K, 2))
+    out['joints'] = js
+    out['rots'] = rng.normal(0, 0.5, size=(S, B, T, 216))
+    lab[..., 2] = rng.choice([0., 1., 1., 0.5], size=(B, T, K))
+    out['labels'] = lab
+    out['gt_rots'] = rng.normal(0, 0.5, size=(B, T, 216))
+    out['gt_shape'] = rng.normal(0, 0.5, size=(B, 10))
+    out['gt3ds'] = rng.normal(0, 0.5, size=(B, T, 14, 3))
+    pat = np.array([[1, 0], [0, 1], [0, 0], [1, 1]], np.float64)
+    has = pat[np.arange(B) % 4]
+    out['w_joints'], out['w_smpl'] = has[:, 0].copy(), has[:, 1].copy()
+    if 'strips' in obj.inputs:
+        out['strips'] = rng.normal(0, 1, size=(B, T, 2048))
+        out['pred_strips'] = out['strips'] + rng.normal(0, 0.3, size=(B, T, 2048))
+    if flip_frame and obj.cam_terms:
+        i, (group, dt) = obj.cam_terms[0]
+        s = obj.sets.index((group, dt))
+        t = obj.terms[i]
+        pf, qf = t['p'][4], t['q'][4]
+        out['labels'][0, qf, :, 2] = 1.
+        out['joints'][s, 0, pf, :, 0] = -out['labels'][0, qf, :, 0]
+        out['joints'][s, 0, pf, :, 1] = out['labels'][0, qf, :, 1]
+    return {k: np.ascontiguousarray(v, dtype=dtype) for k, v in out.items()}

@@ -397,6 +397,54 @@ int hd_dpose_trunk_backward(const float *x, const float *h1, const float *h2, co
                             const float *W1, const float *W2, const float *wj, float *dx, void *ws, size_t ws_bytes, int N, void *stream);
 int hd_dpose_grad_reduce(const void *ws, size_t ws_bytes, int N, float *grad, void *stream);
 
+/* ---- The trainer's encoder objective (src/trainer_sequence_fc.py:791-1018, src/ops.py, src/tf_smpl/projection.py; csrc/losses.cu) ----
+ * One objective is a host array of term descriptors.  A term reads B clips x a window of Tw frames: frame f of clip b of a tensor X is
+ * the row X + b * X_clip + (X_t0 + f) * X_frame (strides in floats; X_T = frames per clip, for the bound check).  Two kinds:
+ *   HD_LOSS_KP_L1     sum_{b,f,k,c<2} v * |xhat - x| / (2 * #{v != 0}),  labels q [K, 3] = (x, y, v) per frame, p [K, D] (xy first).
+ *                     xhat = s * (p_xy + t) with cam = (s, tx, ty) read at p's frame (HD_LOSS_KP_CAMERA, compute_loss_e_kp after
+ *                     batch_orth_proj_idrot), the optimal camera of procrustes2d_vis over the points with v > 0 (HD_LOSS_KP_OPTCAM: 1e-6 I
+ *                     before the 2 x 2 inverse, scale clipped to [0.7, 10], no gradient through it; written to cam_out [B, Tw, 3] when
+ *                     given), or p_xy itself (HD_LOSS_KP_RAW).  A frame without a visible point in an OPTCAM term contributes 0 to value
+ *                     and gradient and gets the camera (0.7, 0, 0) (the reference's value is NaN there).
+ *   HD_LOSS_MSE_ROWS  scale * sum_{b,f,i<D} w[b] * (p - q)^2 / (D * #{rows with w[b] != 0}),  w NULL = 1, q NULL = 0; proj = 1 aligns
+ *                     both rows by the pelvis first (rows of D / 3 >= 14 joints x 3, LSP hips 2 and 3: align_by_pelvis).
+ * A count of 0 gives a value of 0.  The counts come from the weights alone.
+ * hd_loss_forward writes values[n] with two launches (fixed-partition partial sums, fixed-order reduce) for any n; the workspace of
+ * hd_loss_workspace_bytes(terms, n) (8-byte aligned) keeps the counts for the backward.  hd_loss_backward (one launch) WRITES grad for every target
+ * {src, grad, numel}: for each element of src, the sum over the terms whose p / q (MSE) / cam (KP_CAMERA) lie inside src, in term order,
+ * of dvalues[i] * d value_i / d element (dvalues: device, n floats); KP_L1 labels are constants (a target over them gets 0).  A target must be laid out like src (same strides); an element no
+ * term reads gets 0.  L1's gradient at a residual of exactly 0 is 0.  Deterministic, no atomics; a frame's gradient depends only on
+ * its own data, the counts and dvalues.  HD_ERR_INVALID (checked before any launch): null pointers, n outside [1, HD_LOSS_MAX_TERMS],
+ * more than HD_LOSS_MAX_GRADS targets, B / Tw / D / K <= 0, a window that overruns X_T, pelvis alignment on rows of fewer than 14
+ * joints, a gradient through a side with frame stride 0, or a workspace smaller than hd_loss_workspace_bytes (which is 0 for an
+ * invalid list). */
+enum { HD_LOSS_KP_L1 = 0, HD_LOSS_MSE_ROWS = 1 };
+enum { HD_LOSS_KP_CAMERA = 0, HD_LOSS_KP_OPTCAM = 1, HD_LOSS_KP_RAW = 2 };
+enum { HD_LOSS_MAX_TERMS = 64, HD_LOSS_MAX_GRADS = 16 };
+typedef struct {
+  int kind, proj;                 /* HD_LOSS_KP_L1: HD_LOSS_KP_*;  HD_LOSS_MSE_ROWS: 1 = pelvis alignment, 0 = none */
+  int B, Tw, p_t0, q_t0, p_T, q_T;
+  int K, D;                       /* KP_L1: keypoints, floats per keypoint of p;  MSE_ROWS: K unused, floats per row */
+  const float *p;
+  long long p_clip, p_frame;
+  const float *q;
+  long long q_clip, q_frame;
+  const float *cam;               /* KP_CAMERA only */
+  long long cam_clip, cam_frame;
+  const float *w;                 /* MSE_ROWS: per-clip weights [B] or NULL */
+  float *cam_out;                 /* KP_OPTCAM: [B, Tw, 3] or NULL */
+  float scale;                    /* MSE_ROWS: the term's factor (0.5 for compute_loss_mse / _e_smooth); KP_L1: 1 */
+} hd_loss_term;
+typedef struct {
+  const float *src;
+  float *grad;
+  long long numel;
+} hd_loss_grad;
+size_t hd_loss_workspace_bytes(const hd_loss_term *terms, int n);
+int hd_loss_forward(const hd_loss_term *terms, int n, float *values, void *ws, size_t ws_bytes, void *stream);
+int hd_loss_backward(const hd_loss_term *terms, int n, const hd_loss_grad *grads, int n_grads, const float *dvalues, const void *ws,
+                     size_t ws_bytes, void *stream);
+
 /* ---- Mesh rendering (the visualiser of src/util/render/nmr_renderer.py:43-240: NMR with camera_mode='look_at',
  * perspective=False, anti_aliasing and fill_back on), one colour per mesh.  The model is R1-R8 of oracle/render_ref.py:
  *   x = s*(X + tx), y = -s*(Y + ty), z = Z - eye_z  (R1); a 2S x 2S sample grid whose sample (r, c) sits at image

@@ -2,7 +2,7 @@
 
 `OmegasPred` stores B x T x 85 predictions [cams 3 | poses 72 | shapes 10] and computes SMPL + keypoint
 projection for all of them at once (omega.py:197-342).  Tensors are float32 CUDA torch.Tensors.
-`OmegasGt` (training-only, omega.py:161-194) is out of scope.
+`OmegasGt` (omega.py:161-194) holds the ground truth the training losses read.
 """
 import torch
 
@@ -59,6 +59,30 @@ class Omegas(object):
         """Gathers a subset over time (omega.py:144-158)."""
         idx = torch.as_tensor(indices, dtype=torch.long, device=values.device)
         return values.index_select(1, idx)
+
+
+class OmegasGt(Omegas):
+    """Ground-truth omegas (omega.py:161-194): poses_aa (B,T,24,3) or (B,T,72), shapes (B,10), joints (B,T,14,3), kps (B,T,K,3)."""
+
+    def __init__(self, config, poses_aa, shapes, joints, kps, batch_size=None):
+        from src.tf_smpl.batch_lbs import batch_rodrigues
+        from src.ops import compute_deltas_batched
+        super(OmegasGt, self).__init__(config, batch_size=batch_size)
+        self.length = poses_aa.shape[1]
+        self.poses_aa = poses_aa
+        self.poses_rot = batch_rodrigues(poses_aa.reshape(-1, 3)).reshape(self.batch_size, -1, 24, 3, 3)
+        self.shapes = shapes
+        self.joints = joints
+        self.kps = kps
+        self.deltas_rot = compute_deltas_batched(self.poses_rot[:, :-1], self.poses_rot[:, 1:])
+
+    def get_shapes(self, t=None):
+        if t is None:
+            return self.shapes.unsqueeze(1).expand(-1, self.length, -1)
+        return self.shapes
+
+    def get_deltas_aa(self, t=None):
+        raise Exception('No axis-aligned deltas.')
 
 
 class OmegasPred(Omegas):
