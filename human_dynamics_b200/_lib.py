@@ -100,6 +100,21 @@ class LossGrad(C.Structure):
     _fields_ = [('src', C.c_void_p), ('grad', C.c_void_p), ('numel', C.c_longlong)]
 
 
+HD_AUG_SRC_U8, HD_AUG_ROTATE, HD_AUG_FLIP = 1, 2, 4
+
+
+class TubeAugArgs(C.Structure):
+    """Mirror of hd_tube_aug_args."""
+    _fields_ = [
+        ('frames', C.c_void_p), ('F', C.c_int), ('H', C.c_int), ('W', C.c_int), ('flags', C.c_int),
+        ('trans', C.c_void_p), ('scale', C.c_void_p), ('rot', C.c_void_p), ('flip', C.c_void_p),
+        ('labels', C.c_void_p), ('K', C.c_int), ('centers', C.c_void_p), ('poses', C.c_void_p), ('gt3ds', C.c_void_p),
+        ('S', C.c_int), ('trans_max', C.c_int), ('geom', C.c_void_p),
+        ('labels_out', C.c_void_p), ('centers_out', C.c_void_p), ('poses_out', C.c_void_p), ('gt3ds_out', C.c_void_p),
+        ('crops', C.c_void_p), ('plane_hi', C.c_void_p), ('plane_lo', C.c_void_p), ('WP', C.c_int),
+    ]
+
+
 # name -> (restype, argtypes); must list every symbol include/hd_b200.h declares.
 _vp, _i, _ll, _f, _sz = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_size_t
 SIGNATURES = {
@@ -169,6 +184,7 @@ SIGNATURES = {
     'hd_loss_forward': (_i, [_vp, _i, _vp, _vp, _sz, _vp]),
     'hd_loss_backward': (_i, [_vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
     'hd_render_workspace_bytes': (_sz, [_i, _i, _i]),
+    'hd_tube_augment': (_i, [C.POINTER(TubeAugArgs), _vp]),
     'hd_render_mesh': (_i, [_vp, _ll, _i, _i, _vp, _i, _vp, _i, C.POINTER(RenderParams), _vp, _i, _vp, _vp, _vp, _sz, _vp]),
 }
 

@@ -345,21 +345,11 @@ __global__ void __launch_bounds__(128) global_rigid_kernel(Tree tree, const floa
   }
 }
 
-// batch_rot2aa (src/tf_smpl/batch_lbs.py:63-105): theta = acos(clip((tr R - 1)/2)), axis = (R21-R12, R02-R20, R10-R01) / norm,
-// left un-normalised where |theta| < 1e-5 (tf.where in the reference), result theta * axis.
+// batch_rot2aa (src/tf_smpl/batch_lbs.py:63-105), one thread per matrix (hd_smpl::rot2aa).
 __global__ void rot2aa_kernel(const float *__restrict__ Rs, float *__restrict__ aa, int M) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= M) return;
-  const float *R = Rs + (size_t)i * 9;
-  float c = 0.5f * ((R[0] + R[4] + R[8]) - 1.0f);
-  c = fminf(fmaxf(c, -1.0f), 1.0f);
-  const float theta = acosf(c);
-  const float m21 = R[7] - R[5], m02 = R[2] - R[6], m10 = R[3] - R[1];
-  const float denom = sqrtf(m21 * m21 + m02 * m02 + m10 * m10);
-  const bool tiny = fabsf(theta) < 0.00001f;
-  aa[(size_t)i * 3 + 0] = theta * (tiny ? m21 : m21 / denom);
-  aa[(size_t)i * 3 + 1] = theta * (tiny ? m02 : m02 / denom);
-  aa[(size_t)i * 3 + 2] = theta * (tiny ? m10 : m10 / denom);
+  hd_smpl::rot2aa(Rs + (size_t)i * 9, aa + (size_t)i * 3);
 }
 
 __global__ void orth_proj_kernel(const float *__restrict__ X, const float *__restrict__ cam, float *__restrict__ out,

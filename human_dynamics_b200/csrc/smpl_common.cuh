@@ -43,6 +43,20 @@ __device__ __forceinline__ void rodrigues(float tx, float ty, float tz, float *R
   R[8] = c + oc * (rz * rz);
 }
 
+// batch_rot2aa (src/tf_smpl/batch_lbs.py:63-105): theta = acos(clip((tr R - 1)/2)), axis = (R21-R12, R02-R20, R10-R01) / norm,
+// left un-normalised where |theta| < 1e-5 (tf.where in the reference), result theta * axis.
+__device__ __forceinline__ void rot2aa(const float *R, float *aa) {
+  float c = 0.5f * ((R[0] + R[4] + R[8]) - 1.0f);
+  c = fminf(fmaxf(c, -1.0f), 1.0f);
+  const float theta = acosf(c);
+  const float m21 = R[7] - R[5], m02 = R[2] - R[6], m10 = R[3] - R[1];
+  const float denom = sqrtf(m21 * m21 + m02 * m02 + m10 * m10);
+  const bool tiny = fabsf(theta) < 0.00001f;
+  aa[0] = theta * (tiny ? m21 : m21 / denom);
+  aa[1] = theta * (tiny ? m02 : m02 / denom);
+  aa[2] = theta * (tiny ? m10 : m10 / denom);
+}
+
 // Forward kinematics over the tree, one lane per joint (lanes >= 24 idle but take part in shuffles).
 // In: local rotation Rl, rest joint J (per lane).  Out: world rotation Rw, world translation tw.
 __device__ __forceinline__ void fk_chain(const Tree &tree, int lane, const float *Rl, const float *J,

@@ -154,6 +154,52 @@ int hd_process_image(const unsigned char *frames, int N, int H, int W, const int
  * return a crop smaller than img_size x img_size. */
 int hd_crop_geometry(int H, int W, const double *bbox, int img_size, int *geom, int *center, int *start_pt);
 
+/* ---- training-time tube augmentation: TubePreprocessor.preprocess_image (src/util/tube_augmentation.py:114-186 with
+ * src/util/data_utils.py's jitter_center, jitter_scale, pad_image_edge, rotate_img, flip_image), per frame, F frames of one
+ * source size H x W from any number of tubes.  Two launches, no host synchronisation:
+ *   1. one thread per frame: centre + trans; sf = 2^scale; Hs = int(float(H) * sf), Ws likewise; keypoints and centre scaled by
+ *      Hs/H, Ws/W (centre truncated); the S x S slice of the edge-padded scaled image around it; with HD_AUG_ROTATE, rotate_img by
+ *      rot[f] (keypoints about (S/2, S/2), gt3d about its scalar mean, pose[:3] <- rot2aa(R^T rodrigues(pose[:3]))); where flip[f]
+ *      is set, flip_image (25-keypoint swap, reflect_pose, reflect_joints3d); labels -> [2x/S - 1, 2y/S - 1, vis > 0] * (vis > 0).
+ *      Writes the frame's geometry row and the transformed labels.
+ *   2. one thread per output pixel: the crop straight from the source frame (TF 1.x resize_bilinear taps, edge replication by
+ *      clamping into the scaled image, contrib.image.rotate's bilinear taps with zero fill, the width mirror), then (v - 0.5) * 2.
+ * frames: uint8 [F,H,W,3] (HD_AUG_SRC_U8; value = u8 / 255 in float32) or float32 [F,H,W,3] in [0, 1].  Walks: trans int32 [F,2]
+ * (x, y), scale float32 [F], rot float32 [F] (HD_AUG_ROTATE only, else ignored), flip int32 [F] (HD_AUG_FLIP only, else ignored).
+ * Labels: labels float32 [F,3,K] (x row, y row, visibility row), centers int32 [F,2] (x, y), poses float32 [F,72], gt3ds float32
+ * [F,14,3]; the *_out arrays have the same shapes (centers_out = the scaled jittered centre, the reference's `centers`).
+ * geom int32 [F,16] (16-byte aligned): {Hs, Ws, cx, cy, x0, y0, flip, 0} then, as float bits, the rotation's projective
+ * transform a0..a5 and the resize steps H/Hs, W/Ws; (x0, y0) = the crop's top-left corner in the scaled image.
+ * Outputs: crops float32 [F,S,S,3] in [-1, 1] and / or plane_hi / plane_lo, the padded RGBX fp16 planes [F,S+6,WP,4] of
+ * hd_pack_conv1_planes (border cleared once by the caller).  A centre whose crop leaves the edge-padded image (where the reference's
+ * tf.slice fails) is not an error here: the crop keeps clamping into the scaled image.  trans_max only enters the keypoints' float
+ * rounding (the reference pads by S/2 + trans_max + 50 before it slices).
+ * HD_ERR_INVALID (before any launch): a null pointer, F, H, W, K or S <= 0, S odd, trans_max < 0, an unknown flag bit, HD_AUG_FLIP
+ * with K != 25, or a bad plane layout (WP even and >= S + 8, 16-byte aligned planes). */
+#define HD_AUG_SRC_U8 1
+#define HD_AUG_ROTATE 2
+#define HD_AUG_FLIP 4
+typedef struct {
+  const void *frames;
+  int F, H, W, flags;
+  const int *trans;
+  const float *scale, *rot;
+  const int *flip;
+  const float *labels;
+  int K;
+  const int *centers;
+  const float *poses, *gt3ds;
+  int S, trans_max;
+  int *geom;
+  float *labels_out;
+  int *centers_out;
+  float *poses_out, *gt3ds_out;
+  float *crops;
+  void *plane_hi, *plane_lo;
+  int WP;
+} hd_tube_aug_args;                                   /* host struct */
+int hd_tube_augment(const hd_tube_aug_args *a, void *stream);
+
 /* ---- f_movie GroupNorm statistics (tf.contrib.layers.group_norm at src/models.py:155,188) ----
  * x [B,T,C]; per (clip, group) mean / biased variance over T*(C/groups) elements (two-pass);
  * gain[b,c] = rsqrt(var+eps)*gamma[c]; offset[b,c] = beta[c] - mean*gain[b,c]. */
