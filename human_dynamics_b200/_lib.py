@@ -115,6 +115,20 @@ class TubeAugArgs(C.Structure):
     ]
 
 
+HD_EVAL_KP, HD_EVAL_KP_PA, HD_EVAL_KP_PCK, HD_EVAL_JOINTS, HD_EVAL_JOINTS_PA, HD_EVAL_ACCEL, HD_EVAL_ACCEL_ERROR, HD_EVAL_VIS3D = range(8)
+HD_EVAL_COLS = 8
+
+
+class EvalFramesArgs(C.Structure):
+    """Mirror of hd_eval_frames_args."""
+    _fields_ = [
+        ('N', C.c_int), ('n_seq', C.c_int), ('seq_start', C.c_void_p), ('K', C.c_int), ('J', C.c_int),
+        ('kps_gt', C.c_void_p), ('kps_gt_ld', C.c_longlong), ('kps_pred', C.c_void_p), ('kps_pred_ld', C.c_longlong),
+        ('joints_gt', C.c_void_p), ('joints_gt_ld', C.c_longlong), ('joints_pred', C.c_void_p), ('joints_pred_ld', C.c_longlong),
+        ('img_size', C.c_float), ('min_visible', C.c_int), ('out', C.c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); must list every symbol include/hd_b200.h declares.
 _vp, _i, _ll, _f, _sz = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_size_t
 SIGNATURES = {
@@ -186,6 +200,9 @@ SIGNATURES = {
     'hd_render_workspace_bytes': (_sz, [_i, _i, _i]),
     'hd_tube_augment': (_i, [C.POINTER(TubeAugArgs), _vp]),
     'hd_render_mesh': (_i, [_vp, _ll, _i, _i, _vp, _i, _vp, _i, C.POINTER(RenderParams), _vp, _i, _vp, _vp, _vp, _sz, _vp]),
+    'hd_eval_frames': (_i, [C.POINTER(EvalFramesArgs), _vp]),
+    'hd_eval_mesh_tpose': (_i, [C.POINTER(SmplConsts), _vp, _i, _vp, _i, _i, _vp, _vp]),
+    'hd_eval_verts_error': (_i, [_vp, _ll, _vp, _ll, _i, _i, _vp, _vp]),
 }
 
 

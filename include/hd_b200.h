@@ -517,6 +517,51 @@ int hd_render_mesh(const float *verts, long long verts_ld, int N, int V, const i
                    unsigned char *out_rgb /* [N,S,S,3] */, float *out_alpha /* [N,S,S], nullable */, void *ws, size_t ws_bytes,
                    void *stream);
 
+/* ---- Evaluation (the per-frame metrics of src/evaluation/eval.py compute_errors_batched over eval_util.py) ----
+ * hd_eval_frames: one launch, one warp per frame, for every frame of n_seq tubes laid end to end (device seq_start[n_seq + 1],
+ * seq_start[0] = 0, non-decreasing, seq_start[n_seq] = N).  Writes one fp64 row of HD_EVAL_COLS per frame into out [N, HD_EVAL_COLS]:
+ *   KP, KP_PA, KP_PCK   mean pixel error over the visible keypoints (vis != 0), the same after the optimal 2-D camera (eps 1e-6 I,
+ *                       scale = trace(A^-1 x^T y) / 2, trans = mu2 / scale - mu1) and the fraction of aligned errors < 0.05 * img_size;
+ *                       NaN when no keypoint or fewer than min_visible keypoints are visible.  The prediction is brought to pixels as
+ *                       ((k + 1) * 0.5) * img_size in fp32 with one rounding per operation, like the reference's float32 numpy.
+ *   JOINTS, JOINTS_PA   MPJPE after pelvis alignment (LSP hips 2 and 3) and after the similarity transform of the prediction onto the
+ *                       ground truth (rotation with det +1, scale = trace(R K) / var1); computed for every frame (the reference keeps the
+ *                       VIS3D frames); NaN without joints_gt.
+ *   ACCEL               mean over the J joints of |p[f] - 2 p[f+1] + p[f+2]| for the prediction, NaN when f + 2 leaves the tube.
+ *   ACCEL_ERROR         the same of (prediction - ground truth), NaN unless the whole triple lies in the tube and is VIS3D.
+ *   VIS3D               1 when joints_gt is given and sum(kps_gt[f, :min(K,14), 2]) > min_visible, else 0.
+ * Everything past the fp32 pixel scaling is fp64.  Inputs are fp32 rows at the given strides (in floats), so a [N,25,3] prediction's
+ * first 14 joints are read in place.  A frame's row depends only on its tube; no atomics, bit-identical across launches and batchings.
+ * hd_eval_mesh_tpose: mean vertex distance between the T-pose meshes of beta_gt and beta_pred per frame without running SMPL: at theta = 0
+ * every joint transform is the identity, so verts = (sum_k w_vk) * v_shaped and the difference is (sum_k w_vk) * shapedirs_v * (beta_gt -
+ * beta_pred); from c->dirs and c->lbs_w, fp64, one fixed-order mean per frame.  One launch.
+ * hd_eval_verts_error: mean vertex distance per frame between meshes a [N, V, 3] and b at frame strides a_ld / b_ld floats (>= 3V),
+ * fp64, fixed-order reduction.  One launch.
+ * HD_ERR_INVALID (before any launch): a null pointer, N < 0, n_seq < 1, K outside [1, 32], J outside [4, 32], a row stride shorter than
+ * its row, img_size <= 0, min_visible < 0, V <= 0. */
+enum { HD_EVAL_KP = 0, HD_EVAL_KP_PA = 1, HD_EVAL_KP_PCK = 2, HD_EVAL_JOINTS = 3, HD_EVAL_JOINTS_PA = 4, HD_EVAL_ACCEL = 5,
+       HD_EVAL_ACCEL_ERROR = 6, HD_EVAL_VIS3D = 7, HD_EVAL_COLS = 8 };
+typedef struct {
+  int N, n_seq;
+  const int *seq_start;           /* device [n_seq + 1] */
+  int K, J;                       /* keypoints (<= 32) and 3-D joints (4..32; 14 in the reference's evaluation) per frame */
+  const float *kps_gt;            /* [N, K, 3] x, y, vis in pixels */
+  long long kps_gt_ld;            /* >= 3K */
+  const float *kps_pred;          /* [N, K, 2] in [-1, 1] */
+  long long kps_pred_ld;          /* >= 2K */
+  const float *joints_gt;         /* [N, J, 3] or NULL (dataset without 3-D) */
+  long long joints_gt_ld;         /* >= 3J */
+  const float *joints_pred;       /* [N, J, 3] */
+  long long joints_pred_ld;       /* >= 3J */
+  float img_size;
+  int min_visible;
+  double *out;                    /* [N, HD_EVAL_COLS] */
+} hd_eval_frames_args;
+int hd_eval_frames(const hd_eval_frames_args *a, void *stream);
+int hd_eval_mesh_tpose(const hd_smpl_consts *c, const float *beta_gt, int beta_gt_ld, const float *beta_pred, int beta_pred_ld, int N,
+                       double *out, void *stream);
+int hd_eval_verts_error(const float *a, long long a_ld, const float *b, long long b_ld, int N, int V, double *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
