@@ -25,7 +25,8 @@
 // fused epilogue (scale/shift, residual, ReLU, fp32 output or its strided subsample, the next layer's fp16 pair)
 // straight from the accumulator fragments.  RES (pre-split input, residual row-aligned with the output, K <= 512): each
 // consumer warpgroup's 64 residual rows arrive by TMA in a shared-memory slot while the tile's main loop runs.  Pre-split
-// layers stage their outputs in shared memory (the fp32 output over the residual slot) and write them with TMA stores.
+// layers stage their outputs in shared memory (the fp32 output over the residual slot) and write them with TMA stores; a staged
+// pass runs column pair by column pair, the thread's two rows sharing each pair's epilogue vectors.
 //
 // Warp roles:
 //   warps 0-7    two consumer warpgroups: wgmma issue, drains, epilogue (warpgroup g owns tile rows 64 g .. 64 g + 63)
@@ -452,9 +453,9 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(C::CONS_REGS));
     const int wg = warp >> 2;                             // rows 64 wg .. 64 wg + 63 of the tile
     const bool prof = p.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0;
-    long long t_wait = 0, t_start = prof && !RES ? clock64() : 0;
-    if (RES && prof) p.dbg[2] = clock64();    // start stamp in memory (RES, BN = 128: keeps the consumers within 232 registers spill-free)
-    if (prof) p.dbg[4] = 0;                   // epilogue clocks, summed in memory for the same reason
+    long long t_wait = 0, t_start = prof && BN == 64 && !RES ? clock64() : 0;
+    if ((RES || BN == 128) && prof) p.dbg[2] = clock64();    // start stamp in memory (keeps the BN = 128 consumers within 232 registers spill-free)
+    if (prof) { p.dbg[3] = 0; p.dbg[4] = 0; p.dbg[5] = 0; p.dbg[6] = 0; }   // epilogue clocks and their split, summed in memory for the same reason
     const int hw = p.Ho * p.Wo;
     const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's fragment rows: frow, frow + 8
     const int fcol = 2 * (lane & 3);                            // and columns 8 j + fcol, + 1
@@ -487,9 +488,11 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         const int s = q % STAGES;
         const uint32_t ph = (uint32_t)(q / STAGES) & 1u;
         const bool group_start = (kc % PCH) == 0;
-        long long tw0 = prof ? clock64() : 0;
+        if (BN == 128 && prof) p.dbg[3] -= clock64();     // BN = 128: summed in memory, like the epilogue's clocks
+        const long long tw0 = BN == 64 && prof ? clock64() : 0;
         mbar_wait(full_bar(s), ph);
-        if (prof) t_wait += clock64() - tw0;
+        if (BN == 64 && prof) t_wait += clock64() - tw0;
+        if (BN == 128 && prof) p.dbg[3] += clock64();
         if (ASPLIT) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async (generic proxy) data -> wgmma (async proxy)
         const uint32_t a_hi = smem_base + s * C::STAGE_BYTES + wg * (64 * 128);
         const uint32_t a_lo = a_hi + A_TILE_BYTES;
@@ -537,7 +540,9 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
       if (prof) p.dbg[4] -= clock64();                   // the epilogue's clocks, summed in memory (see above)
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
       const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
+      if (RES && prof) p.dbg[5] -= clock64();            // of the epilogue: waiting for the residual
       if (RES) mbar_wait(res_bar(wg), (uint32_t)ti & 1u);
+      if (RES && prof) p.dbg[5] += clock64();
       // Epilogue from the fragments, per row and pair of adjacent columns c, c + 1 (the four threads of a quad cover 8 contiguous
       // columns of a row): v = acc * scale + shift (+ residual) (ReLU) -> fp32 output (or its strided subsample), and the next
       // layer's pre-activation relu?(v * s2 + b2) as an fp16 head / remainder pair.
@@ -592,17 +597,48 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         const int r0 = m0 + 64 * wg;
         const uint32_t rsw = (uint32_t)(lane >> 2);            // the swizzle of this thread's rows: (frow + 8 h) & 7
         auto acquire = [&](bool after_out) {   // the staging buffer may be rewritten: its last stores have been read
+          if (prof) p.dbg[6] -= clock64();                     // of the epilogue: waiting for stores to be read
           if (stg_issuer) {
             if (after_out) bulk_wait_read<1>();                // RES: the fp32 stores just issued read the slot, not the buffer
             else bulk_wait_read<0>();
           }
           named_bar_sync(3 + wg, 128);
+          if (prof) p.dbg[6] += clock64();
         };
 #pragma unroll
         for (int cc = 0; cc < BN / 64; ++cc) {
           const int c0 = n0 + 64 * cc;
           const bool issue = stg_issuer && r0 < p.M && c0 < p.Cout;
           if (st32 && !RES) acquire(false);
+          // A thread's two rows (frow, frow + 8) have the same columns.  Where everything is staged and no residual comes from global
+          // memory (every trunk layer but the strided subsamples) the pass goes column pair by column pair: the epilogue vectors of a
+          // pair are read once for both rows, from one base pointer per vector, and nothing per row is kept but its validity.  Each
+          // product and sum is rounded on its own (__fmul_rn / __fadd_rn are never contracted), as in the row-by-row loops.
+          const bool rok[2] = {m0 + frow < p.M, m0 + frow + 8 < p.M};
+          if (st32 && (RES || !p.res)) {
+            uint8_t *brow = (RES ? res_sm + 2 * cc * BOX_BYTES : stg) + (frow - 64 * wg) * 128 + 8 * (lane & 1);    // row frow + 8 h: + 1024 h
+            const float *vsc = p.post_scale ? p.post_scale + c0 + fcol : nullptr, *vsh = p.post_shift ? p.post_shift + c0 + fcol : nullptr;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * cc + jj;
+              if (c0 + 8 * jj + fcol >= p.Cout) continue;
+              const uint32_t piece = (uint32_t)(2 * (jj & 3) + ((lane & 3) >> 1)) ^ rsw;
+              const float2 sc = vsc ? __ldg(reinterpret_cast<const float2 *>(vsc + 8 * jj)) : make_float2(0.f, 0.f);
+              const float2 sh = vsh ? __ldg(reinterpret_cast<const float2 *>(vsh + 8 * jj)) : make_float2(0.f, 0.f);
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                if (!rok[h]) continue;
+                float2 *f32 = reinterpret_cast<float2 *>(brow + h * 1024 + (jj >> 2) * BOX_BYTES + piece * 16);
+                float y0 = sums[4 * j + 2 * h], y1 = sums[4 * j + 2 * h + 1];
+                if (vsc) { y0 = __fmul_rn(y0, sc.x); y1 = __fmul_rn(y1, sc.y); }
+                if (vsh) { y0 = __fadd_rn(y0, sh.x); y1 = __fadd_rn(y1, sh.y); }
+                if (RES) { const float2 r = *f32; y0 = __fadd_rn(y0, r.x); y1 = __fadd_rn(y1, r.y); }
+                if (p.post_relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+                *f32 = make_float2(y0, y1);
+                sums[4 * j + 2 * h] = y0; sums[4 * j + 2 * h + 1] = y1;
+              }
+            }
+          } else {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int m = m0 + frow + 8 * h;
@@ -627,6 +663,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
               sums[4 * j + 2 * h] = y0; sums[4 * j + 2 * h + 1] = y1;
             }
           }
+          }
           if (st32) {
             fence_proxy_async();
             named_bar_sync(3 + wg, 128);
@@ -639,6 +676,31 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           }
           if (p.out_hi) {
             if (st2) acquire(RES && st32);
+            if (st2) {
+              uint8_t *brow = stg + (frow - 64 * wg) * 128 + 4 * (lane & 3);
+              const float *vsc = p.post2_scale ? p.post2_scale + c0 + fcol : nullptr, *vsh = p.post2_shift ? p.post2_shift + c0 + fcol : nullptr;
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj) {
+                const int j = 8 * cc + jj;
+                if (c0 + 8 * jj + fcol >= p.Cout) continue;
+                const float2 sc = vsc ? __ldg(reinterpret_cast<const float2 *>(vsc + 8 * jj)) : make_float2(0.f, 0.f);
+                const float2 sh = vsh ? __ldg(reinterpret_cast<const float2 *>(vsh + 8 * jj)) : make_float2(0.f, 0.f);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  if (!rok[h]) continue;
+                  float a0 = sums[4 * j + 2 * h], a1 = sums[4 * j + 2 * h + 1];
+                  if (vsc) { a0 = __fmul_rn(a0, sc.x); a1 = __fmul_rn(a1, sc.y); }
+                  if (vsh) { a0 = __fadd_rn(a0, sh.x); a1 = __fadd_rn(a1, sh.y); }
+                  if (p.post2_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+                  uint32_t hh, ll;
+                  split_f16x2(a0, a1, hh, ll);
+                  // columns 8 j + fcol, + 1 of the pass: piece jj of the 128-byte row
+                  uint32_t *hs = reinterpret_cast<uint32_t *>(brow + h * 1024 + (((uint32_t)jj ^ rsw) * 16));
+                  hs[0] = hh;
+                  hs[BOX_BYTES / 4] = ll;
+                }
+              }
+            } else {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const int m = m0 + frow + 8 * h;
@@ -662,6 +724,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
                   *reinterpret_cast<uint32_t *>(lrow + c) = ll;
                 }
               }
+            }
             }
             if (st2) {
               fence_proxy_async();
@@ -717,6 +780,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
       }
       }
       if (RES && ti + 1 < my_tiles) {
+        if (prof) p.dbg[6] -= clock64();
         named_bar_sync(1 + wg, 128);                       // every thread of the warpgroup has read the slot
         if (res_issuer) {
           if (stage & STAGE_OUT) {                         // the slot's fp32 stores have read it (the pair's may still run)
@@ -725,11 +789,12 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           }
           load_res(ti + 1);
         }
+        if (prof) p.dbg[6] += clock64();
       }
       if (prof) p.dbg[4] += clock64();
     }
     if (stg_issuer) bulk_wait_all();                       // the last stores have completed before the CTA exits
-    if (prof) { p.dbg[2] = clock64() - (RES ? p.dbg[2] : t_start); p.dbg[3] = t_wait; }
+    if (prof) { p.dbg[2] = clock64() - (RES || BN == 128 ? p.dbg[2] : t_start); if (BN == 64) p.dbg[3] = t_wait; }
   }
 }
 

@@ -10,7 +10,8 @@ from human_dynamics_b200 import synthetic                         # noqa: E402
 from human_dynamics_b200._lib import lib, check                   # noqa: E402
 from human_dynamics_b200.nets import PackedResNet, ResNetPlan     # noqa: E402
 
-NAMES = ['prod_loop', 'prod_wait_empty', 'cons_loop', 'cons_wait_full', 'epilogue']      # dbg[0..4] (conv_simt.cu)
+# dbg[0..6] (conv_simt.cu); the last two are parts of `epilogue`, the rest of it is arithmetic and issuing stores
+NAMES = ['prod_loop', 'prod_wait_empty', 'cons_loop', 'cons_wait_full', 'epilogue', 'epi_wait_res', 'epi_wait_stores']
 
 
 def main():
