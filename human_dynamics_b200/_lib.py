@@ -146,6 +146,9 @@ SIGNATURES = {
     'hd_maxpool3x3s2_same': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     'hd_subsample': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp]),
     'hd_bnrelu_avgpool': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    'hd_bn_stats_workspace_bytes': (_sz, [_ll, _i]),
+    'hd_bn_batch_stats': (_i, [_vp, _ll, _i, _ll, _vp, _vp, _f] + [_vp] * 6 + [C.c_double, _vp, _sz, _vp]),
+    'hd_bn_moving_update': (_i, [_vp, _vp, _ll, _i, C.c_double, _vp, _vp, _vp]),
     'hd_process_image': (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _vp]),
     'hd_crop_geometry': (_i, [_i, _i, _vp, _i, _vp, _vp, _vp]),
     'hd_groupnorm_stats': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),

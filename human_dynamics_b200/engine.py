@@ -122,6 +122,8 @@ class HMMREngine(object):
             self.hal = PackedHal(w, self.device, tc=tc) if 'fc2_res/fc1/weights' in w else None
             self.smpl = smpl_model if isinstance(smpl_model, SMPLConstants) else SMPLConstants(smpl_model, device=self.device)
         self._resnet_plans = _Bounded(8)
+        self._weights = w                       # the training-mode trunk reads gamma / beta / moving statistics on first use
+        self._train_trunk = None
         self._fmovie_plans = _Bounded(4)
         self._ief_plans = _Bounded(4)
         self._hal_plans = _Bounded(4)
@@ -233,6 +235,20 @@ class HMMREngine(object):
         if N:
             self._trunk(images, phi)
         return phi
+
+    def encode_images_train(self, images):
+        """encoder_resnet(is_training=True): (N,H,W,3) float32 CUDA NHWC -> (N,2048), every batch norm with the moments of these N
+        frames (nets.ResNetTrainPlan over the whole batch).  The moving statistics are left alone, as a TF graph leaves them when its
+        update ops are not run."""
+        from .objective import _TrainTrunk
+        if not isinstance(images, torch.Tensor) or not images.is_cuda or images.dtype != torch.float32 or images.dim() != 4:
+            raise _lib.HDError('encode_images_train: float32 CUDA tensor (N,S,S,3) required (no CPU fallback exists)')
+        if images.shape[0] < 1:
+            raise _lib.HDError('encode_images_train: batch statistics need at least one frame')
+        if self._train_trunk is None:
+            self._train_trunk = _TrainTrunk(self._weights, self.device)
+        phi, _ = self._train_trunk(images[None])
+        return phi[0]
 
     def temporal_encode(self, feats):
         """az_fc2_groupnorm ("f_movie"): (B,T,2048) -> (B,T,2048)."""

@@ -17,6 +17,12 @@ from ._lib import lib, check, fptr, current_stream, ConvDesc
 
 RESNET_BLOCKS = ((64, 3, 2), (128, 4, 2), (256, 6, 2), (512, 3, 1))
 BN_EPS = 1e-5        # resnet_arg_scope batch_norm_epsilon [TF-ext]
+# Training-mode batch norm [TF-ext] (slim batch_norm with is_training=True; TF 1.8 takes its fused kernel for 4-D NHWC input): a map is
+# normalised with its batch mean and BIASED batch variance over frames x H x W, and the layer's UPDATE_OPS move the moving statistics
+# by one step of assign_moving_average, m -= (m - v) * (1 - BN_DECAY), with v = the batch mean and the BESSEL-CORRECTED batch variance
+# var_b * rows / (rows - 1) (the variance output of the fused kernel).  The fused op also raises an epsilon below 1.001e-5 to that
+# value; both trunks here use BN_EPS, as the inference trunk always has.  Pinned only through the TF stand-in (oracle/ref_exec).
+BN_DECAY = 0.997     # resnet_arg_scope batch_norm_decay [TF-ext]
 GN_EPS = 1e-6        # tf.contrib.layers.group_norm epsilon [TF-ext]
 GN_GROUPS = 32
 
@@ -119,10 +125,12 @@ class PackedConv(object):
         pack_weight(src, KH, Cin, self.Cout, self.w_nk_hi, self.w_nk_lo, stream)
 
     def bind(self, inp, n_img, H, W, out, in_ld=None, out_ld=None, pre=None, res=None, res_geom=None, impl='auto',
-             inp_split=None, out_split=None, post2=None, out_subsample=0):
+             inp_split=None, out_split=None, post2=None, out_subsample=0, post=None):
         """Fill a descriptor.  inp/out/res: CUDA float32 tensors (only their data_ptr is used).
 
         pre = (scale, shift, img_stride, relu); res_geom = (res_ld, res_H, res_W, res_stride).
+        post = (scale|None, shift|None, relu): epilogue vectors in place of the layer's own (the training-mode trunk writes conv1 /
+        conv2 raw, post = (None, None, False), and normalises them with batch statistics in the next layer's prologue).
         out_subsample = s > 1: `out` is the dense [n, ceil(Ho/s), ceil(Wo/s), Cout] tensor x[:, ::s, ::s] (hd_b200.h);
         inp_split = (hi, lo) fp16 tensors: pre-activated, pre-split A operand (then `inp` may be None);
         out_split = (hi, lo) fp16 tensors + post2 = (scale|None, shift|None, relu): second output (then `out` may be None).
@@ -143,11 +151,12 @@ class PackedConv(object):
         if pre is not None:
             d.pre_scale, d.pre_shift = pre[0].data_ptr(), pre[1].data_ptr()
             d.pre_img_stride, d.pre_relu = int(pre[2]), int(pre[3])
-        if self.post_scale is not None:
-            d.post_scale = self.post_scale.data_ptr()
-        if self.post_shift is not None:
-            d.post_shift = self.post_shift.data_ptr()
-        d.post_relu = int(self.post_relu)
+        post_scale, post_shift, post_relu = (self.post_scale, self.post_shift, self.post_relu) if post is None else post
+        if post_scale is not None:
+            d.post_scale = post_scale.data_ptr()
+        if post_shift is not None:
+            d.post_shift = post_shift.data_ptr()
+        d.post_relu = int(post_relu)
         if res is not None:
             d.res = res.data_ptr()
             if res_geom is None:
@@ -179,7 +188,7 @@ class PackedConv(object):
             d.tmap_lo = C.cast(self.tmap_lo, C.c_void_p)
         else:
             d.impl = _lib.HD_IMPL_SIMT
-        op = ConvOp(d, (self, inp, out, pre, res, inp_split, out_split, post2), (Ho, Wo))
+        op = ConvOp(d, (self, inp, out, pre, res, inp_split, out_split, post2, post), (Ho, Wo))
         if not TMA_EPILOGUE:
             d.flags |= _lib.HD_CONV_NO_TMA_EPILOGUE
         op.encode_act_maps()
@@ -551,6 +560,192 @@ class ResNetPlan(object):
     @property
     def num_launches(self):
         return ((3 if self.planes is not None else 2) if self.root else 0) + len(self.ops) + (1 if self.tail else 0)
+
+
+# ------------------------------------------------------------------------------------------------
+# ResNet-v2-50 in training mode (is_training=True: batch statistics) -- src/models.py:50-77 as trainer_sequence_fc.py:562-575 calls it
+# ------------------------------------------------------------------------------------------------
+def resnet_bn_scopes(blocks=RESNET_BLOCKS):
+    """The trunk's 49 batch-norm scopes in the order a forward pass meets them: per unit preact, conv1/BatchNorm, conv2/BatchNorm; then
+    postnorm."""
+    p = 'resnet_v2_50'
+    out = []
+    for b, (_, units, _) in enumerate(blocks, start=1):
+        for u in range(1, units + 1):
+            q = '%s/block%d/unit_%d/bottleneck_v2' % (p, b, u)
+            out += [q + '/preact', q + '/conv1/BatchNorm', q + '/conv2/BatchNorm']
+    return out + [p + '/postnorm']
+
+
+class ResNetBatchNorm(object):
+    """gamma, beta and the moving statistics of the trunk's batch-norm layers, each a flat device vector with one slice per scope
+    (`scopes` order, `offsets`).  Training-mode plans read gamma / beta and step moving_mean / moving_variance in place."""
+
+    def __init__(self, w, device, blocks=RESNET_BLOCKS):
+        self.device = device
+        self.scopes = resnet_bn_scopes(blocks)
+        missing = [s + '/' + k for s in self.scopes for k in ('gamma', 'beta', 'moving_mean', 'moving_variance') if s + '/' + k not in w]
+        if missing:
+            raise _lib.HDError('training-mode ResNet: weights lack %d batch-norm variables, e.g. %s' % (len(missing), missing[0]))
+        self.sizes = [int(np.size(w[s + '/gamma'])) for s in self.scopes]
+        self.offsets = [0] + [int(v) for v in np.cumsum(self.sizes)]
+
+        def flat(k):
+            return _dev(np.concatenate([np.asarray(w[s + '/' + k], np.float32).reshape(-1) for s in self.scopes]), device)
+        self.gamma, self.beta = flat('gamma'), flat('beta')
+        self.moving_mean, self.moving_variance = flat('moving_mean'), flat('moving_variance')
+
+    def view(self, t, i):
+        return t[self.offsets[i]:self.offsets[i + 1]]
+
+    def moving(self):
+        """{'<scope>/moving_mean' | '<scope>/moving_variance': float32 ndarray}, copied to the host."""
+        mm, mv = self.moving_mean.cpu().numpy(), self.moving_variance.cpu().numpy()
+        out = {}
+        for i, s in enumerate(self.scopes):
+            a, b = self.offsets[i], self.offsets[i + 1]
+            out[s + '/moving_mean'], out[s + '/moving_variance'] = mm[a:b].copy(), mv[a:b].copy()
+        return out
+
+
+class BatchStatsOp(object):
+    """hd_bn_batch_stats over one [rows, C] map: one op in a training plan's op list, writing the scale / shift the next layers'
+    prologue (or the tail) applies and the layer's batch mean / biased variance."""
+    __slots__ = ('x', 'rows', 'C', 'gamma', 'beta', 'scale', 'shift', 'mean', 'var', 'ws', 'd')
+
+    def __init__(self, x, rows, C, gamma, beta, scale, shift, mean, var, ws):
+        self.x, self.rows, self.C = x, rows, C
+        self.gamma, self.beta, self.scale, self.shift, self.mean, self.var, self.ws = gamma, beta, scale, shift, mean, var, ws
+        self.d = None
+
+    def encode_act_maps(self):
+        pass
+
+    def run(self, stream):
+        check(lib.hd_bn_batch_stats(fptr(self.x), self.rows, self.C, self.C, fptr(self.gamma), fptr(self.beta), BN_EPS, fptr(self.scale),
+                                    fptr(self.shift), fptr(self.mean), fptr(self.var), None, None, 0.0, C.c_void_p(self.ws.data_ptr()),
+                                    self.ws.numel(), stream), 'hd_bn_batch_stats')
+
+
+class ResNetTrainPlan(object):
+    """Training-mode forward of the whole trunk over n frames (slim resnet_v2_50 with is_training=True, no dropout on this path): every
+    batch norm normalises with the moments of the current batch over all n frames x H x W.  The fp32 layer chain of ResNetPlan with
+    the batch statistics of each map taken right before the layers that apply them:
+
+      root   conv1 + pool1 exactly as in the inference plan (no batch norm there)
+      unit   stats(x) -> preact scale/shift, applied (+ReLU) in the A producer of the shortcut conv and of conv1; conv1 writes raw fp32;
+             stats -> conv2's prologue (padded 3x3, strided in a block's last unit); conv2 writes raw; stats -> conv3's prologue;
+             conv3 adds its bias and the residual (the identity shortcut reads the raw unit input, as slim does)
+      tail   stats(final map) -> hd_bnrelu_avgpool's scale / shift
+
+    49 BatchStatsOps.  The scale / shift / mean / variance vectors are plan-owned device buffers rewritten on every run, so the
+    descriptors never change.  `run` leaves the moving statistics alone; `apply_moving_update` takes the one step of the update ops
+    from this run's moments."""
+
+    def __init__(self, packed: PackedResNet, bn: ResNetBatchNorm, n, size=224, impl='auto'):
+        self.p, self.bn, self.n, self.size = packed, bn, n, size
+        dev = packed.device
+        H1 = size // 2
+        H2 = (H1 + 1) // 2
+        self.H1, self.H2 = H1, H2
+        mx_io, mx_r, h = max(H1 * H1 * 64, H2 * H2 * 64), 0, H2
+        for unit in packed.units:
+            ho = (h - 1) // unit['stride'] + 1
+            mx_io = max(mx_io, h * h * unit['depth'], ho * ho * unit['depth'])
+            mx_r = max(mx_r, h * h * unit['base'])
+            h = ho
+        f32 = dict(dtype=torch.float32, device=dev)
+        self.bufA, self.bufB, self.bufS = (torch.empty(n * mx_io, **f32) for _ in range(3))
+        self.bufR1, self.bufR2 = torch.empty(n * mx_r, **f32), torch.empty(n * mx_r, **f32)
+        L = bn.offsets[-1]
+        self.scale, self.shift, self.mean, self.var = (torch.empty(L, **f32) for _ in range(4))
+        self.planes = None
+        self.conv1_op = None
+        if packed.conv1_planes is not None and impl in ('auto', 'tc3h') and CONV1_PLANES and size % 2 == 0:
+            self.planes = packed.conv1_planes.alloc_planes(n, size)
+            self.conv1_op = packed.conv1_planes.bind(self.planes, n, size, self.bufS)
+        elif packed.conv1.tc and impl != 'simt':
+            self.conv1_op = packed.conv1.bind(self.bufS, n, size, size, self.bufS, in_ld=3, impl=impl)
+        self.ops, self.stats = [], []
+        shapes = []                           # (map, rows, C) of every normalised map, in scope order
+        h = H2
+        for unit in packed.units:
+            ho = (h - 1) // unit['stride'] + 1
+            shapes += [(n * h * h, unit['d_in']), (n * h * h, unit['base']), (n * ho * ho, unit['base'])]
+            h = ho
+        shapes.append((n * h * h, packed.out_dim))
+        ws_bytes = max(int(lib.hd_bn_stats_workspace_bytes(rows, Cc)) for rows, Cc in shapes)
+        self.ws = torch.empty(max(16, ws_bytes), dtype=torch.uint8, device=dev)
+
+        def stats(x, rows, Cc):
+            i = len(self.stats)
+            assert (rows, Cc) == shapes[i], (i, rows, Cc, shapes[i])
+            v = lambda t: bn.view(t, i)          # noqa: E731
+            op = BatchStatsOp(x, rows, Cc, v(bn.gamma), v(bn.beta), v(self.scale), v(self.shift), v(self.mean), v(self.var), self.ws)
+            self.ops.append(op)
+            self.stats.append(op)
+            return (op.scale, op.shift, 0, 1)
+
+        raw = (None, None, False)
+        x, y, H = self.bufA, self.bufB, H2
+        for unit in packed.units:
+            s = unit['stride']
+            Ho = (H - 1) // s + 1
+            pre = stats(x, n * H * H, unit['d_in'])
+            if 'shortcut' in unit:
+                self.ops.append(unit['shortcut'].bind(x, n, H, H, self.bufS, pre=pre, impl=impl))
+                res, res_geom = self.bufS, (unit['depth'], Ho, Ho, 1)
+            else:
+                res, res_geom = x, (unit['depth'], H, H, s)      # identity, or max_pool2d(1x1, stride) = subsample, of the raw input
+            self.ops.append(unit['conv1'].bind(x, n, H, H, self.bufR1, pre=pre, impl=impl, post=raw))
+            pre1 = stats(self.bufR1, n * H * H, unit['base'])
+            self.ops.append(unit['conv2'].bind(self.bufR1, n, H, H, self.bufR2, pre=pre1, impl=impl, post=raw))
+            pre2 = stats(self.bufR2, n * Ho * Ho, unit['base'])
+            self.ops.append(unit['conv3'].bind(self.bufR2, n, Ho, Ho, y, pre=pre2, res=res, res_geom=res_geom, impl=impl))
+            x, y = y, x
+            H = Ho
+        self.final, self.final_hw = x, H * H
+        self.tail = stats(x, n * H * H, packed.out_dim)
+        assert len(self.stats) == len(bn.scopes)
+
+    def run(self, images, out, stream=None):
+        """images (n,size,size,3) contiguous float32 CUDA NHWC in [-1, 1] (None: the conv1 planes were filled by the caller) -> out
+        (n,2048) float32 view: the phis with batch statistics.  The moving statistics are not touched."""
+        st = current_stream() if stream is None else stream
+        n, p = self.n, self.p
+        if self.planes is not None:
+            if images is not None:
+                check(lib.hd_pack_conv1_planes(fptr(images), C.c_void_p(self.planes[0].data_ptr()), C.c_void_p(self.planes[1].data_ptr()),
+                                               n, self.size, self.size, self.planes[0].shape[2], st), 'hd_pack_conv1_planes')
+            self.conv1_op.run(st)
+        elif self.conv1_op is not None:
+            self.conv1_op.d.in_ = images.data_ptr()
+            self.conv1_op.run(st)
+        else:
+            check(lib.hd_conv1_7x7s2(fptr(images), fptr(p.conv1_w), fptr(p.conv1_b), fptr(self.bufS), n, self.size, self.size, st),
+                  'hd_conv1_7x7s2')
+        check(lib.hd_maxpool3x3s2_same(fptr(self.bufS), fptr(self.bufA), n, self.H1, self.H1, 64, None, None, None, None, st),
+              'hd_maxpool3x3s2_same')
+        for op in self.ops:
+            op.run(st)
+        check(lib.hd_bnrelu_avgpool(fptr(self.final), fptr(self.tail[0]), fptr(self.tail[1]), fptr(out), n, self.final_hw, p.out_dim, st),
+              'hd_bnrelu_avgpool')
+
+    def apply_moving_update(self, decay=BN_DECAY, stream=None):
+        """One step of the 49 layers' update ops from the moments of the last `run`: bn.moving_mean / moving_variance in place."""
+        st = current_stream() if stream is None else stream
+        bn = self.bn
+        for i, op in enumerate(self.stats):
+            check(lib.hd_bn_moving_update(fptr(op.mean), fptr(op.var), op.rows, op.C, float(decay), fptr(bn.view(bn.moving_mean, i)),
+                                          fptr(bn.view(bn.moving_variance, i)), st), 'hd_bn_moving_update')
+
+    def moments(self):
+        """{scope: (batch mean, biased batch variance)} of the last `run`, device views."""
+        return {s: (op.mean, op.var) for s, op in zip(self.bn.scopes, self.stats)}
+
+    @property
+    def num_launches(self):
+        return (3 if self.planes is not None else 2) + sum(2 if isinstance(op, BatchStatsOp) else 1 for op in self.ops) + 1
 
 
 # ------------------------------------------------------------------------------------------------

@@ -11,10 +11,17 @@ sum of its terms, with the weights of trainer_sequence_fc.py:280-310.
         out = trainer.step(batch, mocap)              # device scalars, no synchronise
     trainer.save_checkpoint('/path/model.ckpt-1000')  # Tester and PoseDiscriminator load it
 
+With precomputed_phi=False (the reference's online-augmentation path) a batch carries `images` (B, T, S, S, 3) float32 in [-1, 1], e.g.
+augment.TubeAugmentor(...)['images'], instead of `phis`: the frozen ResNet runs over all B*T crops in training mode (batch statistics,
+nets.ResNetTrainPlan) without autograd, and each `step` applies the trunk's update ops once (one moving-average step of its 49
+batch-norm layers, decay 0.997), which save_checkpoint writes.
+
 Differences from the reference trainer: IEF dropout is the identity (the backward of trainable.TemporalModel follows the inference
-graph); torch's Adam adds eps to sqrt(v_hat) where TF's adds it to sqrt(v) before the bias correction; the static `use_hmr_only` branch,
-freeze_phi=False and image input are not built.  A frame with no visible keypoint in an optimal-camera term contributes 0 (the
-reference's procrustes2d_vis divides 0 / 0 there and the loss is NaN).
+graph); torch's Adam adds eps to sqrt(v_hat) where TF's adds it to sqrt(v) before the bias correction; the static `use_hmr_only` branch
+and freeze_phi=False (it needs the trunk's backward) are not built.  A frame with no visible keypoint in an optimal-camera term
+contributes 0 (the reference's procrustes2d_vis divides 0 / 0 there and the loss is NaN).  The moving statistics start from whatever
+`weights` holds, so a resumed run continues them; a fresh reference run restores only the trainable variables from its hmr_noS5
+checkpoint (trainer_sequence_fc.py:346-392), so its moving statistics start at 0 / 1 -- pass those values in `weights` to reproduce it.
 """
 from __future__ import annotations
 
@@ -28,6 +35,7 @@ from torch.autograd.function import once_differentiable
 from . import _lib
 from ._lib import lib, check, current_stream
 from .config import HMMRConfig
+from .nets import RESNET_BLOCKS
 
 F32 = torch.float32
 
@@ -50,6 +58,8 @@ class TrainConfig(HMMRConfig):
     predict_delta: bool = True
     do_hallucinate: bool = False
     do_hallucinate_preds: bool = False
+    precomputed_phi: bool = True
+    freeze_phi: bool = True
 
 
 def loss_weights(config):
@@ -317,7 +327,8 @@ class HMMRTrainer(object):
     d_opt): f_movie (and fc2_res with do_hallucinate) over precomputed phis, the IEF heads from the tiled mean_param, one SMPL call over
     every prediction set, the objective, D_pose on reals + fakes, and both updates from the same pre-step parameters.
 
-    `optimizer`: optional factory (params, lr) -> torch optimizer, default torch.optim.Adam."""
+    `optimizer`: optional factory (params, lr) -> torch optimizer, default torch.optim.Adam.
+    With config.precomputed_phi=False, `weights` must also hold the resnet_v2_50/* variables (see the module docstring)."""
 
     def __init__(self, config, weights, smpl_model, disc_weights=None, optimizer=None, device=None):
         from .adversarial import PoseDiscriminator
@@ -326,7 +337,12 @@ class HMMRTrainer(object):
         self.config = config
         if config.do_hallucinate and not config.predict_delta:
             raise _lib.HDError('do_hallucinate needs predict_delta (the reference asserts it, src/config.py:271)')
+        if not config.freeze_phi:
+            raise _lib.HDError('freeze_phi=False is not built: training the ResNet needs its backward (conv data / weight gradients, '
+                               'batch-norm and max-pool backward)')
         self.model = TemporalModel(weights, config, device=device)
+        self.trunk = None if config.precomputed_phi else _TrainTrunk(self.model._source, self.model.device)
+        self._pending = None                  # the trunk plan of the last forward: step applies its update ops
         self.disc = PoseDiscriminator(disc_weights, device=self.model.device) if disc_weights is not None else \
             PoseDiscriminator(seed=0, device=self.model.device)
         self.smpl = smpl_model if hasattr(smpl_model, 'consts') else SMPL(smpl_model)
@@ -351,7 +367,10 @@ class HMMRTrainer(object):
         from .smpl import batch_rodrigues
         from src.ops import compute_loss_d_fake, compute_loss_d_real, compute_loss_e_fake
         cfg, model = self.config, self.model
-        phis = batch['phis']
+        if cfg.precomputed_phi:
+            phis = batch['phis']
+        else:
+            phis, self._pending = self.trunk(batch['images'])
         B, T = int(phis.shape[0]), int(phis.shape[1])
         K = int(batch['labels'].shape[2])
         obj = self.objective(B, T, K)
@@ -401,6 +420,9 @@ class HMMRTrainer(object):
         """One iteration: both updates computed from the same pre-step parameters, then applied.  e_loss moves the temporal model,
         d_loss D_pose (not at all when d_lw_pose = 0).  Returns {key: loss, 'e_loss', 'd_loss'} as detached device scalars."""
         named, e_loss, d_loss = self.forward(batch, mocap_poses)
+        if self._pending is not None:         # UPDATE_OPS, grouped with e_loss (trainer_sequence_fc.py:745-750)
+            self._pending.apply_moving_update()
+            self._pending = None
         ge = torch.autograd.grad(e_loss, self.e_params, retain_graph=True, allow_unused=True)
         use_d = self.config.d_lw_pose > 0
         gd = torch.autograd.grad(d_loss, self.d_params, allow_unused=True) if use_d else None
@@ -418,7 +440,10 @@ class HMMRTrainer(object):
         return out
 
     def tf_variables(self):
+        """E and D variables; with image input the trunk's moving statistics are the current ones."""
         v = self.model.tf_variables()
+        if self.trunk is not None:
+            v.update(self.trunk.bn.moving())
         v.update(self.disc.tf_variables())
         return v
 
@@ -427,6 +452,53 @@ class HMMRTrainer(object):
         from .tf_checkpoint import save_checkpoint
         save_checkpoint(prefix, self.tf_variables())
         return prefix
+
+
+class _TrainTrunk(object):
+    """The frozen ResNet of an image-input trainer: packed once, one ResNetTrainPlan per (frames, size), the moving statistics shared by
+    all of them.  Called with images (B, T, S, S, 3) -> (phis (B, T, 2048) without autograd, the plan that made them)."""
+
+    def __init__(self, w, device):
+        from .nets import PackedResNet, ResNetBatchNorm
+        p = 'resnet_v2_50'
+        need = [p + '/conv1/weights', p + '/conv1/biases']
+        for b, (_, units, _) in enumerate(RESNET_BLOCKS, start=1):
+            for u in range(1, units + 1):
+                q = '%s/block%d/unit_%d/bottleneck_v2' % (p, b, u)
+                need += [q + '/conv%d/weights' % k for k in (1, 2, 3)] + [q + '/conv3/biases']
+                if u == 1:
+                    need += [q + '/shortcut/weights', q + '/shortcut/biases']
+        missing = [k for k in need if k not in w]
+        if missing:
+            raise _lib.HDError('precomputed_phi=False runs the ResNet: weights lack %d resnet_v2_50 variables, e.g. %s'
+                               % (len(missing), missing[0]))
+        with torch.cuda.device(device):
+            self.bn = ResNetBatchNorm(w, device)
+            self.packed = PackedResNet(w, device, tc='auto')
+        self.device = device
+        self._plans = {}
+
+    def plan(self, n, size):
+        from .nets import ResNetTrainPlan
+        key = (n, size)
+        if key not in self._plans:
+            self._plans.clear()                   # one batch shape at a time: a plan holds gigabytes of activations at 224 x 224
+            self._plans[key] = ResNetTrainPlan(self.packed, self.bn, n, size)
+        return self._plans[key]
+
+    def __call__(self, images):
+        if not isinstance(images, torch.Tensor) or not images.is_cuda or images.dtype != F32 or images.dim() != 5 or \
+                images.shape[4] != 3 or images.shape[2] != images.shape[3]:
+            raise _lib.HDError('batch["images"] must be a float32 CUDA tensor (B, T, S, S, 3), got %s'
+                               % ((images.dtype, tuple(images.shape)) if isinstance(images, torch.Tensor) else type(images),))
+        if images.device != self.device:
+            raise _lib.HDError('batch["images"] is on %s, the trainer on %s' % (images.device, self.device))
+        B, T, S = int(images.shape[0]), int(images.shape[1]), int(images.shape[2])
+        plan = self.plan(B * T, S)
+        phis = torch.empty((B * T, self.packed.out_dim), dtype=F32, device=self.device)
+        with torch.no_grad():
+            plan.run(images.detach().reshape(B * T, S, S, 3).contiguous(), phis)
+        return phis.view(B, T, -1), plan
 
 
 # ------------------------------------------------------------------------------------------------------------------------------------

@@ -140,6 +140,24 @@ int hd_subsample(const float *in, float *out, int N, int H, int W, int C, int st
 /* postnorm BN+ReLU then global mean over HxW: in [N,HW,C] -> out [N,C]. */
 int hd_bnrelu_avgpool(const float *in, const float *scale, const float *shift, float *out, int N, int HW, int C, void *stream);
 
+/* ---- training-mode batch norm (slim batch_norm with is_training=True; resnet_arg_scope, src/models.py:65-74 under
+ * trainer_sequence_fc.py:562-575).  x is an NHWC map viewed as [rows, C] with row pitch ld floats (rows = frames x H x W).  Writes
+ *   mean_b[c] = mean over the rows, var_b[c] = biased variance over the rows (both accumulated in fp64 about row 0's value),
+ *   scale[c] = gamma[c] / sqrt(var_b + eps), shift[c] = beta[c] - mean_b * scale    (the pre_* / post_* vectors of hd_conv_gemm)
+ * and, when `mean` / `var` are non-NULL, mean_b / var_b as fp32.  When moving_mean / moving_var are non-NULL (both or neither) they
+ * take one in-place float32 step of TF's assign_moving_average: m -= (m - v) * (float)(1 - decay), with v = mean_b for the mean and
+ * the Bessel-corrected var_b * rows / (rows - 1) for the variance.  Partials per fixed chunk of rows are merged in a fixed order:
+ * repeats are bit-identical.  `workspace` (16-byte aligned) holds hd_bn_stats_workspace_bytes(rows, C) bytes.  x 16-byte aligned,
+ * C % 4 == 0, ld % 4 == 0, ld >= C, rows >= 2, else HD_ERR_INVALID and nothing is launched. */
+size_t hd_bn_stats_workspace_bytes(long long rows, int C);
+int hd_bn_batch_stats(const float *x, long long rows, int C, long long ld, const float *gamma, const float *beta, float eps,
+                      float *scale, float *shift, float *mean, float *var, float *moving_mean, float *moving_var, double decay,
+                      void *workspace, size_t workspace_bytes, void *stream);
+/* The same moving-average step from a saved mean_b / var_b (the fp32 outputs of hd_bn_batch_stats over `rows` rows), bit-identical to
+ * the step hd_bn_batch_stats takes itself: lets a trainer apply the update ops of an iteration after its forward pass. */
+int hd_bn_moving_update(const float *mean, const float *var, long long rows, int C, double decay, float *moving_mean, float *moving_var,
+                        void *stream);
+
 /* ---- crop pre-processing, the caller of the path: process_image (src/evaluation/run_video.py:56-107) + resize_img
  * (src/util/common.py:7-14), batched.  frames uint8 [N,H,W,3]; geom int32 [N,4] (16-byte aligned) = {Hs, Ws, x0, y0}: size of the
  * cv2.resize'd frame and the top-left corner of the SxS crop in its coordinates (may lie outside: edge replication = the

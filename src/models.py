@@ -38,10 +38,13 @@ def get_temporal_encoder(model_type='AZ_FC2GN'):
 def encoder_resnet(x, is_training=True, weight_decay=0.001, reuse=False):
     """Resnet v2-50 (models.py:50-77).  x: N x H x W x 3 (NHWC, [-1,1]) -> (N x 2048, 'resnet_v2_50').
 
-    Inference only: is_training=True is rejected (no backward pass exists on this path)."""
+    is_training=True normalises every batch norm with the moments of these N frames (the trainer's call, trainer_sequence_fc.py:562-575)
+    and leaves the engine's moving averages alone, as a TF graph does without its update ops.  Forward only: no gradient flows into the
+    trunk (the reference's default freeze_phi=True)."""
+    eng = _rt.default_engine()
     if is_training:
-        raise NotImplementedError('encoder_resnet: the CUDA path is inference-only (is_training must be False)')
-    return _rt.default_engine().encode_images(x), 'resnet_v2_50'
+        return eng.encode_images_train(x), 'resnet_v2_50'
+    return eng.encode_images(x), 'resnet_v2_50'
 
 
 def az_fc2_groupnorm(is_training, net, num_conv_layers):
