@@ -13,7 +13,7 @@ void set_last_error_text(const char *what) { snprintf(t_err, sizeof(t_err), "%s"
 
 extern "C" {
 
-int hd_version(void) { return 106; }
+int hd_version(void) { return 107; }
 
 const char *hd_status_string(int s) {
   switch (s) {

@@ -23,6 +23,8 @@ BN_EPS = 1e-5        # resnet_arg_scope batch_norm_epsilon [TF-ext]
 # var_b * rows / (rows - 1) (the variance output of the fused kernel).  The fused op also raises an epsilon below 1.001e-5 to that
 # value; both trunks here use BN_EPS, as the inference trunk always has.  Pinned only through the TF stand-in (oracle/ref_exec).
 BN_DECAY = 0.997     # resnet_arg_scope batch_norm_decay [TF-ext]
+# Trunk backward conventions [TF-ext]: ReluGrad is 0 at 0; MaxPoolGrad of pool1 (3x3 stride 2 SAME) sends each window's gradient to its
+# FIRST maximum in scan order (ky, then kx), as TF's CPU kernel does (hd_maxpool3x3s2_same_backward).
 GN_EPS = 1e-6        # tf.contrib.layers.group_norm epsilon [TF-ext]
 GN_GROUPS = 32
 
@@ -122,6 +124,8 @@ class PackedConv(object):
         """Rewrite w_nk_hi / w_nk_lo on `stream` from the fp32 source `pack_src` (w_kn; for the gather layout its zero-padded copy
         [KH, segp, Cout] made at construction)."""
         src, KH, Cin = self.pack_src
+        if self.gather:                    # the zero-padded copy follows w_kn (a trainable weight changes in place)
+            src[:, :self.KW * self.Cin].copy_(self.w_kn.view(self.KH, self.KW * self.Cin, self.Cout))
         pack_weight(src, KH, Cin, self.Cout, self.w_nk_hi, self.w_nk_lo, stream)
 
     def bind(self, inp, n_img, H, W, out, in_ld=None, out_ld=None, pre=None, res=None, res_geom=None, impl='auto',
@@ -276,18 +280,24 @@ class PackedConv1Planes(object):
     A tile.  GEMM view: K = 8 kernel rows x 8 pixels x 4 channels = 256 (the 8th row / pixel / channel carry zero weights)."""
 
     def __init__(self, w_hwio, bias, device):
-        w = np.asarray(w_hwio, np.float32)
-        assert w.shape == (7, 7, 3, 64), w.shape
+        # w_hwio: a host array, or a device tensor (a trainable weight) that `repack` reads again
+        w = w_hwio if isinstance(w_hwio, torch.Tensor) else torch.from_numpy(np.asarray(w_hwio, np.float32))
+        assert tuple(w.shape) == (7, 7, 3, 64), tuple(w.shape)
         self.device = device
+        self.w = w
         self.Cout, self.K = 64, 256
-        wp = np.zeros((8, 8, 4, 64), np.float32)                   # [ky, kx, c, co]: K index ky*32 + kx*4 + c
-        wp[:7, :7, :3] = w
+        self.wp = torch.zeros((8, 8, 4, 64), dtype=torch.float32, device=device)    # [ky, kx, c, co]: K index ky*32 + kx*4 + c
         self.w_nk_hi = torch.empty((64, 256), dtype=torch.float16, device=device)
         self.w_nk_lo = torch.empty((64, 256), dtype=torch.float16, device=device)
         if _packs_on(device):
-            pack_weight(_dev(wp, device), 8, 32, 64, self.w_nk_hi, self.w_nk_lo, current_stream())
+            self.repack(current_stream())
         self.bias = _dev(bias, device)
         self.tmap_hi, self.tmap_lo = weight_tmap(self.w_nk_hi), weight_tmap(self.w_nk_lo)
+
+    def repack(self, stream):
+        """Rewrite the packs on `stream` from the current weight (through the zero-padded [8, 8, 4, 64] layout)."""
+        self.wp[:7, :7, :3].copy_(self.w)
+        pack_weight(self.wp, 8, 32, 64, self.w_nk_hi, self.w_nk_lo, stream)
 
     @staticmethod
     def plane_width(size):
@@ -326,7 +336,8 @@ class PackedResNet(object):
         p = 'resnet_v2_50'
         self.device = device
         self.blocks = blocks
-        self.conv1_w = _dev(np.asarray(w[p + '/conv1/weights'], np.float32).reshape(147, 64), device)
+        w1 = w[p + '/conv1/weights']          # a device tensor (a trainable weight) is read in place, like PackedConv's
+        self.conv1_w = w1.reshape(147, 64) if isinstance(w1, torch.Tensor) else _dev(np.asarray(w1, np.float32).reshape(147, 64), device)
         self.conv1_b = _dev(w[p + '/conv1/biases'], device)
         # conv2d_same(7x7, stride 2): explicit pad 3+3 then VALID (A.2); tensor-core path gathers the ragged K=147 element-wise
         self.conv1 = PackedConv(w[p + '/conv1/weights'], device, post_shift=w[p + '/conv1/biases'], stride=2, pad=(3, 3), tc=tc)
@@ -640,10 +651,17 @@ class ResNetTrainPlan(object):
 
     49 BatchStatsOps.  The scale / shift / mean / variance vectors are plan-owned device buffers rewritten on every run, so the
     descriptors never change.  `run` leaves the moving statistics alone; `apply_moving_update` takes the one step of the update ops
-    from this run's moments."""
+    from this run's moments.
 
-    def __init__(self, packed: PackedResNet, bn: ResNetBatchNorm, n, size=224, impl='auto'):
-        self.p, self.bn, self.n, self.size = packed, bn, n, size
+    keep=True (training the trunk, freeze_phi=False): the layer chain writes every map the backward reads into its own buffer -- the root
+    conv1 output, each unit's input and its raw conv1 / conv2 outputs -- instead of ping-ponging (about 32 MB per frame at 224 x 224);
+    the kernels, descriptors and arithmetic are the same, so the phis are bit-identical to keep=False.  `backward(dphi, images)` then
+    walks the units in reverse (csrc/resnet_grad.cu + hd_conv_gemm 3xTF32); it needs a `bwd` data-gradient pack on every conv but the
+    root's (trunk.TrainableResNet sets them)."""
+
+    def __init__(self, packed: PackedResNet, bn: ResNetBatchNorm, n, size=224, impl='auto', keep=False):
+        self.p, self.bn, self.n, self.size, self.keep = packed, bn, n, size, bool(keep)
+        self.generation = 0                   # runs so far: a recorded graph checks that its saved maps are still the plan's
         dev = packed.device
         H1 = size // 2
         H2 = (H1 + 1) // 2
@@ -655,17 +673,31 @@ class ResNetTrainPlan(object):
             mx_r = max(mx_r, h * h * unit['base'])
             h = ho
         f32 = dict(dtype=torch.float32, device=dev)
-        self.bufA, self.bufB, self.bufS = (torch.empty(n * mx_io, **f32) for _ in range(3))
-        self.bufR1, self.bufR2 = torch.empty(n * mx_r, **f32), torch.empty(n * mx_r, **f32)
+        self.mx_io, self.mx_r = mx_io, mx_r
+        if self.keep:                         # one buffer per kept map; bufS only carries the shortcut convs' outputs
+            self.bufS = torch.empty(n * mx_io, **f32)
+            self.root_out = torch.empty(n * H1 * H1 * 64, **f32)
+            self.xs, self.r1s, self.r2s, h = [torch.empty(n * H2 * H2 * 64, **f32)], [], [], H2
+            for unit in packed.units:
+                ho = (h - 1) // unit['stride'] + 1
+                self.r1s.append(torch.empty(n * h * h * unit['base'], **f32))
+                self.r2s.append(torch.empty(n * ho * ho * unit['base'], **f32))
+                self.xs.append(torch.empty(n * ho * ho * unit['depth'], **f32))
+                h = ho
+        else:
+            self.bufA, self.bufB, self.bufS = (torch.empty(n * mx_io, **f32) for _ in range(3))
+            self.bufR1, self.bufR2 = torch.empty(n * mx_r, **f32), torch.empty(n * mx_r, **f32)
+        root_out = self.root_out if self.keep else self.bufS
         L = bn.offsets[-1]
         self.scale, self.shift, self.mean, self.var = (torch.empty(L, **f32) for _ in range(4))
         self.planes = None
         self.conv1_op = None
         if packed.conv1_planes is not None and impl in ('auto', 'tc3h') and CONV1_PLANES and size % 2 == 0:
             self.planes = packed.conv1_planes.alloc_planes(n, size)
-            self.conv1_op = packed.conv1_planes.bind(self.planes, n, size, self.bufS)
+            self.conv1_op = packed.conv1_planes.bind(self.planes, n, size, root_out)
         elif packed.conv1.tc and impl != 'simt':
-            self.conv1_op = packed.conv1.bind(self.bufS, n, size, size, self.bufS, in_ld=3, impl=impl)
+            self.conv1_op = packed.conv1.bind(root_out, n, size, size, root_out, in_ld=3, impl=impl)
+        self.root_buf = root_out
         self.ops, self.stats = [], []
         shapes = []                           # (map, rows, C) of every normalised map, in scope order
         h = H2
@@ -687,10 +719,13 @@ class ResNetTrainPlan(object):
             return (op.scale, op.shift, 0, 1)
 
         raw = (None, None, False)
-        x, y, H = self.bufA, self.bufB, H2
-        for unit in packed.units:
+        x, y, H = (self.xs[0], None, H2) if self.keep else (self.bufA, self.bufB, H2)
+        self.pool_out = x
+        for ui, unit in enumerate(packed.units):
             s = unit['stride']
             Ho = (H - 1) // s + 1
+            if self.keep:
+                x, y, self.bufR1, self.bufR2 = self.xs[ui], self.xs[ui + 1], self.r1s[ui], self.r2s[ui]
             pre = stats(x, n * H * H, unit['d_in'])
             if 'shortcut' in unit:
                 self.ops.append(unit['shortcut'].bind(x, n, H, H, self.bufS, pre=pre, impl=impl))
@@ -707,6 +742,7 @@ class ResNetTrainPlan(object):
         self.final, self.final_hw = x, H * H
         self.tail = stats(x, n * H * H, packed.out_dim)
         assert len(self.stats) == len(bn.scopes)
+        self._bwd = None
 
     def run(self, images, out, stream=None):
         """images (n,size,size,3) contiguous float32 CUDA NHWC in [-1, 1] (None: the conv1 planes were filled by the caller) -> out
@@ -722,10 +758,11 @@ class ResNetTrainPlan(object):
             self.conv1_op.d.in_ = images.data_ptr()
             self.conv1_op.run(st)
         else:
-            check(lib.hd_conv1_7x7s2(fptr(images), fptr(p.conv1_w), fptr(p.conv1_b), fptr(self.bufS), n, self.size, self.size, st),
+            check(lib.hd_conv1_7x7s2(fptr(images), fptr(p.conv1_w), fptr(p.conv1_b), fptr(self.root_buf), n, self.size, self.size, st),
                   'hd_conv1_7x7s2')
-        check(lib.hd_maxpool3x3s2_same(fptr(self.bufS), fptr(self.bufA), n, self.H1, self.H1, 64, None, None, None, None, st),
+        check(lib.hd_maxpool3x3s2_same(fptr(self.root_buf), fptr(self.pool_out), n, self.H1, self.H1, 64, None, None, None, None, st),
               'hd_maxpool3x3s2_same')
+        self.generation += 1
         for op in self.ops:
             op.run(st)
         check(lib.hd_bnrelu_avgpool(fptr(self.final), fptr(self.tail[0]), fptr(self.tail[1]), fptr(out), n, self.final_hw, p.out_dim, st),
@@ -746,6 +783,151 @@ class ResNetTrainPlan(object):
     @property
     def num_launches(self):
         return (3 if self.planes is not None else 2) + sum(2 if isinstance(op, BatchStatsOp) else 1 for op in self.ops) + 1
+
+    # ---------------------------------------------------------------------------------------------------------------------------- backward
+    def unit_scopes(self):
+        """The variable scope of every bottleneck unit, in order."""
+        return ['resnet_v2_50/block%d/unit_%d/bottleneck_v2' % (b, u) for b, (_, units, _) in enumerate(self.p.blocks, start=1)
+                for u in range(1, units + 1)]
+
+    @property
+    def num_backward_launches(self):
+        """Kernel launches of one `backward`: 3 per batch-norm backward, 2 per weight gradient, 1 per data-gradient GEMM, zero
+        insertion and pool1 backward."""
+        out = 3 + 1 + 2                       # the tail's batch norm; pool1; the root conv's weight gradient
+        for unit in self.p.units:
+            out += 3 * 3 + 3 * 2 + 3 + (1 if unit['stride'] > 1 else 0) + (3 if 'shortcut' in unit else 0)
+        return out
+
+    def _backward_state(self):
+        """Scratch maps, workspaces and the data-gradient descriptors of `backward` (3xTF32 hd_conv_gemm over each conv's `bwd` pack),
+        made on the first call; every pointer is plan-owned, so the descriptors never change."""
+        if self._bwd is not None:
+            return self._bwd
+        if not self.keep:
+            raise _lib.HDError('ResNetTrainPlan.backward needs a plan built with keep=True (the maps the backward reads)')
+        p, n = self.p, self.n
+        f32 = dict(dtype=torch.float32, device=p.device)
+        G = [torch.empty(n * self.mx_io, **f32) for _ in range(2)]        # gradients of the unit outputs / inputs, alternating
+        D1, D2, Z = (torch.empty(n * self.mx_r, **f32) for _ in range(3))
+        P = torch.empty(n * self.mx_io, **f32)
+        ws_w = lib.hd_conv_wgrad_workspace_bytes(n * self.H1 * self.H1, 147, 64, 1)
+        ws_b = max(int(lib.hd_bn_relu_backward_workspace_bytes(op.rows, op.C)) for op in self.stats)
+        ops, H, U = [], self.H2, len(p.units)
+        for ui, unit in enumerate(p.units):
+            s, base, depth, d_in = unit['stride'], unit['base'], unit['depth'], unit['d_in']
+            Ho = (H - 1) // s + 1
+            for c in ('conv1', 'conv2', 'conv3', 'shortcut'):
+                if c in unit and getattr(unit[c], 'bwd', None) is None:
+                    raise _lib.HDError('ResNetTrainPlan.backward: %s of unit %d has no data-gradient pack' % (c, ui))
+            if 'shortcut' in unit and s != 1:
+                raise _lib.HDError('ResNetTrainPlan.backward: a strided shortcut conv is not part of resnet_v2_50')
+            k = U - 1 - ui
+            gy, gx = G[k % 2], G[(k + 1) % 2]
+            for pix, K, Cout, bias in ((Ho * Ho, base, depth, 1), (Ho * Ho, 9 * base, base, 0), (H * H, d_in, base, 0),
+                                       (H * H, d_in, depth, 1)):
+                ws_w = max(ws_w, lib.hd_conv_wgrad_workspace_bytes(n * pix, K, Cout, bias))
+            u = {'gy': gy, 'gx': gx, 'H': H, 'Ho': Ho}
+            u['conv3'] = _dgrad_op(unit['conv3'], gy, n, Ho, Ho, 1, D1)
+            u['conv2'] = _dgrad_op(unit['conv2'], D2 if s == 1 else Z, n, H, H, 3, D1)
+            if 'shortcut' in unit:
+                u['shortcut'] = _dgrad_op(unit['shortcut'], gy, n, H, H, 1, P)
+                u['conv1'] = _dgrad_op(unit['conv1'], D2, n, H, H, 1, P, res=P)
+            else:
+                u['conv1'] = _dgrad_op(unit['conv1'], D2, n, H, H, 1, P)
+            ops.append(u)
+            H = Ho
+        self._bwd = dict(G=G, D1=D1, D2=D2, Z=Z, P=P, units=ops, ws_w=torch.empty(max(16, int(ws_w)), dtype=torch.uint8, device=p.device),
+                         ws_b=torch.empty(max(16, ws_b), dtype=torch.uint8, device=p.device))
+        return self._bwd
+
+    def _bn_backward(self, i, dz, out, dgamma, dbeta, group=1, addend=None, add_geom=(0, 0, 0), stream=None):
+        op, bn, ws = self.stats[i], self.bn, self._bwd['ws_b']
+        check(lib.hd_bn_relu_backward(fptr(op.x), fptr(dz), int(group), op.rows, op.C, fptr(op.scale), fptr(op.shift), fptr(op.var),
+                                      fptr(op.gamma), BN_EPS, fptr(addend) if addend is not None else None, add_geom[0], add_geom[1],
+                                      add_geom[2], fptr(out), fptr(bn.view(dgamma, i)), fptr(bn.view(dbeta, i)),
+                                      C.c_void_p(ws.data_ptr()), ws.numel(), stream), 'hd_bn_relu_backward')
+
+    def _wgrad(self, x, geom, pre, dy, Cout, dw, db, stream):
+        """hd_conv_wgrad; geom = (n, H, W, Cin, Ho, Wo, KH, KW, stride, pad_t, pad_l); pre = a stats op (relu(bn(x))) or None."""
+        n, H, W, Cin, Ho, Wo, KH, KW, s, pt, pl = geom
+        ws = self._bwd['ws_w']
+        check(lib.hd_conv_wgrad(fptr(x), Cin, n, H, W, Cin, Ho, Wo, KH, KW, s, pt, pl, fptr(pre.scale) if pre is not None else None,
+                                fptr(pre.shift) if pre is not None else None, fptr(dy), Cout, Cout, fptr(dw),
+                                fptr(db) if db is not None else None, C.c_void_p(ws.data_ptr()), ws.numel(), stream), 'hd_conv_wgrad')
+
+    def backward(self, dphi, images, stream=None):
+        """Gradients of sum(phis * dphi) after the last `run` (keep=True), images (n,size,size,3) being that run's input: returns
+        {TF variable name: gradient} for the 53 conv weights (HWIO) and 21 biases, plus 'gamma' / 'beta': the batch-norm gradients as
+        flat vectors laid out like bn.gamma / bn.beta.  The images get no gradient.  Deterministic; `num_backward_launches` launches."""
+        st = current_stream() if stream is None else stream
+        S = self._backward_state()
+        p, n, bn = self.p, self.n, self.bn
+        dev = p.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        L = bn.offsets[-1]
+        dgamma, dbeta = torch.empty(L, **f32), torch.empty(L, **f32)
+        grads = {'gamma': dgamma, 'beta': dbeta}
+        G, D1, D2, Z, P = S['G'], S['D1'], S['D2'], S['Z'], S['P']
+        U = len(p.units)
+        # postnorm + ReLU + mean over H x W
+        self._bn_backward(3 * U, dphi.contiguous(), G[0], dgamma, dbeta, group=self.final_hw, stream=st)
+        scopes = self.unit_scopes()
+        for ui in range(U - 1, -1, -1):
+            unit, u, q = p.units[ui], S['units'][ui], scopes[ui]
+            s, base, depth, d_in, H, Ho = unit['stride'], unit['base'], unit['depth'], unit['d_in'], u['H'], u['Ho']
+            gy, gx = u['gy'], u['gx']
+            st0, st1, st2 = self.stats[3 * ui], self.stats[3 * ui + 1], self.stats[3 * ui + 2]
+            dW3, db3 = torch.empty((1, 1, base, depth), **f32), torch.empty(depth, **f32)
+            self._wgrad(self.r2s[ui], (n, Ho, Ho, base, Ho, Ho, 1, 1, 1, 0, 0), st2, gy, depth, dW3, db3, st)
+            u['conv3'].run(st)                                                          # d relu(bn(conv2 out)) -> D1
+            self._bn_backward(3 * ui + 2, D1, D2, dgamma, dbeta, stream=st)             # d conv2 out -> D2
+            dW2 = torch.empty((3, 3, base, base), **f32)
+            self._wgrad(self.r1s[ui], (n, H, H, base, Ho, Ho, 3, 3, s, 1, 1), st1, D2, base, dW2, None, st)
+            if s > 1:
+                check(lib.hd_zero_insert(fptr(D2), fptr(Z), n, Ho, Ho, base, s, H, H, st), 'hd_zero_insert')
+            u['conv2'].run(st)                                                          # d relu(bn(conv1 out)) -> D1
+            self._bn_backward(3 * ui + 1, D1, D2, dgamma, dbeta, stream=st)             # d conv1 out -> D2
+            dW1 = torch.empty((1, 1, d_in, base), **f32)
+            self._wgrad(self.xs[ui], (n, H, H, d_in, H, H, 1, 1, 1, 0, 0), st0, D2, base, dW1, None, st)
+            addend, geom = None, (0, 0, 0)
+            if 'shortcut' in unit:
+                dWs, dbs = torch.empty((1, 1, d_in, depth), **f32), torch.empty(depth, **f32)
+                self._wgrad(self.xs[ui], (n, H, H, d_in, H, H, 1, 1, 1, 0, 0), st0, gy, depth, dWs, dbs, st)
+                u['shortcut'].run(st)                                                   # d preact, shortcut path -> P
+                grads[q + '/shortcut/weights'], grads[q + '/shortcut/biases'] = dWs, dbs
+            else:
+                addend, geom = gy, ((0, 0, 0) if s == 1 else (H, H, s))
+            u['conv1'].run(st)                                                          # d preact (+ the shortcut's, in the epilogue) -> P
+            self._bn_backward(3 * ui, P, gx, dgamma, dbeta, addend=addend, add_geom=geom, stream=st)
+            grads[q + '/conv1/weights'], grads[q + '/conv2/weights'], grads[q + '/conv3/weights'] = dW1, dW2, dW3
+            grads[q + '/conv3/biases'] = db3
+        # pool1, then the root conv (7x7 stride 2, explicit pad 3) over the images
+        check(lib.hd_maxpool3x3s2_same_backward(fptr(self.root_buf), fptr(G[U % 2]), fptr(P), n, self.H1, self.H1, 64, st),
+              'hd_maxpool3x3s2_same_backward')
+        dW, db = torch.empty((7, 7, 3, 64), **f32), torch.empty(64, **f32)
+        self._wgrad(images, (n, self.size, self.size, 3, self.H1, self.H1, 7, 7, 2, 3, 3), None, P, 64, dW, db, st)
+        grads['resnet_v2_50/conv1/weights'], grads['resnet_v2_50/conv1/biases'] = dW, db
+        return grads
+
+
+def _dgrad_op(conv, inp, n, H, W, KH, out, res=None):
+    """The data gradient of a stride-1 KH x KH SAME conv (or, over the zero-inserted gradient, of a strided conv2d_same 3x3) as an
+    hd_conv_gemm op in its 3xTF32 mode: out[n, H, W, Cin] (+ res) = conv(inp [n, H, W, Cout], tap-flipped W^T = conv.bwd)."""
+    bwd = conv.bwd
+    d = ConvDesc()
+    d.in_, d.in_ld = inp.data_ptr(), conv.Cout
+    d.n_img, d.H, d.W, d.Cin = n, H, W, conv.Cout
+    d.Ho, d.Wo, d.KH, d.KW, d.stride, d.pad_t, d.pad_l = H, W, KH, KH, 1, KH // 2, KH // 2
+    d.w_kn = bwd.w_nk_hi.data_ptr()
+    d.w_nk_hi, d.w_nk_lo = bwd.w_nk_hi.data_ptr(), bwd.w_nk_lo.data_ptr()
+    d.Cout, d.K_pad = conv.Cin, KH * KH * conv.Cout
+    if res is not None:
+        d.res, d.res_ld, d.res_H, d.res_W, d.res_stride = res.data_ptr(), conv.Cin, H, W, 1
+    d.out, d.out_ld = out.data_ptr(), conv.Cin
+    d.impl = _lib.HD_IMPL_TC_3XTF32
+    d.tmap_hi, d.tmap_lo = C.cast(bwd.tmap_hi, C.c_void_p), C.cast(bwd.tmap_lo, C.c_void_p)
+    return ConvOp(d, (conv, bwd, inp, out, res), (H, W))
 
 
 # ------------------------------------------------------------------------------------------------

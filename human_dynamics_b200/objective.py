@@ -14,11 +14,14 @@ sum of its terms, with the weights of trainer_sequence_fc.py:280-310.
 With precomputed_phi=False (the reference's online-augmentation path) a batch carries `images` (B, T, S, S, 3) float32 in [-1, 1], e.g.
 augment.TubeAugmentor(...)['images'], instead of `phis`: the frozen ResNet runs over all B*T crops in training mode (batch statistics,
 nets.ResNetTrainPlan) without autograd, and each `step` applies the trunk's update ops once (one moving-average step of its 49
-batch-norm layers, decay 0.997), which save_checkpoint writes.
+batch-norm layers, decay 0.997), which save_checkpoint writes.  With freeze_phi=False as well, the trunk trains: its conv weights, biases
+and batch-norm gamma / beta (trunk.TrainableResNet) join E's optimizer, e_loss's gradient reaches them through the phis, and
+save_checkpoint writes their trained values.  Like the reference (whose gather_losses never adds slim's regularisation losses), the
+trunk trains without weight decay.
 
 Differences from the reference trainer: IEF dropout is the identity (the backward of trainable.TemporalModel follows the inference
 graph); torch's Adam adds eps to sqrt(v_hat) where TF's adds it to sqrt(v) before the bias correction; the static `use_hmr_only` branch
-and freeze_phi=False (it needs the trunk's backward) are not built.  A frame with no visible keypoint in an optimal-camera term
+is not built, and freeze_phi=False needs image input (precomputed phis have no trunk to train).  A frame with no visible keypoint in an optimal-camera term
 contributes 0 (the reference's procrustes2d_vis divides 0 / 0 there and the loss is NaN).  The moving statistics start from whatever
 `weights` holds, so a resumed run continues them; a fresh reference run restores only the trainable variables from its hmr_noS5
 checkpoint (trainer_sequence_fc.py:346-392), so its moving statistics start at 0 / 1 -- pass those values in `weights` to reproduce it.
@@ -337,17 +340,20 @@ class HMMRTrainer(object):
         self.config = config
         if config.do_hallucinate and not config.predict_delta:
             raise _lib.HDError('do_hallucinate needs predict_delta (the reference asserts it, src/config.py:271)')
-        if not config.freeze_phi:
-            raise _lib.HDError('freeze_phi=False is not built: training the ResNet needs its backward (conv data / weight gradients, '
-                               'batch-norm and max-pool backward)')
+        if not config.freeze_phi and config.precomputed_phi:
+            raise _lib.HDError('freeze_phi=False trains the ResNet, which needs image input: set precomputed_phi=False (precomputed '
+                               'phis have no trunk to train)')
         self.model = TemporalModel(weights, config, device=device)
-        self.trunk = None if config.precomputed_phi else _TrainTrunk(self.model._source, self.model.device)
+        self.trunk = None if config.precomputed_phi else _TrainTrunk(self.model._source, self.model.device,
+                                                                     trainable=not config.freeze_phi)
         self._pending = None                  # the trunk plan of the last forward: step applies its update ops
         self.disc = PoseDiscriminator(disc_weights, device=self.model.device) if disc_weights is not None else \
             PoseDiscriminator(seed=0, device=self.model.device)
         self.smpl = smpl_model if hasattr(smpl_model, 'consts') else SMPL(smpl_model)
         make = optimizer or (lambda params, lr: torch.optim.Adam(params, lr))
         self.e_params = list(self.model.parameters())
+        if self.trunk is not None and self.trunk.net is not None:     # get_unfrozen_E_vars without freeze_phi: the resnet_v2_50/* variables
+            self.e_params += list(self.trunk.net.parameters())
         self.d_params = list(self.disc.parameters())
         self.e_opt = make(self.e_params, config.e_lr)
         self.d_opt = make(self.d_params, config.d_lr)
@@ -440,10 +446,11 @@ class HMMRTrainer(object):
         return out
 
     def tf_variables(self):
-        """E and D variables; with image input the trunk's moving statistics are the current ones."""
+        """E and D variables; with image input the trunk's moving statistics are the current ones, and with freeze_phi=False its
+        trained weights, biases, gamma and beta as well."""
         v = self.model.tf_variables()
         if self.trunk is not None:
-            v.update(self.trunk.bn.moving())
+            v.update(self.trunk.bn.moving() if self.trunk.net is None else self.trunk.net.tf_variables())
         v.update(self.disc.tf_variables())
         return v
 
@@ -455,10 +462,11 @@ class HMMRTrainer(object):
 
 
 class _TrainTrunk(object):
-    """The frozen ResNet of an image-input trainer: packed once, one ResNetTrainPlan per (frames, size), the moving statistics shared by
-    all of them.  Called with images (B, T, S, S, 3) -> (phis (B, T, 2048) without autograd, the plan that made them)."""
+    """The ResNet of an image-input trainer: packed once, one ResNetTrainPlan per (frames, size), the moving statistics shared by all of
+    them.  Called with images (B, T, S, S, 3) -> (phis (B, T, 2048), the plan that made them): frozen, without autograd; trainable
+    (freeze_phi=False), on the graph of trunk.TrainableResNet."""
 
-    def __init__(self, w, device):
+    def __init__(self, w, device, trainable=False):
         from .nets import PackedResNet, ResNetBatchNorm
         p = 'resnet_v2_50'
         need = [p + '/conv1/weights', p + '/conv1/biases']
@@ -472,11 +480,17 @@ class _TrainTrunk(object):
         if missing:
             raise _lib.HDError('precomputed_phi=False runs the ResNet: weights lack %d resnet_v2_50 variables, e.g. %s'
                                % (len(missing), missing[0]))
+        self.device = device
+        self._plans = {}
+        self.net = None
+        if trainable:
+            from .trunk import TrainableResNet
+            self.net = TrainableResNet(w, device)
+            self.bn = self.net.bn
+            return
         with torch.cuda.device(device):
             self.bn = ResNetBatchNorm(w, device)
             self.packed = PackedResNet(w, device, tc='auto')
-        self.device = device
-        self._plans = {}
 
     def plan(self, n, size):
         from .nets import ResNetTrainPlan
@@ -494,6 +508,9 @@ class _TrainTrunk(object):
         if images.device != self.device:
             raise _lib.HDError('batch["images"] is on %s, the trainer on %s' % (images.device, self.device))
         B, T, S = int(images.shape[0]), int(images.shape[1]), int(images.shape[2])
+        if self.net is not None:
+            phis, plan = self.net(images.reshape(B * T, S, S, 3))
+            return phis.view(B, T, -1), plan
         plan = self.plan(B * T, S)
         phis = torch.empty((B * T, self.packed.out_dim), dtype=F32, device=self.device)
         with torch.no_grad():

@@ -158,6 +158,46 @@ int hd_bn_batch_stats(const float *x, long long rows, int C, long long ld, const
 int hd_bn_moving_update(const float *mean, const float *var, long long rows, int C, double decay, float *moving_mean, float *moving_var,
                         void *stream);
 
+/* ---- backward of the training-mode trunk (csrc/resnet_grad.cu): what the ResNet needs to train with freeze_phi=False
+ * (trainer_sequence_fc.py:681-685).  Deterministic: no atomics, every sum over a partition fixed by the shapes and merged in a fixed
+ * order, so repeats are bit-identical and results do not depend on the device's SM count.  Every argument is checked before any launch
+ * (HD_ERR_INVALID). ----
+ * hd_conv_wgrad: the weight gradient of a conv with hd_conv_gemm's geometry (x [n_img, H, W, Cin] at pixel pitch x_ld; output
+ *   [n_img, Ho, Wo, Cout]; input pixel of (oy, ox, ky, kx) = (oy*stride - pad_t + ky, ox*stride - pad_l + kx), zero outside):
+ *     dw[(ky*KW + kx)*Cin + ci, co] = sum_{n,oy,ox} a[n, iy, ix, ci] * dy[(n*Ho + oy)*Wo + ox][co]     (dy row pitch dy_ld)
+ *     a = relu(fma(x, pre_scale[ci], pre_shift[ci])) on real pixels when pre_scale is given (hd_conv_gemm's prologue; padding stays 0),
+ *     else x;   db[co] = sum of dy's column co (when db is non-NULL: one extra all-ones row of the GEMM's A operand).
+ *   An implicit GEMM on the tensor cores (wgmma m64n64k8 in the 3xTF32 split; a producer warpgroup gathers and splits the operands
+ *   into a 3-stage shared-memory ring, float4 gathers when Cin, Cout, x_ld, dy_ld % 4 == 0 and x, dy are 16-byte aligned), reduced over
+ *   the pixels in fixed chunks of 2048 whose fp32 partials hd_conv_wgrad_workspace_bytes(n_img*Ho*Wo, KH*KW*Cin, Cout, db != NULL)
+ *   bytes of workspace hold (the bias: per-chunk column sums of dy taken while loading it); a second launch adds them in chunk order
+ *   in fp64. */
+size_t hd_conv_wgrad_workspace_bytes(long long pixels, int K, int Cout, int bias);
+int hd_conv_wgrad(const float *x, long long x_ld, int n_img, int H, int W, int Cin, int Ho, int Wo, int KH, int KW, int stride, int pad_t,
+                  int pad_l, const float *pre_scale, const float *pre_shift, const float *dy, long long dy_ld, int Cout, float *dw, float *db,
+                  void *workspace, size_t workspace_bytes, void *stream);
+/* hd_bn_relu_backward: training-mode batch norm + ReLU backward over the raw map x [rows, C] (dense) that hd_bn_batch_stats normalised
+ * into scale / shift (and its biased variance var), gamma the layer's gamma:
+ *   z = fma(x, scale, shift), g = dz * (z > 0)  (TF's ReluGrad is 0 at 0), xhat = (x - mean_b) * rstd, rstd = 1 / sqrt(var + eps)
+ *   dbeta = sum_rows g,  dgamma = sum_rows g * xhat,  dx = gamma * rstd * (g - mean(g) - xhat * mean(g * xhat)) + addend
+ * with the batch mean re-accumulated in fp64 about row 0 (as hd_bn_batch_stats does), fp64 chunk partials merged in a fixed order.
+ * dz: [rows, C], or with dz_group > 1 [rows / dz_group, C] broadcast over each group of dz_group rows and divided by dz_group (the
+ * gradient of a mean over H x W: the tail's global pooling).  addend (nullable): added to dx, [rows, C]; with add_stride > 1 it is the
+ * dense [frames, ceil(add_H/s), ceil(add_W/s), C] gradient of x[:, ::s, ::s] (the strided identity shortcut), scattered to every s-th
+ * row and column of the [frames, add_H, add_W] map.  dx must not alias x, dz or addend.  Three launches; workspace
+ * hd_bn_relu_backward_workspace_bytes(rows, C) (16-byte aligned); C % 4 == 0, x 16-byte aligned, rows >= 2. */
+size_t hd_bn_relu_backward_workspace_bytes(long long rows, int C);
+int hd_bn_relu_backward(const float *x, const float *dz, int dz_group, long long rows, int C, const float *scale, const float *shift,
+                        const float *var, const float *gamma, float eps, const float *addend, int add_H, int add_W, int add_stride,
+                        float *dx, float *dgamma, float *dbeta, void *workspace, size_t workspace_bytes, void *stream);
+/* Backward of hd_maxpool3x3s2_same (pool1): in [N,H,W,C] the pool's input, dout [N,ceil(H/2),ceil(W/2),C] -> din [N,H,W,C].  Each window
+ * sends its gradient to one input, its FIRST maximum in scan order (ky, then kx) [TF-ext: TF's CPU MaxPoolGrad]; computed as a gather
+ * (each input adds the windows that chose it, in window order).  din must not alias in / dout. */
+int hd_maxpool3x3s2_same_backward(const float *in, const float *dout, float *din, int N, int H, int W, int C, void *stream);
+/* out [N,Ho,Wo,C] = in [N,Hi,Wi,C] spread to every stride-th row and column (out[n, y, x] = in[n, y/s, x/s] where y % s == 0 and
+ * x % s == 0, else 0): with it, the data gradient of a stride-s conv2d_same 3x3 is a stride-1 SAME conv over the flipped weights. */
+int hd_zero_insert(const float *in, float *out, int N, int Hi, int Wi, int C, int stride, int Ho, int Wo, void *stream);
+
 /* ---- crop pre-processing, the caller of the path: process_image (src/evaluation/run_video.py:56-107) + resize_img
  * (src/util/common.py:7-14), batched.  frames uint8 [N,H,W,3]; geom int32 [N,4] (16-byte aligned) = {Hs, Ws, x0, y0}: size of the
  * cv2.resize'd frame and the top-left corner of the SxS crop in its coordinates (may lie outside: edge replication = the
@@ -404,7 +444,8 @@ int hd_orth_proj_backward(const float *X, const float *cam, const float *dout, f
 enum { HD_PACK_FORWARD = 0, HD_PACK_BACKWARD_DATA = 1 };
 /* Device-side weight packing into the K-major [rows, k_pad] head / remainder layout of hd_conv_gemm's B operand (TMA maps from
  * hd_make_weight_tmap); the only writer of that layout.  w: fp32 [KH, Cin, Cout]: an FC [in, out] with KH = 1, or, in forward mode, any
- * HWIO conv with KH*KW passed as KH (backward-data mode: KW = 1).  elem_bytes 2 = fp16 head / 2^11-scaled remainder (impl 3), 4 = TF32
+ * HWIO conv with KH*KW passed as KH (backward-data mode too: the flip of the flattened (ky, kx) index, KH*KW-1-k, is the 2-D flip
+ * (KH-1-ky, KW-1-kx), so a KH x KW conv's pack is its dX conv over dY with SAME padding mirrored).  elem_bytes 2 = fp16 head / 2^11-scaled remainder (impl 3), 4 = TF32
  * head / remainder in fp32 storage (impl 1).
  *   HD_PACK_FORWARD:       dst[co, kh*Cin + ci] = W[kh, ci, co]  (hi = RN_f16(w), lo = RN_f16((w - hi) * 2^11); TF32: hi = RN_tf32(w),
  *                          lo = RN_tf32(w - hi));
