@@ -18,9 +18,10 @@
 //
 // N tile: 128 for pre-split layers with Cout > 64 that give the SMs enough tiles (wide_n_tile), 64 otherwise.  The 128-wide
 // tile needs 3 x 64 accumulator registers per consumer thread and halves the A gathers and the shared-memory reads per MMA
-// of the 64-wide one.
+// of the 64-wide one.  Pre-split 1x1 layers with K <= 128 (SHORT) flush the running sums once per tile, so they need only the
+// two fragments: 64-wide tiles, two CTAs per SM, one CTA's epilogue running under the other's loads and MMAs.
 //
-// Persistent: grid = min(#tiles, #SMs); each CTA walks tiles blockIdx.x, +gridDim.x, ...  Barrier phases run
+// Persistent: grid = min(#tiles, #SMs) (SHORT: 2 x #SMs); each CTA walks tiles blockIdx.x, +gridDim.x, ...  Barrier phases run
 // continuously across tiles, and the producers keep prefetching the next tile's chunks while the consumers run the
 // fused epilogue (scale/shift, residual, ReLU, fp32 output or its strided subsample, the next layer's fp16 pair)
 // straight from the accumulator fragments.  RES (pre-split input, residual row-aligned with the output, K <= 512): each
@@ -32,6 +33,7 @@
 //   warps 0-7    two consumer warpgroups: wgmma issue, drains, epilogue (warpgroup g owns tile rows 64 g .. 64 g + 63)
 //   warps 8-11   BN = 128 (384 threads): the cp.async A producers, 8 rows each; registers 256 x 232 + 128 x 40
 //   warps 8-15   BN = 64 (512 threads): the A producers, 4 rows each; registers 256 x 152 + 256 x 104
+//   warps 8-11   SHORT (384 threads, 2 CTAs per SM): the A producers, 8 rows each; registers 256 x 104 + 128 x 32
 // Producer thread 0 also issues the chunk's B tile (TMA).
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -51,31 +53,39 @@ constexpr int STAGE_OUT = 1, STAGE_PAIR = 2;
 
 using namespace ptx;
 
-template <bool HALF, bool ASPLIT, int BN, bool RES = false>
+// SHORT: pre-split layers with K <= PCH chunks (K <= 128), two CTAs per SM.  The running sums flush exactly once per tile, so the
+// flushed fragment itself holds them; the CTA has one operand stage, and each warpgroup's residual slot doubles as its output
+// staging.
+template <bool HALF, bool ASPLIT, int BN, bool RES = false, bool SHORT = false>
 struct Cfg {
   static_assert(BN == 64 || (BN == 128 && HALF && ASPLIT), "128-wide N tiles: pre-split fp16 path only");
   static_assert(!RES || ASPLIT, "residual by TMA: pre-split fp16 path only");
-  static constexpr int PROD_THREADS = BN == 128 ? 128 : 256;
+  static_assert(!SHORT || (BN == 64 && HALF && ASPLIT), "two CTAs per SM: 64-wide pre-split fp16 tiles only");
+  static constexpr int CTAS = SHORT ? 2 : 1;                    // CTAs per SM (__launch_bounds__, persistent grid)
+  static constexpr int PROD_THREADS = BN == 128 || SHORT ? 128 : 256;
   static constexpr int NUM_THREADS = 256 + PROD_THREADS;
   static constexpr int ROW_STEP = PROD_THREADS / 8;             // a producer thread's rows: rb + ROW_STEP * i
   static constexpr int ROWS = BM / ROW_STEP;
-  static constexpr int PROD_REGS = BN == 128 ? 40 : 104, CONS_REGS = BN == 128 ? 232 : 152;
-  static_assert(256 * CONS_REGS + PROD_THREADS * PROD_REGS <= 65536, "setmaxnreg split beyond the register file");
+  static constexpr int PROD_REGS = SHORT ? 32 : BN == 128 ? 40 : 104, CONS_REGS = SHORT ? 104 : BN == 128 ? 232 : 152;
+  static_assert(CTAS * (256 * CONS_REGS + PROD_THREADS * PROD_REGS) <= 65536, "setmaxnreg split beyond the register file");
   static constexpr int NACC = BN / 2;                           // fp32 registers of one m64nBN fragment per thread
   // RES: the residual slots do not fit beside three 64 KB stages (BN = 128) or four 48 KB ones plus the output staging (BN = 64).
   // Residual layers have K <= 512 (<= 8 chunks).
-  static constexpr int STAGES = BN == 128 ? (RES ? 2 : 3) : (RES ? 3 : 4);
+  static constexpr int STAGES = SHORT ? 1 : BN == 128 ? (RES ? 2 : 3) : (RES ? 3 : 4);
   static constexpr int BKE = HALF ? 64 : 32;                    // K elements per chunk (one 128-byte row)
   static constexpr int B_TILE_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
   static constexpr int RES_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr int RES_SLOT_BYTES = RES ? 64 * BN * 4 : 0; // one warpgroup's 64 rows x BN fp32 residual (BN / 32 TMA boxes)
-  static constexpr int STG_OFFSET = RES_OFFSET + 2 * RES_SLOT_BYTES;
+  // one warpgroup's 64 rows x BN fp32 residual (BN / 32 TMA boxes); SHORT: also the warpgroup's output staging
+  static constexpr int RES_SLOT_BYTES = RES || SHORT ? 64 * BN * 4 : 0;
+  static constexpr int STG_OFFSET = SHORT ? RES_OFFSET : RES_OFFSET + 2 * RES_SLOT_BYTES;
   // ASPLIT: one warpgroup's output staging, two 64-row x 128-byte TMA boxes (64 columns of fp32, or of the fp16 head and remainder)
   static constexpr int STG_BYTES = ASPLIT ? 2 * BOX_BYTES : 0;
-  static constexpr int BAR_OFFSET = STG_OFFSET + 2 * STG_BYTES;
+  static_assert(!SHORT || STG_BYTES == RES_SLOT_BYTES, "SHORT: the staging buffer is the residual slot");
+  static constexpr int BAR_OFFSET = SHORT ? RES_OFFSET + 2 * RES_SLOT_BYTES : STG_OFFSET + 2 * STG_BYTES;
   static constexpr int SMEM_BYTES = BAR_OFFSET + 128 + 1024;    // + alignment slack
   static_assert(SMEM_BYTES <= 232448, "dynamic shared memory beyond the 227 KB a CTA can opt into");
+  static_assert(CTAS * (SMEM_BYTES + 1024) <= 233472, "CTAS CTAs (and the 1 KB each reserves) beyond an SM's 228 KB");
   static constexpr int PF = HALF ? 2 : 3;                       // producer prefetch ring depth (chunks in flight per thread)
   static constexpr int V = HALF ? 2 : 1;                        // float4 loads per row per chunk per thread
 };
@@ -85,12 +95,14 @@ struct RowState {       // R output rows of one producer thread: image index and
   int n[R], iy[R], ix[R];
 };
 
-template <bool SPLIT, int PCH, bool HALF, bool GATHER, bool ASPLIT, int BN, bool RES>
-__global__ void __launch_bounds__((Cfg<HALF, ASPLIT, BN, RES>::NUM_THREADS), 1)
+template <bool SPLIT, int PCH, bool HALF, bool GATHER, bool ASPLIT, int BN, bool RES, bool SHORT>
+__global__ void __launch_bounds__((Cfg<HALF, ASPLIT, BN, RES, SHORT>::NUM_THREADS), (Cfg<HALF, ASPLIT, BN, RES, SHORT>::CTAS))
 conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap_hi, const __grid_constant__ CUtensorMap tmap_lo,
                     const __grid_constant__ CUtensorMap tmap_res, const __grid_constant__ CUtensorMap tmap_out,
                     const __grid_constant__ CUtensorMap tmap_out_hi, const __grid_constant__ CUtensorMap tmap_out_lo, const int stage) {
-  using C = Cfg<HALF, ASPLIT, BN, RES>;
+  using C = Cfg<HALF, ASPLIT, BN, RES, SHORT>;
+  // BN = 128 and SHORT keep the profile's start stamps and summed clocks in memory (hd_conv_gemm_profile): spill-free registers
+  constexpr bool MEM_STAMPS = BN == 128 || SHORT;
   constexpr int BKE = C::BKE, PF = C::PF, V = C::V, STAGES = C::STAGES, R = C::ROWS, RS = C::ROW_STEP, NA = C::NACC;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -126,8 +138,15 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     const int rb = t >> 3;                // rows rb + RS*i, i < R (all with the same row & 7, so one swizzle offset)
     const uint32_t sw_off = (uint32_t)((j ^ (rb & 7)) << 4);
     const bool prof = p.dbg != nullptr && blockIdx.x == 0 && t == 0;
-    long long t_wait = 0, t_start = prof && BN == 64 ? clock64() : 0;
-    if (BN == 128 && prof) p.dbg[0] = clock64();   // start stamp in memory, replaced by the loop's length: keeps 40 registers spill-free
+    long long t_wait = 0, t_start = prof && !MEM_STAMPS ? clock64() : 0;
+    if (MEM_STAMPS && prof) { p.dbg[0] = clock64(); p.dbg[1] = 0; }   // start stamp in memory, replaced by the loop's length
+    auto wait_empty = [&](int s, uint32_t ph) {     // MEM_STAMPS: the profile's wait clocks are summed in memory too
+      if (MEM_STAMPS && prof) p.dbg[1] -= clock64();
+      const long long tw0 = !MEM_STAMPS && prof ? clock64() : 0;
+      mbar_wait(empty_bar(s), ph ^ 1u);
+      if (!MEM_STAMPS && prof) t_wait += clock64() - tw0;
+      if (MEM_STAMPS && prof) p.dbg[1] += clock64();
+    };
     const int total = my_tiles * num_k;
     auto load_b = [&](int s, int ti, int kc) {      // producer thread 0: the chunk's B tile (weights, hi and lo) by TMA
       if (t != 0) return;
@@ -166,7 +185,8 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
       // ---- pre-split fp16 activations: cp.async straight into the swizzled tile, STAGES chunks in flight, no registers ----
       const __half *ihi = reinterpret_cast<const __half *>(p.in_hi);
       const __half *ilo = reinterpret_cast<const __half *>(p.in_lo);
-      if (!p.planes && p.KH * p.KW <= 32 && (long long)p.n_img * p.H * p.W * p.in_ld < (1ll << 31)) {
+      // SHORT: launch_conv_tc takes it for layers that meet the lean loop's conditions, and the other loops are not compiled
+      if (SHORT || (!p.planes && p.KH * p.KW <= 32 && (long long)p.n_img * p.H * p.W * p.in_ld < (1ll << 31))) {
         // Lean loop (on the long-K layers these warps can pace the whole kernel: the general loop below spends instructions per
         // chunk on two integer divisions and 64-bit addressing).  Per tile: one 32-bit
         // element offset and one tap-validity bit mask per row.  Per chunk: (tap, channel) advance incrementally -- a 64-wide chunk
@@ -197,22 +217,20 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
                   for (int xx = 0; xx < p.KW; ++xx, ++t)
                     if ((unsigned)(iy0 + yy) < (unsigned)p.H && (unsigned)(ix0 + xx) < (unsigned)p.W) mk |= 1u << t;
               }
-              base[i] = b;
+              base[i] = SHORT && !(mk & 1u) ? -1 : b;        // SHORT (1x1 windows): the row's one tap bit is the sign of its offset
               mask[i] = mk;
             }
             tap = 0; ci0 = 0; kx = 0; ky = 0; tap_off = 0;
           }
           const int s = q % STAGES;
           const uint32_t ph = (uint32_t)(q / STAGES) & 1u;
-          long long tw0 = prof ? clock64() : 0;
-          mbar_wait(empty_bar(s), ph ^ 1u);
-          if (prof) t_wait += clock64() - tw0;
+          wait_empty(s, ph);
           load_b(s, ti, kc);
           const uint32_t a_hi = smem_base + s * C::STAGE_BYTES + off0;
-          const int eo = tap_off + ci0;
+          const int eo = SHORT ? ci0 : tap_off + ci0;
 #pragma unroll
           for (int i = 0; i < R; ++i) {
-            const bool ok = (mask[i] >> tap) & 1u;
+            const bool ok = SHORT ? base[i] >= 0 : (mask[i] >> tap) & 1u;
             const int e = ok ? base[i] + eo : 0;
             cp_async16(a_hi + i * RS * 128, ihi + e, ok ? 16u : 0u);
             cp_async16(a_hi + A_TILE_BYTES + i * RS * 128, ilo + e, ok ? 16u : 0u);
@@ -226,7 +244,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           }
           if (++kc == num_k) { kc = 0; ++ti; }
         }
-      } else if (p.planes && (long long)p.n_img * p.H * p.W * p.in_ld < (1ll << 31)) {
+      } else if (!SHORT && p.planes && (long long)p.n_img * p.H * p.W * p.in_ld < (1ll << 31)) {
         // resnet conv1 over the padded RGBX fp16 planes, same lean scheme: Cin = 32 halves = one kernel row of 7(+1) pixels x 4, so a
         // 64-wide chunk holds TWO kernel rows (taps 2 kc and 2 kc + 1); this thread's 16-byte piece is pixels 2*(j&3), 2*(j&3)+1 of row
         // 2 kc + (j >> 2).  KH = 8: row 7 is a phantom (zero weights) and is zero-filled.  No padding tests: the planes are pre-padded.
@@ -255,9 +273,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           }
           const int s = q % STAGES;
           const uint32_t ph = (uint32_t)(q / STAGES) & 1u;
-          long long tw0 = prof ? clock64() : 0;
-          mbar_wait(empty_bar(s), ph ^ 1u);
-          if (prof) t_wait += clock64() - tw0;
+          wait_empty(s, ph);
           load_b(s, ti, kc);
           const uint32_t a_hi = smem_base + s * C::STAGE_BYTES + off0;
           const bool tap_ok = 2 * kc + jt < 7;
@@ -273,16 +289,14 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(full_bar(s)) : "memory");
           if (++kc == num_k) { kc = 0; ++ti; }
         }
-      } else {
+      } else if (!SHORT) {
       RowState<R> rs;
       int kc = 0, ti = 0;
       for (int q = 0; q < total; ++q) {
         if (kc == 0) enter_tile(ti, rs);
         const int s = q % STAGES;
         const uint32_t ph = (uint32_t)(q / STAGES) & 1u;
-        long long tw0 = prof ? clock64() : 0;
-        mbar_wait(empty_bar(s), ph ^ 1u);
-        if (prof) t_wait += clock64() - tw0;
+        wait_empty(s, ph);
         load_b(s, ti, kc);
         const int kb = kc * BKE;
         // planes (resnet conv1 over the padded RGBX fp16 planes, Cin = 32 halves = one kernel row of 7(+1) pixels x 4): a 64-wide
@@ -316,7 +330,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
       }
       cp_async_commit();
       cp_async_wait<0>();
-      if (prof) { p.dbg[0] = clock64() - (BN == 128 ? p.dbg[0] : t_start); p.dbg[1] = t_wait; }
+      if (prof) { p.dbg[0] = clock64() - (MEM_STAMPS ? p.dbg[0] : t_start); if (!MEM_STAMPS) p.dbg[1] = t_wait; }
     } else {
     RowState<R> pf_rs, st_rs;              // prefetch-side and store-side row state (may be one tile apart)
     float4 ring[PF][4 * V];
@@ -453,13 +467,15 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(C::CONS_REGS));
     const int wg = warp >> 2;                             // rows 64 wg .. 64 wg + 63 of the tile
     const bool prof = p.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 0;
-    long long t_wait = 0, t_start = prof && BN == 64 && !RES ? clock64() : 0;
-    if ((RES || BN == 128) && prof) p.dbg[2] = clock64();    // start stamp in memory (keeps the BN = 128 consumers within 232 registers spill-free)
+    long long t_wait = 0, t_start = prof && !MEM_STAMPS && !RES ? clock64() : 0;
+    if ((RES || MEM_STAMPS) && prof) p.dbg[2] = clock64();    // start stamp in memory (keeps the BN = 128 and SHORT consumers spill-free)
     if (prof) { p.dbg[3] = 0; p.dbg[4] = 0; p.dbg[5] = 0; p.dbg[6] = 0; }   // epilogue clocks and their split, summed in memory for the same reason
     const int hw = p.Ho * p.Wo;
     const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's fragment rows: frow, frow + 8
     const int fcol = 2 * (lane & 3);                            // and columns 8 j + fcol, + 1
-    float acc[NA], accx[NA], sums[NA];
+    // SHORT: the single flush per tile is done in place, so the running sums are acc itself and take no registers of their own
+    float acc[NA], accx[NA], sums_[SHORT ? 1 : NA];
+    float *const sums = SHORT ? acc : sums_;
 #pragma unroll
     for (int i = 0; i < NA; ++i) { acc[i] = 0.f; accx[i] = 0.f; }
     // RES: the warpgroup's 64 residual rows of a tile arrive by TMA in 32-column boxes (128-byte swizzle: row r at r * 128 B, its
@@ -482,17 +498,19 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     if (res_issuer && my_tiles > 0) load_res(0);
     int q = 0;
     for (int ti = 0; ti < my_tiles; ++ti) {
+      if (!SHORT) {
 #pragma unroll
-      for (int i = 0; i < NA; ++i) sums[i] = 0.f;
+        for (int i = 0; i < NA; ++i) sums[i] = 0.f;
+      }
       for (int kc = 0; kc < num_k; ++kc, ++q) {
         const int s = q % STAGES;
         const uint32_t ph = (uint32_t)(q / STAGES) & 1u;
         const bool group_start = (kc % PCH) == 0;
-        if (BN == 128 && prof) p.dbg[3] -= clock64();     // BN = 128: summed in memory, like the epilogue's clocks
-        const long long tw0 = BN == 64 && prof ? clock64() : 0;
+        if (MEM_STAMPS && prof) p.dbg[3] -= clock64();    // summed in memory, like the epilogue's clocks
+        const long long tw0 = !MEM_STAMPS && prof ? clock64() : 0;
         mbar_wait(full_bar(s), ph);
-        if (BN == 64 && prof) t_wait += clock64() - tw0;
-        if (BN == 128 && prof) p.dbg[3] += clock64();
+        if (!MEM_STAMPS && prof) t_wait += clock64() - tw0;
+        if (MEM_STAMPS && prof) p.dbg[3] += clock64();
         if (ASPLIT) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async (generic proxy) data -> wgmma (async proxy)
         const uint32_t a_hi = smem_base + s * C::STAGE_BYTES + wg * (64 * 128);
         const uint32_t a_lo = a_hi + A_TILE_BYTES;
@@ -528,10 +546,14 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         if (SPLIT) fence_regs(accx);
         __syncwarp();
         if (lane == 0) mbar_arrive(empty_bar(s));       // this warp's share of the stage has been read
-        if ((kc % PCH) == PCH - 1 || kc == num_k - 1) {
+        if (!SHORT && ((kc % PCH) == PCH - 1 || kc == num_k - 1)) {
 #pragma unroll
           for (int i = 0; i < NA; ++i) sums[i] += acc[i];      // round-to-nearest fp32 adds
         }
+      }
+      if (SHORT) {                                       // the one flush: 0 + acc, as above (a -0 becomes +0)
+#pragma unroll
+        for (int i = 0; i < NA; ++i) acc[i] = __fadd_rn(0.f, acc[i]);
       }
       if (SPLIT) {
 #pragma unroll
@@ -675,7 +697,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
             if (stg_issuer) bulk_commit();
           }
           if (p.out_hi) {
-            if (st2) acquire(RES && st32);
+            if (st2) acquire(RES && st32 && !SHORT);          // SHORT: the pair is staged in the slot the fp32 stores read
             if (st2) {
               uint8_t *brow = stg + (frow - 64 * wg) * 128 + 4 * (lane & 3);
               const float *vsc = p.post2_scale ? p.post2_scale + c0 + fcol : nullptr, *vsh = p.post2_shift ? p.post2_shift + c0 + fcol : nullptr;
@@ -783,7 +805,9 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         if (prof) p.dbg[6] -= clock64();
         named_bar_sync(1 + wg, 128);                       // every thread of the warpgroup has read the slot
         if (res_issuer) {
-          if (stage & STAGE_OUT) {                         // the slot's fp32 stores have read it (the pair's may still run)
+          if (SHORT) {                                     // every store staged in the slot has read it
+            if (stage) bulk_wait_read<0>();
+          } else if (stage & STAGE_OUT) {                  // the slot's fp32 stores have read it (the pair's may still run)
             if (stage & STAGE_PAIR) bulk_wait_read<1>();
             else bulk_wait_read<0>();
           }
@@ -794,7 +818,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
       if (prof) p.dbg[4] += clock64();
     }
     if (stg_issuer) bulk_wait_all();                       // the last stores have completed before the CTA exits
-    if (prof) { p.dbg[2] = clock64() - (RES || BN == 128 ? p.dbg[2] : t_start); if (BN == 64) p.dbg[3] = t_wait; }
+    if (prof) { p.dbg[2] = clock64() - (RES || MEM_STAMPS ? p.dbg[2] : t_start); if (!MEM_STAMPS) p.dbg[3] = t_wait; }
   }
 }
 
@@ -839,9 +863,9 @@ int encode_epilogue_map(CUtensorMap *tm, bool fp16, const void *base, int cols, 
   return HD_OK;
 }
 
-template <bool SPLIT, int PCH, bool HALF, bool GATHER = false, bool ASPLIT = false, int BN = 64, bool RES = false>
+template <bool SPLIT, int PCH, bool HALF, bool GATHER = false, bool ASPLIT = false, int BN = 64, bool RES = false, bool SHORT = false>
 int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
-  using C = Cfg<HALF, ASPLIT, BN, RES>;
+  using C = Cfg<HALF, ASPLIT, BN, RES, SHORT>;
   // function attributes and the SM count are per device: a process may drive several GPUs through this library
   static bool configured[kMaxDevices] = {};
   static int num_sms[kMaxDevices] = {};
@@ -849,7 +873,7 @@ int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= kMaxDevices) { set_last_error_text("conv_gemm_tc: device ordinal out of range"); return HD_ERR_UNSUPPORTED; }
   if (!configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES>,
+    cudaError_t e = cudaFuncSetAttribute(conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES, SHORT>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (e != cudaSuccess) { set_last_error("conv_gemm_tc attr", e); return HD_ERR_CUDA; }
     cudaDeviceGetAttribute(&num_sms[dev], cudaDevAttrMultiProcessorCount, dev);
@@ -886,8 +910,9 @@ int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
   }
   if (rc != HD_OK) return rc;
   const int num_tiles = ceil_div(p.M, BM) * ceil_div(p.Cout, BN);
-  dim3 grid(num_tiles < num_sms[dev] ? num_tiles : num_sms[dev]);     // persistent: one CTA per SM walks the tile list
-  conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES>
+  const int ctas = C::CTAS * num_sms[dev];       // persistent: one CTA per SM (SHORT: two) walks the tile list
+  dim3 grid(num_tiles < ctas ? num_tiles : ctas);
+  conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES, SHORT>
       <<<grid, C::NUM_THREADS, C::SMEM_BYTES, st>>>(p, thi, tlo, tres, tout, tohi, tolo, stage);
   return check_launch("conv_gemm_tc_kernel");
 }
@@ -903,6 +928,27 @@ bool wide_n_tile(const ConvParams &p) {
   const long long m_tiles = ceil_div(p.M, BM);
   const long long w128 = (m_tiles * ceil_div(p.Cout, 128) + sms - 1) / sms, w64 = (m_tiles * ceil_div(p.Cout, 64) + sms - 1) / sms;
   return 16 * w128 <= 9 * w64;      // 2 w128 <= 1.125 w64
+}
+
+// Whether the SHORT kernel runs two CTAs per SM on this device (checked once per device); if not, its layers keep the one-CTA kernels.
+template <bool RES>
+bool short_k_two_ctas() {
+  using C = Cfg<true, true, 64, RES, true>;
+  static int two[kMaxDevices] = {};      // 0 not checked yet, 1 yes, -1 no
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= kMaxDevices) return false;
+  if (two[dev] == 0) {
+    const auto kernel = conv_gemm_tc_kernel<true, 2, true, false, true, 64, RES, true>;
+    int n = 0;
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, C::NUM_THREADS, C::SMEM_BYTES) != cudaSuccess) {
+      (void)cudaGetLastError();
+      n = 0;
+    }
+    two[dev] = n >= 2 ? 1 : -1;
+  }
+  return two[dev] > 0;
 }
 
 }  // namespace
@@ -949,6 +995,14 @@ int launch_conv_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) 
     // the epilogue; vec_out (checked above) gives it the 16-byte aligned base and row pitch a tensor map needs.  Residual layers
     // have short K, so the 128-wide tile gives up its third stage for the slots.
     const bool res_rows = p.res && p.res_stride == 1 && p.res_H == p.Ho && p.res_W == p.Wo && p.K <= 8 * 64;
+    // K <= 128 (one running-sum flush per tile), 1x1 windows with 32-bit input offsets (the lean producer loop): the
+    // 64-wide tile two CTAs per SM, so one CTA's epilogue runs under the other's loads and MMAs.  Only for epilogues that add a
+    // row-aligned residual or write the next layer's pair: a layer that writes the fp32 output alone (block 1's shortcut conv)
+    // measured slower this way than on the 128-wide tile (DESIGN.md section 8).
+    const bool short_k = p.K <= 2 * 64 && p.KH * p.KW == 1 && (long long)p.n_img * p.H * p.W * p.in_ld < (1ll << 31) &&
+                         (p.res ? res_rows : p.out_hi != nullptr);
+    if (short_k && (res_rows ? short_k_two_ctas<true>() : short_k_two_ctas<false>()))
+      return res_rows ? launch_tc<true, 2, true, false, true, 64, true, true>(p, d, st) : launch_tc<true, 2, true, false, true, 64, false, true>(p, d, st);
     if (wide_n_tile(p))
       return res_rows ? launch_tc<true, 2, true, false, true, 128, true>(p, d, st) : launch_tc<true, 2, true, false, true, 128>(p, d, st);
     return res_rows ? launch_tc<true, 2, true, false, true, 64, true>(p, d, st) : launch_tc<true, 2, true, false, true>(p, d, st);
