@@ -11,11 +11,12 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libhd_b200.so')
 
-HD_IMPL_SIMT, HD_IMPL_TC_3XTF32, HD_IMPL_TC_1XTF32, HD_IMPL_TC_3XF16 = 0, 1, 2, 3
+HD_IMPL_SIMT, HD_IMPL_TC_3XTF32, HD_IMPL_TC_1XTF32, HD_IMPL_TC_3XF16, HD_IMPL_TC_1XF16 = 0, 1, 2, 3, 4
 HD_CONV_NO_TMA_EPILOGUE = 1
 HD_CONV_INPUT_PLANES = 2
 HD_PACK_FORWARD, HD_PACK_BACKWARD_DATA = 0, 1
-IMPL_BY_NAME = {'simt': HD_IMPL_SIMT, 'tc3': HD_IMPL_TC_3XTF32, 'tc1': HD_IMPL_TC_1XTF32, 'tc3h': HD_IMPL_TC_3XF16}
+IMPL_BY_NAME = {'simt': HD_IMPL_SIMT, 'tc3': HD_IMPL_TC_3XTF32, 'tc1': HD_IMPL_TC_1XTF32, 'tc3h': HD_IMPL_TC_3XF16,
+                'tc1h': HD_IMPL_TC_1XF16}
 
 
 class ConvDesc(C.Structure):

@@ -161,6 +161,8 @@ def tube_augment(frames, labels, centers, poses, gt3ds, walks, img_size, trans_m
     a.poses_out, a.gt3ds_out = poses_out.data_ptr(), gt3ds_out.data_ptr()
     a.crops = crops.data_ptr() if crops is not None else None
     if planes is not None:
+        if planes[1] is None:                 # hd_tube_augment writes both planes: a training-data path, FP32-class input
+            raise _lib.HDError("tube_augment: conv1 planes without a remainder (impl 'tc1h') are not a training input; use impl 'auto'")
         a.plane_hi, a.plane_lo, a.WP = planes[0].data_ptr(), planes[1].data_ptr(), planes[0].shape[2]
     check(lib.hd_tube_augment(C.byref(a), current_stream()), 'hd_tube_augment')
     return labels_out, centers_out, poses_out, gt3ds_out, geom

@@ -27,7 +27,10 @@ class HMMRConfig(object):
     smpl_model_path: str = ''
     weights: Any = None
     smpl_model: Any = None
-    impl: str = os.environ.get('HD_IMPL', 'auto')   # 'auto' (= 'tc3h' where Cin % 64 == 0, else 'tc3', else 'simt') | 'tc3h' | 'tc3' | 'tc1' | 'simt'
+    # 'auto' (= 'tc3h' where Cin % 64 == 0, else 'tc3', else 'simt') | 'tc3h' | 'tc3' | 'tc1' | 'simt': FP32-class except 'tc1' (1xTF32).
+    # 'tc1h': half-precision inference (HD_IMPL_TC_1XF16): the networks' GEMMs on fp16 heads alone, one MMA per product, no remainder
+    # buffers; about 1e-3 relative on the phis (DESIGN.md section 2).  SMPL stays FP32-class.  The training entries refuse it.
+    impl: str = os.environ.get('HD_IMPL', 'auto')
     frame_chunk: int = 160        # frames per pass of ResNet root + blocks 1-2 (activation working set vs. L2)
     late_chunk: int = 640         # frames per pass of ResNet blocks 3-4 (small maps: batch wide to fill 132 SMs)
     extra: dict = field(default_factory=dict)

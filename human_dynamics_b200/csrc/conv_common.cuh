@@ -41,8 +41,13 @@ __device__ __forceinline__ void split_f16x2(float a0, float a1, uint32_t &hi, ui
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 inline int fill_params(const hd_conv_desc *d, ConvParams &p) {
-  if (!d || !(d->in || (d->in_hi && d->in_lo)) || !(d->out || (d->out_hi && d->out_lo))) {
+  const bool heads = d && d->impl == HD_IMPL_TC_1XF16;    // pre-split operands are the fp16 heads alone
+  if (!d || !(d->in || (d->in_hi && (d->in_lo || heads))) || !(d->out || (d->out_hi && (d->out_lo || heads)))) {
     set_last_error_text("hd_conv_gemm: null in/out");
+    return HD_ERR_INVALID;
+  }
+  if (heads && (d->w_nk_lo || d->tmap_lo || d->tmap_lo_n64 || d->in_lo || d->out_lo)) {
+    set_last_error_text("hd_conv_gemm: impl 4 (1xFP16) reads and writes heads only: w_nk_lo, tmap_lo, tmap_lo_n64, in_lo and out_lo must be NULL");
     return HD_ERR_INVALID;
   }
   if (d->n_img <= 0 || d->H <= 0 || d->W <= 0 || d->Cin <= 0 || d->Cout <= 0 || d->KH <= 0 || d->KW <= 0 ||

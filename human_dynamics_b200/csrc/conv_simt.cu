@@ -246,7 +246,8 @@ static int conv_gemm_impl(const hd_conv_desc *d, void *stream, long long *dbg) {
   p.dbg = dbg;
   cudaStream_t st = (cudaStream_t)stream;
   if (d->impl == HD_IMPL_SIMT) return hd::launch_conv_simt(p, st);
-  if (d->impl == HD_IMPL_TC_3XTF32 || d->impl == HD_IMPL_TC_1XTF32 || d->impl == HD_IMPL_TC_3XF16) return hd::launch_conv_tc(p, d, st);
+  if (d->impl == HD_IMPL_TC_3XTF32 || d->impl == HD_IMPL_TC_1XTF32 || d->impl == HD_IMPL_TC_3XF16 || d->impl == HD_IMPL_TC_1XF16)
+    return hd::launch_conv_tc(p, d, st);
   hd::set_last_error_text("hd_conv_gemm: unknown impl");
   return HD_ERR_INVALID;
 }

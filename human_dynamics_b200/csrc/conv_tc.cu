@@ -2,6 +2,9 @@
 //
 //   D[128 x BN] (fp32)  =  sum over K chunks of   A_hi*B_hi  +  (A_lo*B_hi + A_hi*B_lo)
 //
+// SPLIT = false drops the bracket: one MMA per product on the heads alone (1xTF32, impl 2; 1xFP16, impl 4).  Nothing of a
+// remainder is then loaded, stored or kept: no A_lo / B_lo tiles in a stage, no cross-term fragment, no pair remainder written.
+//
 // A (activations) never exists in HBM in im2col form.  For pre-split fp16 activations (every ResNet trunk layer, the SMPL
 // blend GEMM) one producer warpgroup cp.asyncs the 128-row hi/lo pair of one K chunk straight into the 128-byte-swizzled
 // K-major layout the wgmma shared-memory descriptor expects.  Otherwise eight producer warps gather the tile (zero padding,
@@ -56,7 +59,7 @@ using namespace ptx;
 // SHORT: pre-split layers with K <= PCH chunks (K <= 128), two CTAs per SM.  The running sums flush exactly once per tile, so the
 // flushed fragment itself holds them; the CTA has one operand stage, and each warpgroup's residual slot doubles as its output
 // staging.
-template <bool HALF, bool ASPLIT, int BN, bool RES = false, bool SHORT = false>
+template <bool SPLIT, bool HALF, bool ASPLIT, int BN, bool RES = false, bool SHORT = false>
 struct Cfg {
   static_assert(BN == 64 || (BN == 128 && HALF && ASPLIT), "128-wide N tiles: pre-split fp16 path only");
   static_assert(!RES || ASPLIT, "residual by TMA: pre-split fp16 path only");
@@ -74,7 +77,10 @@ struct Cfg {
   static constexpr int STAGES = SHORT ? 1 : BN == 128 ? (RES ? 2 : 3) : (RES ? 3 : 4);
   static constexpr int BKE = HALF ? 64 : 32;                    // K elements per chunk (one 128-byte row)
   static constexpr int B_TILE_BYTES = BN * 128;
-  static constexpr int STAGE_BYTES = 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
+  // a stage: the A head tile (+ its remainder), then the B head tile (+ its remainder).  !SPLIT keeps the stage counts of the split
+  // kernels: the pipeline depth in chunks is the same, each chunk is half the bytes.
+  static constexpr int B_OFFSET = (SPLIT ? 2 : 1) * A_TILE_BYTES;
+  static constexpr int STAGE_BYTES = (SPLIT ? 2 : 1) * (A_TILE_BYTES + B_TILE_BYTES);
   static constexpr int RES_OFFSET = STAGES * STAGE_BYTES;
   // one warpgroup's 64 rows x BN fp32 residual (BN / 32 TMA boxes); SHORT: also the warpgroup's output staging
   static constexpr int RES_SLOT_BYTES = RES || SHORT ? 64 * BN * 4 : 0;
@@ -96,11 +102,11 @@ struct RowState {       // R output rows of one producer thread: image index and
 };
 
 template <bool SPLIT, int PCH, bool HALF, bool GATHER, bool ASPLIT, int BN, bool RES, bool SHORT>
-__global__ void __launch_bounds__((Cfg<HALF, ASPLIT, BN, RES, SHORT>::NUM_THREADS), (Cfg<HALF, ASPLIT, BN, RES, SHORT>::CTAS))
+__global__ void __launch_bounds__((Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT>::NUM_THREADS), (Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT>::CTAS))
 conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap_hi, const __grid_constant__ CUtensorMap tmap_lo,
                     const __grid_constant__ CUtensorMap tmap_res, const __grid_constant__ CUtensorMap tmap_out,
                     const __grid_constant__ CUtensorMap tmap_out_hi, const __grid_constant__ CUtensorMap tmap_out_lo, const int stage) {
-  using C = Cfg<HALF, ASPLIT, BN, RES, SHORT>;
+  using C = Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT>;
   // BN = 128 and SHORT keep the profile's start stamps and summed clocks in memory (hd_conv_gemm_profile): spill-free registers
   constexpr bool MEM_STAMPS = BN == 128 || SHORT;
   constexpr int BKE = C::BKE, PF = C::PF, V = C::V, STAGES = C::STAGES, R = C::ROWS, RS = C::ROW_STEP, NA = C::NACC;
@@ -151,7 +157,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     auto load_b = [&](int s, int ti, int kc) {      // producer thread 0: the chunk's B tile (weights, hi and lo) by TMA
       if (t != 0) return;
       const int n0 = (((int)blockIdx.x + ti * (int)gridDim.x) % tiles_n) * BN;
-      const uint32_t b_hi = smem_base + s * C::STAGE_BYTES + 2 * A_TILE_BYTES;
+      const uint32_t b_hi = smem_base + s * C::STAGE_BYTES + C::B_OFFSET;
       if (xmode & 2) { mbar_arrive(full_bar(s)); return; }
       // BN = 128: two 64-row boxes.  Weight rows are padded to 64, so the second box is either wholly inside the weights or
       // wholly past Cout; then it is not loaded, and the stale columns it would have filled only reach outputs c >= Cout,
@@ -233,7 +239,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
             const bool ok = SHORT ? base[i] >= 0 : (mask[i] >> tap) & 1u;
             const int e = ok ? base[i] + eo : 0;
             cp_async16(a_hi + i * RS * 128, ihi + e, ok ? 16u : 0u);
-            cp_async16(a_hi + A_TILE_BYTES + i * RS * 128, ilo + e, ok ? 16u : 0u);
+            if (SPLIT) cp_async16(a_hi + A_TILE_BYTES + i * RS * 128, ilo + e, ok ? 16u : 0u);
           }
           asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(full_bar(s)) : "memory");
           ci0 += BKE;
@@ -284,7 +290,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
             const int e = ok ? base[i] + eo : 0;
             // neighbouring output pixels read overlapping 64-byte windows (each 16-byte piece 4x): keep them in L1
             cp_async16_ca(a_hi + i * RS * 128, ihi + e, ok ? 16u : 0u);
-            cp_async16_ca(a_hi + A_TILE_BYTES + i * RS * 128, ilo + e, ok ? 16u : 0u);
+            if (SPLIT) cp_async16_ca(a_hi + A_TILE_BYTES + i * RS * 128, ilo + e, ok ? 16u : 0u);
           }
           asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(full_bar(s)) : "memory");
           if (++kc == num_k) { kc = 0; ++ti; }
@@ -315,10 +321,10 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           const uint32_t off = (uint32_t)(rb + RS * i) * 128u + sw_off;
           if (p.planes) {        // conv1: neighbouring output pixels read overlapping 64-byte windows (each 16-byte piece 4x): keep them in L1
             cp_async16_ca(a_hi + off, ihi + e, ok ? 16u : 0u);
-            cp_async16_ca(a_lo + off, ilo + e, ok ? 16u : 0u);
+            if (SPLIT) cp_async16_ca(a_lo + off, ilo + e, ok ? 16u : 0u);
           } else {
             cp_async16(a_hi + off, ihi + e, ok ? 16u : 0u);
-            cp_async16(a_lo + off, ilo + e, ok ? 16u : 0u);
+            if (SPLIT) cp_async16(a_lo + off, ilo + e, ok ? 16u : 0u);
           }
         }
         // the barrier itself is told to arrive (without a pending-count increment) once this thread's copies have landed:
@@ -474,10 +480,14 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's fragment rows: frow, frow + 8
     const int fcol = 2 * (lane & 3);                            // and columns 8 j + fcol, + 1
     // SHORT: the single flush per tile is done in place, so the running sums are acc itself and take no registers of their own
-    float acc[NA], accx[NA], sums_[SHORT ? 1 : NA];
+    // !SPLIT: no cross terms, so no accx fragment
+    float acc[NA], accx[SPLIT ? NA : 1], sums_[SHORT ? 1 : NA];
     float *const sums = SHORT ? acc : sums_;
 #pragma unroll
-    for (int i = 0; i < NA; ++i) { acc[i] = 0.f; accx[i] = 0.f; }
+    for (int i = 0; i < NA; ++i) {
+      acc[i] = 0.f;
+      if constexpr (SPLIT) accx[i] = 0.f;
+    }
     // RES: the warpgroup's 64 residual rows of a tile arrive by TMA in 32-column boxes (128-byte swizzle: row r at r * 128 B, its
     // 16-byte piece k at (k ^ (r & 7)) * 16), issued by the warpgroup's first thread as soon as the previous tile's epilogue has read
     // the slot, so the load overlaps the tile's main loop.  Boxes wholly past M or Cout are not loaded (their values are never read);
@@ -514,26 +524,30 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         if (ASPLIT) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async (generic proxy) data -> wgmma (async proxy)
         const uint32_t a_hi = smem_base + s * C::STAGE_BYTES + wg * (64 * 128);
         const uint32_t a_lo = a_hi + A_TILE_BYTES;
-        const uint32_t b_hi = smem_base + s * C::STAGE_BYTES + 2 * A_TILE_BYTES;
+        const uint32_t b_hi = smem_base + s * C::STAGE_BYTES + C::B_OFFSET;
         const uint32_t b_lo = b_hi + C::B_TILE_BYTES;
         const uint64_t da_hi = make_smem_desc(a_hi), da_lo = make_smem_desc(a_lo);
         const uint64_t db_hi = make_smem_desc(b_hi), db_lo = make_smem_desc(b_lo);
         fence_regs(acc);
-        if (SPLIT) fence_regs(accx);
+        if constexpr (SPLIT) fence_regs(accx);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < 4; ++k) {                // K = 8 tf32 / 16 fp16 = 32 bytes per wgmma: advance inside the swizzle row
           const uint64_t adv = (uint64_t)((k * 32) >> 4);
           if constexpr (BN == 128) {
-            wgmma_m64n128k16_f16(accx, da_lo + adv, db_hi + adv, (kc | k) != 0);
-            wgmma_m64n128k16_f16(accx, da_hi + adv, db_lo + adv, 1u);
+            if constexpr (SPLIT) {
+              wgmma_m64n128k16_f16(accx, da_lo + adv, db_hi + adv, (kc | k) != 0);
+              wgmma_m64n128k16_f16(accx, da_hi + adv, db_lo + adv, 1u);
+            }
             wgmma_m64n128k16_f16(acc, da_hi + adv, db_hi + adv, !(group_start && k == 0));
           } else if constexpr (HALF) {
-            wgmma_m64n64k16_f16(accx, da_lo + adv, db_hi + adv, (kc | k) != 0);
-            wgmma_m64n64k16_f16(accx, da_hi + adv, db_lo + adv, 1u);
+            if constexpr (SPLIT) {
+              wgmma_m64n64k16_f16(accx, da_lo + adv, db_hi + adv, (kc | k) != 0);
+              wgmma_m64n64k16_f16(accx, da_hi + adv, db_lo + adv, 1u);
+            }
             wgmma_m64n64k16_f16(acc, da_hi + adv, db_hi + adv, !(group_start && k == 0));
           } else {
-            if (SPLIT) {
+            if constexpr (SPLIT) {
               wgmma_m64n64k8_tf32(accx, da_lo + adv, db_hi + adv, (kc | k) != 0);
               wgmma_m64n64k8_tf32(accx, da_hi + adv, db_lo + adv, 1u);
             }
@@ -543,7 +557,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(acc);
-        if (SPLIT) fence_regs(accx);
+        if constexpr (SPLIT) fence_regs(accx);
         __syncwarp();
         if (lane == 0) mbar_arrive(empty_bar(s));       // this warp's share of the stage has been read
         if (!SHORT && ((kc % PCH) == PCH - 1 || kc == num_k - 1)) {
@@ -555,7 +569,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
 #pragma unroll
         for (int i = 0; i < NA; ++i) acc[i] = __fadd_rn(0.f, acc[i]);
       }
-      if (SPLIT) {
+      if constexpr (SPLIT) {
 #pragma unroll
         for (int i = 0; i < NA; ++i) sums[i] += accx[i] * (HALF ? (1.0f / 2048.0f) : 1.0f);
       }
@@ -719,7 +733,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
                   // columns 8 j + fcol, + 1 of the pass: piece jj of the 128-byte row
                   uint32_t *hs = reinterpret_cast<uint32_t *>(brow + h * 1024 + (((uint32_t)jj ^ rsw) * 16));
                   hs[0] = hh;
-                  hs[BOX_BYTES / 4] = ll;
+                  if (SPLIT) hs[BOX_BYTES / 4] = ll;
                 }
               }
             } else {
@@ -728,7 +742,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
               const int m = m0 + frow + 8 * h;
               if (m >= p.M) continue;
               __half *hrow = reinterpret_cast<__half *>(p.out_hi) + (size_t)m * p.out2_ld;
-              __half *lrow = reinterpret_cast<__half *>(p.out_lo) + (size_t)m * p.out2_ld;
+              __half *lrow = SPLIT ? reinterpret_cast<__half *>(p.out_lo) + (size_t)m * p.out2_ld : nullptr;
               uint8_t *brow = stg + (frow - 64 * wg + 8 * h) * 128 + 4 * (lane & 3);
 #pragma unroll
               for (int jj = 0; jj < 8; ++jj) {
@@ -740,10 +754,10 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
                 if (st2) {       // columns 8 j + fcol, + 1 of the pass: piece jj of the 128-byte row
                   uint32_t *hs = reinterpret_cast<uint32_t *>(brow + (((uint32_t)jj ^ rsw) * 16));
                   hs[0] = hh;
-                  hs[BOX_BYTES / 4] = ll;
+                  if (SPLIT) hs[BOX_BYTES / 4] = ll;
                 } else {
                   *reinterpret_cast<uint32_t *>(hrow + c) = hh;
-                  *reinterpret_cast<uint32_t *>(lrow + c) = ll;
+                  if (SPLIT) *reinterpret_cast<uint32_t *>(lrow + c) = ll;
                 }
               }
             }
@@ -753,7 +767,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
               named_bar_sync(3 + wg, 128);
               if (issue) {
                 tma_store_2d(&tmap_out_hi, stg_a, c0, r0);
-                tma_store_2d(&tmap_out_lo, stg_a + BOX_BYTES, c0, r0);
+                if (SPLIT) tma_store_2d(&tmap_out_lo, stg_a + BOX_BYTES, c0, r0);
               }
               if (stg_issuer) bulk_commit();
             }
@@ -770,7 +784,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         const float *rrow = res_row(m, n_img, oy, ox);
         float *orow = out_row(m, n_img, oy, ox);
         __half *hrow = p.out_hi ? reinterpret_cast<__half *>(p.out_hi) + (size_t)m * p.out2_ld : nullptr;
-        __half *lrow = p.out_hi ? reinterpret_cast<__half *>(p.out_lo) + (size_t)m * p.out2_ld : nullptr;
+        __half *lrow = SPLIT && p.out_hi ? reinterpret_cast<__half *>(p.out_lo) + (size_t)m * p.out2_ld : nullptr;
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
           const int c = n0 + 8 * j + fcol;
@@ -784,7 +798,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
               uint32_t hh, ll;
               pair2(c, y[0], y[1], hh, ll);
               *reinterpret_cast<uint32_t *>(hrow + c) = hh;
-              *reinterpret_cast<uint32_t *>(lrow + c) = ll;
+              if (SPLIT) *reinterpret_cast<uint32_t *>(lrow + c) = ll;
             }
           } else {             // ragged / unaligned outputs (IEF 85- and 72-wide heads): element-wise
 #pragma unroll
@@ -865,7 +879,7 @@ int encode_epilogue_map(CUtensorMap *tm, bool fp16, const void *base, int cols, 
 
 template <bool SPLIT, int PCH, bool HALF, bool GATHER = false, bool ASPLIT = false, int BN = 64, bool RES = false, bool SHORT = false>
 int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
-  using C = Cfg<HALF, ASPLIT, BN, RES, SHORT>;
+  using C = Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT>;
   // function attributes and the SM count are per device: a process may drive several GPUs through this library
   static bool configured[kMaxDevices] = {};
   static int num_sms[kMaxDevices] = {};
@@ -885,7 +899,7 @@ int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
   const void *mhi = d->tmap_hi_n64 ? d->tmap_hi_n64 : d->tmap_hi;
   const void *mlo = d->tmap_hi_n64 ? d->tmap_lo_n64 : d->tmap_lo;
   memcpy(&thi, mhi, sizeof(CUtensorMap));
-  memcpy(&tlo, mlo ? mlo : mhi, sizeof(CUtensorMap));     // mlo is null only for 1xTF32, which never loads it (launch_conv_tc)
+  memcpy(&tlo, mlo ? mlo : mhi, sizeof(CUtensorMap));     // mlo is null only without SPLIT, which never loads it (launch_conv_tc)
   // The residual and output maps are encoded here from p.res / p.out / p.out_hi / p.out_lo on every launch, never taken from the
   // descriptor's activation maps, so they always describe the buffers this launch reads and writes.  Maps not used stay copies
   // of the weight map.
@@ -906,7 +920,7 @@ int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
   if (ASPLIT && p.out_hi && p.out2_ld % 8 == 0) {
     stage |= STAGE_PAIR;
     if (rc == HD_OK) rc = encode_epilogue_map(&tohi, true, p.out_hi, p.Cout, p.M, p.out2_ld * 2, "output head");
-    if (rc == HD_OK) rc = encode_epilogue_map(&tolo, true, p.out_lo, p.Cout, p.M, p.out2_ld * 2, "output remainder");
+    if (rc == HD_OK && SPLIT) rc = encode_epilogue_map(&tolo, true, p.out_lo, p.Cout, p.M, p.out2_ld * 2, "output remainder");
   }
   if (rc != HD_OK) return rc;
   const int num_tiles = ceil_div(p.M, BM) * ceil_div(p.Cout, BN);
@@ -931,15 +945,15 @@ bool wide_n_tile(const ConvParams &p) {
 }
 
 // Whether the SHORT kernel runs two CTAs per SM on this device (checked once per device); if not, its layers keep the one-CTA kernels.
-template <bool RES>
+template <bool SPLIT, bool RES>
 bool short_k_two_ctas() {
-  using C = Cfg<true, true, 64, RES, true>;
+  using C = Cfg<SPLIT, true, true, 64, RES, true>;
   static int two[kMaxDevices] = {};      // 0 not checked yet, 1 yes, -1 no
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= kMaxDevices) return false;
   if (two[dev] == 0) {
-    const auto kernel = conv_gemm_tc_kernel<true, 2, true, false, true, 64, RES, true>;
+    const auto kernel = conv_gemm_tc_kernel<SPLIT, 2, true, false, true, 64, RES, true>;
     int n = 0;
     if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) != cudaSuccess ||
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, C::NUM_THREADS, C::SMEM_BYTES) != cudaSuccess) {
@@ -951,41 +965,19 @@ bool short_k_two_ctas() {
   return two[dev] > 0;
 }
 
-}  // namespace
-
-int launch_conv_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
-  const bool split_b = d->impl != HD_IMPL_TC_1XTF32;    // 1xTF32 reads no weight remainder
-  if (!d->tmap_hi || (split_b && !d->tmap_lo) || (!d->tmap_hi_n64 && d->tmap_lo_n64) || (d->tmap_hi_n64 && split_b && !d->tmap_lo_n64)) {
-    set_last_error_text("hd_conv_gemm(tc): missing tensor maps (tmap_hi/tmap_lo, and tmap_hi_n64/tmap_lo_n64 together or not at all)");
-    return HD_ERR_INVALID;
-  }
-  const bool half = d->impl == HD_IMPL_TC_3XF16;
-  const int bke = half ? 64 : 32;
-  // Compatibility gate, not a kernel limit: the register epilogue below writes the strided subsample for any descriptor, but
-  // out_subsample keeps the acceptance rule of the C-ABI (hd_b200.h: pre-split input, Cout % 32 == 0, a plain residual, the
-  // activation tensor maps given, HD_CONV_NO_TMA_EPILOGUE unset) so that a descriptor is accepted or refused as before.
-  if (p.out_sub) {
-    const bool res_plain = !p.res || (p.res_stride == 1 && p.res_H == p.Ho && p.res_W == p.Wo);
-    const bool maps = (!p.res || d->tmap_res) && (!p.out_hi || (d->tmap_out_hi && d->tmap_out_lo));
-    if (!p.in_hi || p.planes || !maps || !res_plain || p.Cout % 32 != 0 || (d->flags & HD_CONV_NO_TMA_EPILOGUE)) {
-      set_last_error_text("hd_conv_gemm: out_subsample needs the activation-map epilogue (pre-split input, Cout % 32 == 0, activation maps given)");
-      return HD_ERR_UNSUPPORTED;
-    }
-  }
-  if ((p.out_hi || p.in_hi) && (!half || !p.vec_out)) {
-    set_last_error_text("hd_conv_gemm(tc): pre-split activations need impl 3 and 16-byte aligned, 4-column-multiple outputs");
-    return HD_ERR_INVALID;
-  }
+// The fp16 paths: 3xFP16 (SPLIT, impl 3) or 1xFP16 (heads only, impl 4).  Both select the same kernel variant for a layer.
+template <bool SPLIT>
+int launch_conv_f16(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
   if (p.in_hi && p.planes) {           // resnet conv1 over padded RGBX fp16 planes (hd_pack_conv1_planes)
     if (p.Cin != 32 || p.KH != 8 || p.KW != 1 || p.stride != 2 || p.pad_t != 0 || p.pad_l != 0 || p.in_ld != 4 || p.Cout > 64 ||
         p.W % 2 != 0 || 2 * (p.Wo - 1) + 8 > p.W || 2 * (p.Ho - 1) + 7 > p.H || !aligned16(p.in_hi) || !aligned16(p.in_lo) || p.pre_scale) {
       set_last_error_text("hd_conv_gemm(tc planes): needs the conv1 plane geometry (Cin 32, KH 8, KW 1, stride 2, in_ld 4, even W)");
       return HD_ERR_INVALID;
     }
-    return launch_tc<true, 2, true, false, true>(p, d, st);
+    return launch_tc<SPLIT, 2, true, false, true>(p, d, st);
   }
-  // split modes: drain every 2 chunks = 8 (fp16) / 8 (tf32) tensor-core accumulations between round-to-nearest adds;
-  // 1xTF32 is ~1e-3 anyway: drain rarely
+  // drain every 2 chunks = 8 fp16 tensor-core accumulations between round-to-nearest adds (both modes: impl 4 then runs the
+  // rounded operations impl 3 runs on zero remainders)
   if (p.in_hi) {                       // pre-split fp16 activations: cp.async producer
     if (p.Cin % 64 != 0 || p.K % 64 != 0 || p.in_ld % 8 != 0 || !aligned16(p.in_hi) || !aligned16(p.in_lo) || p.pre_scale) {
       set_last_error_text("hd_conv_gemm(tc split-A): needs Cin % 64 == 0, in_ld % 8 == 0, aligned in_hi/in_lo, no prologue");
@@ -1001,26 +993,61 @@ int launch_conv_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) 
     // measured slower this way than on the 128-wide tile (DESIGN.md section 8).
     const bool short_k = p.K <= 2 * 64 && p.KH * p.KW == 1 && (long long)p.n_img * p.H * p.W * p.in_ld < (1ll << 31) &&
                          (p.res ? res_rows : p.out_hi != nullptr);
-    if (short_k && (res_rows ? short_k_two_ctas<true>() : short_k_two_ctas<false>()))
-      return res_rows ? launch_tc<true, 2, true, false, true, 64, true, true>(p, d, st) : launch_tc<true, 2, true, false, true, 64, false, true>(p, d, st);
+    if (short_k && (res_rows ? short_k_two_ctas<SPLIT, true>() : short_k_two_ctas<SPLIT, false>()))
+      return res_rows ? launch_tc<SPLIT, 2, true, false, true, 64, true, true>(p, d, st)
+                      : launch_tc<SPLIT, 2, true, false, true, 64, false, true>(p, d, st);
     if (wide_n_tile(p))
-      return res_rows ? launch_tc<true, 2, true, false, true, 128, true>(p, d, st) : launch_tc<true, 2, true, false, true, 128>(p, d, st);
-    return res_rows ? launch_tc<true, 2, true, false, true, 64, true>(p, d, st) : launch_tc<true, 2, true, false, true>(p, d, st);
+      return res_rows ? launch_tc<SPLIT, 2, true, false, true, 128, true>(p, d, st) : launch_tc<SPLIT, 2, true, false, true, 128>(p, d, st);
+    return res_rows ? launch_tc<SPLIT, 2, true, false, true, 64, true>(p, d, st) : launch_tc<SPLIT, 2, true, false, true>(p, d, st);
   }
-  if (half && p.Cin % bke != 0) {      // ragged Cin (resnet conv1: 7x7x3): element-wise gather producer, K zero-padded
+  if (p.Cin % 64 != 0) {               // ragged Cin (resnet conv1: 7x7x3): element-wise gather producer, K zero-padded
     const int segp = (p.KW * p.Cin + 7) & ~7;
     if (p.K_pad % 64 != 0 || p.K_pad < p.KH * segp || p.Cout > 64 || p.pre_scale || p.in_ld != p.Cin) {
       set_last_error_text("hd_conv_gemm(tc gather): needs K_pad % 64 == 0, K_pad >= KH*roundup8(KW*Cin), Cout <= 64, dense pixels, no prologue");
       return HD_ERR_INVALID;
     }
-    return launch_tc<true, 2, true, true>(p, d, st);
+    return launch_tc<SPLIT, 2, true, true>(p, d, st);
   }
-  if (!p.in || p.Cin % bke != 0 || p.in_ld % 4 != 0 || !aligned16(p.in) || p.K % bke != 0 ||
+  if (!p.in || p.in_ld % 4 != 0 || !aligned16(p.in) || p.K % 64 != 0 ||
       (p.pre_scale && (!aligned16(p.pre_scale) || !aligned16(p.pre_shift) || p.pre_img_stride % 4 != 0))) {
     set_last_error_text("hd_conv_gemm(tc): needs Cin % 32 (tf32) / % 64 (fp16) == 0 and 16-byte aligned input / prologue vectors");
     return HD_ERR_INVALID;
   }
-  if (half) return launch_tc<true, 2, true>(p, d, st);
+  return launch_tc<SPLIT, 2, true>(p, d, st);
+}
+
+}  // namespace
+
+int launch_conv_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
+  const bool heads = d->impl == HD_IMPL_TC_1XF16;                     // 1xFP16: fp16 heads only (fill_params refuses remainders)
+  const bool split_b = d->impl != HD_IMPL_TC_1XTF32 && !heads;       // 1xTF32 and 1xFP16 read no weight remainder
+  if (!d->tmap_hi || (split_b && !d->tmap_lo) || (!d->tmap_hi_n64 && d->tmap_lo_n64) || (d->tmap_hi_n64 && split_b && !d->tmap_lo_n64)) {
+    set_last_error_text("hd_conv_gemm(tc): missing tensor maps (tmap_hi/tmap_lo, and tmap_hi_n64/tmap_lo_n64 together or not at all)");
+    return HD_ERR_INVALID;
+  }
+  const bool half = d->impl == HD_IMPL_TC_3XF16 || heads;
+  // Compatibility gate, not a kernel limit: the register epilogue below writes the strided subsample for any descriptor, but
+  // out_subsample keeps the acceptance rule of the C-ABI (hd_b200.h: pre-split input, Cout % 32 == 0, a plain residual, the
+  // activation tensor maps given, HD_CONV_NO_TMA_EPILOGUE unset) so that a descriptor is accepted or refused as before.
+  if (p.out_sub) {
+    const bool res_plain = !p.res || (p.res_stride == 1 && p.res_H == p.Ho && p.res_W == p.Wo);
+    const bool maps = (!p.res || d->tmap_res) && (!p.out_hi || (d->tmap_out_hi && (heads || d->tmap_out_lo)));
+    if (!p.in_hi || p.planes || !maps || !res_plain || p.Cout % 32 != 0 || (d->flags & HD_CONV_NO_TMA_EPILOGUE)) {
+      set_last_error_text("hd_conv_gemm: out_subsample needs the activation-map epilogue (pre-split input, Cout % 32 == 0, activation maps given)");
+      return HD_ERR_UNSUPPORTED;
+    }
+  }
+  if ((p.out_hi || p.in_hi) && (!half || !p.vec_out)) {
+    set_last_error_text("hd_conv_gemm(tc): pre-split activations need impl 3 / 4 and 16-byte aligned, 4-column-multiple outputs");
+    return HD_ERR_INVALID;
+  }
+  if (half) return heads ? launch_conv_f16<false>(p, d, st) : launch_conv_f16<true>(p, d, st);
+  if (!p.in || p.Cin % 32 != 0 || p.in_ld % 4 != 0 || !aligned16(p.in) || p.K % 32 != 0 ||
+      (p.pre_scale && (!aligned16(p.pre_scale) || !aligned16(p.pre_shift) || p.pre_img_stride % 4 != 0))) {
+    set_last_error_text("hd_conv_gemm(tc): needs Cin % 32 (tf32) / % 64 (fp16) == 0 and 16-byte aligned input / prologue vectors");
+    return HD_ERR_INVALID;
+  }
+  // 3xTF32: drain every 2 chunks = 8 tensor-core accumulations; 1xTF32 is ~1e-3 anyway: drain rarely
   return d->impl != HD_IMPL_TC_1XTF32 ? launch_tc<true, 2, false>(p, d, st) : launch_tc<false, 8, false>(p, d, st);
 }
 

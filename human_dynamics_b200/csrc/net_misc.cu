@@ -38,7 +38,7 @@ __global__ void maxpool3x3s2_kernel(const float4 *__restrict__ in, float4 *__res
 #pragma unroll
     for (int e = 0; e < 2; ++e) hd::split_f16x2(y[2 * e], y[2 * e + 1], hp[e], lp[e]);
     out_hi[i] = make_uint2(hp[0], hp[1]);
-    out_lo[i] = make_uint2(lp[0], lp[1]);
+    if (out_lo) out_lo[i] = make_uint2(lp[0], lp[1]);
   }
 }
 
@@ -134,7 +134,7 @@ __global__ void process_image_kernel(const uint8_t *__restrict__ frames, int N, 
     hd::split_f16x2(v[2], 0.f, h1, l1);
     const size_t po = ((size_t)n * (S + 6) + y + 3) * WP + x + 3;
     plane_hi[po] = make_uint2(h0, h1);
-    plane_lo[po] = make_uint2(l0, l1);
+    if (plane_lo) plane_lo[po] = make_uint2(l0, l1);
   }
 }
 
@@ -152,7 +152,7 @@ __global__ void pack_conv1_planes_kernel(const float *__restrict__ img, uint2 *_
   hd::split_f16x2(__ldg(s + 2), 0.f, h1, l1);
   const size_t o = ((size_t)n * (H + 6) + y + 3) * WP + x + 3;
   hi[o] = make_uint2(h0, h1);
-  lo[o] = make_uint2(l0, l1);
+  if (lo) lo[o] = make_uint2(l0, l1);
 }
 
 // max_pool2d(1x1, stride s) = spatial subsampling: the identity shortcut of a strided bottleneck unit (A.4).
@@ -236,7 +236,7 @@ __global__ void __launch_bounds__(128) groupnorm_relu_split_kernel(const float *
     hd::split_f16x2(y, 0.f, h, l);
     const size_t o = base + (cg == 64 ? (size_t)(e >> 1) * C : (size_t)(i / cg) * C) + cin;
     out_hi[o] = __ushort_as_half((unsigned short)(h & 0xffffu));
-    out_lo[o] = __ushort_as_half((unsigned short)(l & 0xffffu));
+    if (out_lo) out_lo[o] = __ushort_as_half((unsigned short)(l & 0xffffu));
   }
 }
 
@@ -249,7 +249,7 @@ __global__ void split_f16_kernel(const float4 *__restrict__ x, uint2 *__restrict
   hd::split_f16x2(v.x, v.y, h0, l0);
   hd::split_f16x2(v.z, v.w, h1, l1);
   hi[i] = make_uint2(h0, h1);
-  lo[i] = make_uint2(l0, l1);
+  if (lo) lo[i] = make_uint2(l0, l1);
 }
 
 // IEF fc1, theta part (src/models.py:402,102: state = concat[phi, theta] -> fc1): h1 = relu(P + theta . W1[2048:]) with P = phi . W1[:2048]
@@ -297,7 +297,7 @@ __global__ void __launch_bounds__(256) ief_fc1_theta_kernel(const float *__restr
         hd::split_f16x2(y0, y1, h0, l0);
         hd::split_f16x2(y2, y3, h1, l1);
         *reinterpret_cast<uint2 *>(out_hi + o) = make_uint2(h0, h1);
-        *reinterpret_cast<uint2 *>(out_lo + o) = make_uint2(l0, l1);
+        if (out_lo) *reinterpret_cast<uint2 *>(out_lo + o) = make_uint2(l0, l1);
       }
     }
   }
@@ -383,7 +383,7 @@ int hd_conv1_7x7s2(const float *in, const float *w, const float *bias, float *ou
 int hd_maxpool3x3s2_same(const float *in, float *out, int N, int H, int W, int C, const float *scale, const float *shift,
                          void *out_hi, void *out_lo, void *stream) {
   HD_REQUIRE(in && (out || out_hi) && N > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0, "hd_maxpool3x3s2_same: bad arguments");
-  HD_REQUIRE((out_hi == nullptr) == (out_lo == nullptr) && (!out_hi || (scale && shift)), "hd_maxpool3x3s2_same: split output needs scale, shift, out_hi and out_lo");
+  HD_REQUIRE((out_hi || !out_lo) && (!out_hi || (scale && shift)), "hd_maxpool3x3s2_same: split output needs scale, shift and out_hi");
   const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
   const int pth = (Ho - 1) * 2 + 3 - H, ptw = (Wo - 1) * 2 + 3 - W;
   const int pt = (pth > 0 ? pth : 0) / 2, pl = (ptw > 0 ? ptw : 0) / 2;
@@ -421,7 +421,7 @@ int hd_ief_delta_init(const float *theta, float *dst, int dst_ld, int N, void *s
 extern "C" int hd_process_image(const unsigned char *frames, int N, int H, int W, const int *geom, float *out, int S, void *plane_hi,
                                 void *plane_lo, int WP, void *stream) {
   HD_REQUIRE(frames && geom && (out || plane_hi) && N > 0 && H > 0 && W > 0 && S > 0 && ((uintptr_t)geom & 15u) == 0 &&
-                 ((plane_hi == nullptr) == (plane_lo == nullptr)) && (!plane_hi || (WP >= S + 8 && WP % 2 == 0 && hd::aligned16(plane_hi) && hd::aligned16(plane_lo))),
+                 (plane_hi || !plane_lo) && (!plane_hi || (WP >= S + 8 && WP % 2 == 0 && hd::aligned16(plane_hi) && hd::aligned16(plane_lo))),
              "hd_process_image: bad arguments");
   const long long total = (long long)N * S * S;
   process_image_kernel<<<hd::ceil_div(total, 256), 256, 0, (cudaStream_t)stream>>>(frames, N, H, W, reinterpret_cast<const int4 *>(geom), out, S,
@@ -431,7 +431,7 @@ extern "C" int hd_process_image(const unsigned char *frames, int N, int H, int W
 }
 
 extern "C" int hd_pack_conv1_planes(const float *img, void *plane_hi, void *plane_lo, int N, int H, int W, int WP, void *stream) {
-  HD_REQUIRE(img && plane_hi && plane_lo && N > 0 && H > 0 && W > 0 && WP >= W + 8 && WP % 2 == 0 && hd::aligned16(plane_hi) &&
+  HD_REQUIRE(img && plane_hi && N > 0 && H > 0 && W > 0 && WP >= W + 8 && WP % 2 == 0 && hd::aligned16(plane_hi) &&
                  hd::aligned16(plane_lo),
              "hd_pack_conv1_planes: bad arguments");
   const long long total = (long long)N * H * W;
@@ -452,7 +452,7 @@ extern "C" int hd_subsample(const float *in, float *out, int N, int H, int W, in
 
 extern "C" int hd_groupnorm_relu_split(const float *x, const float *gamma, const float *beta, void *out_hi, void *out_lo, int B, int T, int C,
                                        int groups, float eps, void *stream) {
-  HD_REQUIRE(x && gamma && beta && out_hi && out_lo && B > 0 && T > 0 && C > 0 && groups > 0 && C % groups == 0 && T * (C / groups) <= 40 * 32,
+  HD_REQUIRE(x && gamma && beta && out_hi && B > 0 && T > 0 && C > 0 && groups > 0 && C % groups == 0 && T * (C / groups) <= 40 * 32,
              "hd_groupnorm_relu_split: bad arguments (T * C/groups must be <= 1280)");
   groupnorm_relu_split_kernel<<<hd::ceil_div((long long)B * groups, 4), 128, 0, (cudaStream_t)stream>>>(
       x, gamma, beta, reinterpret_cast<__half *>(out_hi), reinterpret_cast<__half *>(out_lo), B, T, C, groups, eps);
@@ -460,7 +460,7 @@ extern "C" int hd_groupnorm_relu_split(const float *x, const float *gamma, const
 }
 
 extern "C" int hd_split_f16(const float *x, void *hi, void *lo, long long n, void *stream) {
-  HD_REQUIRE(x && hi && lo && n > 0 && n % 4 == 0 && hd::aligned16(x) && hd::aligned16(hi) && hd::aligned16(lo), "hd_split_f16: bad arguments");
+  HD_REQUIRE(x && hi && n > 0 && n % 4 == 0 && hd::aligned16(x) && hd::aligned16(hi) && hd::aligned16(lo), "hd_split_f16: bad arguments");
   split_f16_kernel<<<hd::ceil_div(n / 4, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float4 *>(x), reinterpret_cast<uint2 *>(hi),
                                                                               reinterpret_cast<uint2 *>(lo), n / 4);
   return hd::check_launch("split_f16_kernel");
@@ -468,7 +468,7 @@ extern "C" int hd_split_f16(const float *x, void *hi, void *lo, long long n, voi
 
 extern "C" int hd_ief_fc1_theta(const float *P, const float *theta, int theta_ld, const float *W, int K, int C, void *out_hi, void *out_lo,
                                 float *out_f32, int N, void *stream) {
-  HD_REQUIRE(P && theta && W && (out_hi || out_f32) && ((out_hi == nullptr) == (out_lo == nullptr)) && N > 0 && K > 0 && K <= 96 && theta_ld >= K &&
+  HD_REQUIRE(P && theta && W && (out_hi || out_f32) && (out_hi || !out_lo) && N > 0 && K > 0 && K <= 96 && theta_ld >= K &&
                  C > 0 && C % 4 == 0 && hd::aligned16(P) && hd::aligned16(W) && (!out_hi || (hd::aligned16(out_hi) && hd::aligned16(out_lo))) &&
                  (!out_f32 || hd::aligned16(out_f32)),
              "hd_ief_fc1_theta: bad arguments");

@@ -14,7 +14,7 @@ import torch
 
 from . import _lib
 from .config import HMMRConfig
-from .nets import FMoviePlan, IEFPlan, PackedConv, PackedFMovie, PackedIEF, PackedResNet, ResNetPlan, sync_packing
+from .nets import FMoviePlan, IEFPlan, PackedConv, PackedFMovie, PackedIEF, PackedResNet, ResNetPlan, f16_pair, sync_packing
 from .smpl import SMPLConstants
 from ._lib import current_stream
 
@@ -92,6 +92,13 @@ class _Bounded(dict):
             while len(self) >= self.maxlen:
                 self.pop(next(iter(self)))
         super().__setitem__(key, value)
+
+
+def _rows(pair, i, n):
+    """Rows [i, i + n) of an fp16 activation pair (head, remainder or None); None stays None."""
+    if pair is None:
+        return None
+    return tuple(t[i:i + n] if t is not None else None for t in pair)
 
 
 class PackedHal(object):
@@ -186,8 +193,7 @@ class HMMREngine(object):
         if pa.split and pa.out_split is not None:
             skey = ('mid16', N, size)
             if skey not in self._phi:
-                self._phi[skey] = (torch.empty(mid.shape, dtype=torch.float16, device=self.device),
-                                   torch.empty(mid.shape, dtype=torch.float16, device=self.device))
+                self._phi[skey] = f16_pair(mid.shape, self.device, self.impl)      # 'tc1h': (head, None)
             mid_split = self._phi[skey]
         main = torch.cuda.current_stream()
         for i, n in self.stage_a_schedule(N, events is not None):
@@ -195,7 +201,7 @@ class HMMREngine(object):
             if events is not None:
                 for ev in events[i // self.H2D_PIECE:(i + n + self.H2D_PIECE - 1) // self.H2D_PIECE]:
                     main.wait_event(ev)
-            plan.set_output(mid[i:i + n], (mid_split[0][i:i + n], mid_split[1][i:i + n]) if mid_split else None)
+            plan.set_output(mid[i:i + n], _rows(mid_split, i, n))
             if frames is None:
                 with _nvtx('resnet root + blocks 1-2 [%d:%d]' % (i, i + n)):
                     plan.run(images[i:i + n], None, st)
@@ -204,7 +210,8 @@ class HMMREngine(object):
                 H, W = fr.shape[1], fr.shape[2]
                 if plan.planes is not None:
                     _lib.check(_lib.lib.hd_process_image(C.c_void_p(fr[i:i + n].data_ptr()), n, H, W, C.c_void_p(geom[i:i + n].data_ptr()), None,
-                                                         size, C.c_void_p(plan.planes[0].data_ptr()), C.c_void_p(plan.planes[1].data_ptr()),
+                                                         size, C.c_void_p(plan.planes[0].data_ptr()),
+                                                         C.c_void_p(plan.planes[1].data_ptr()) if plan.planes[1] is not None else None,
                                                          plan.planes[0].shape[2], st), 'hd_process_image')
                     plan.run(None, None, st)
                 else:                                 # conv1 without the plane path (simt / tc3 modes): materialise the fp32 crops
@@ -218,7 +225,7 @@ class HMMREngine(object):
         for i in range(0, N, cB):
             n = min(cB, N - i)
             plan = self._resnet_plan(n, size, 'B')
-            plan.set_input(mid[i:i + n], (mid_split[0][i:i + n], mid_split[1][i:i + n]) if mid_split else None)
+            plan.set_input(mid[i:i + n], _rows(mid_split, i, n))
             with _nvtx('resnet blocks 3-4 + pool5 [%d:%d]' % (i, i + n)):
                 plan.run(None, phi[i:i + n], st)
         return phi

@@ -29,6 +29,32 @@ GN_EPS = 1e-6        # tf.contrib.layers.group_norm epsilon [TF-ext]
 GN_GROUPS = 32
 
 
+# impl names whose networks run on the fp16 formats (pre-split activations, conv1 planes, fast heads).  'tc1h' is the half-precision
+# inference mode (HD_IMPL_TC_1XF16): the fp16 heads alone, one MMA per product, and no remainder buffers at all.
+F16_IMPLS = ('auto', 'tc3h', 'tc1h')
+
+
+def heads_only(impl):
+    """True for the half-precision inference mode: activation pairs are (head, None) and every descriptor leaves the remainders unset."""
+    return impl == 'tc1h'
+
+
+def f16_pair(shape, device, impl):
+    """The fp16 A-operand buffers of one activation: (head, remainder), or (head, None) in the half-precision mode."""
+    hi = torch.empty(shape, dtype=torch.float16, device=device)
+    return (hi, None) if heads_only(impl) else (hi, torch.empty(shape, dtype=torch.float16, device=device))
+
+
+def _vp(t):
+    return C.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def require_training_impl(impl, who):
+    """The training paths run FP32-class arithmetic (their backward passes and the saved activations they read): refuse 'tc1h'."""
+    if heads_only(impl):
+        raise _lib.HDError("%s: impl 'tc1h' is an inference-only half-precision mode; training runs FP32-class ('auto' / 'tc3h')" % who)
+
+
 def _dev(a, device, dtype=np.float32):
     if isinstance(a, torch.Tensor):           # already on the device (TemporalModel's parameters): used in place
         return a
@@ -96,7 +122,7 @@ class PackedConv(object):
         self.post_relu = bool(post_relu)
         self.tc = False            # False | 'f16' | 'tf32': which tensor-core packing this layer carries
         self.K_pad = 0
-        want = {True: 'f16', 'auto': 'f16', 'tc3h': 'f16', 'tc3': 'tf32', 'tc1': 'tf32'}.get(tc, tc)
+        want = {True: 'f16', 'auto': 'f16', 'tc3h': 'f16', 'tc1h': 'f16', 'tc3': 'tf32', 'tc1': 'tf32'}.get(tc, tc)
         gather = want == 'f16' and self.Cin % 32 != 0 and self.Cout <= 64   # conv1: row-segment gather producer
         if want == 'f16' and self.Cin % 64 != 0 and not gather:
             want = 'tf32'
@@ -138,14 +164,18 @@ class PackedConv(object):
         out_subsample = s > 1: `out` is the dense [n, ceil(Ho/s), ceil(Wo/s), Cout] tensor x[:, ::s, ::s] (hd_b200.h);
         inp_split = (hi, lo) fp16 tensors: pre-activated, pre-split A operand (then `inp` may be None);
         out_split = (hi, lo) fp16 tensors + post2 = (scale|None, shift|None, relu): second output (then `out` may be None).
+        impl 'tc1h' (half precision, HD_IMPL_TC_1XF16): the pairs are (hi, None) and no remainder pointer is set.
         """
         d = ConvDesc()
         Ho = (H + 2 * self.pad_t - self.KH) // self.stride + 1 if self.KH > 1 else (H - 1) // self.stride + 1
         Wo = (W + 2 * self.pad_l - self.KW) // self.stride + 1 if self.KW > 1 else (W - 1) // self.stride + 1
         d.in_ = inp.data_ptr() if inp is not None else None
         d.in_ld = self.Cin if in_ld is None else in_ld
+        heads = heads_only(impl)
         if inp_split is not None:
-            d.in_hi, d.in_lo = inp_split[0].data_ptr(), inp_split[1].data_ptr()
+            d.in_hi = inp_split[0].data_ptr()
+            if not heads:
+                d.in_lo = inp_split[1].data_ptr()
         d.n_img, d.H, d.W, d.Cin = n_img, H, W, self.Cin
         d.Ho, d.Wo, d.KH, d.KW = Ho, Wo, self.KH, self.KW
         d.stride, d.pad_t, d.pad_l = self.stride, self.pad_t, self.pad_l
@@ -170,7 +200,9 @@ class PackedConv(object):
         d.out_ld = self.Cout if out_ld is None else out_ld
         d.out_subsample = int(out_subsample) if out is not None else 0
         if out_split is not None:
-            d.out_hi, d.out_lo, d.out2_ld = out_split[0].data_ptr(), out_split[1].data_ptr(), self.Cout
+            d.out_hi, d.out2_ld = out_split[0].data_ptr(), self.Cout
+            if not heads:
+                d.out_lo = out_split[1].data_ptr()
             if post2 is not None:
                 if post2[0] is not None:
                     d.post2_scale = post2[0].data_ptr()
@@ -178,18 +210,20 @@ class PackedConv(object):
                     d.post2_shift = post2[1].data_ptr()
                 d.post2_relu = int(post2[2])
         # ragged layers (Cin % 32 != 0, unaligned views) always run on the exact-FP32 SIMT kernel
-        use_tc = bool(self.tc) and impl in ('auto', 'tc3', 'tc1', 'tc3h') and \
+        use_tc = bool(self.tc) and impl in ('auto', 'tc3', 'tc1', 'tc3h', 'tc1h') and \
             (self.gather or inp_split is not None or ((d.in_ld % 4 == 0) and (inp.data_ptr() % 16 == 0)))
         if (inp_split is not None or out_split is not None) and not (use_tc and self.tc == 'f16'):
-            raise _lib.HDError('pre-split activations need the fp16 tensor-core packing (impl auto / tc3h, Cin % 64 == 0)')
+            raise _lib.HDError('pre-split activations need the fp16 tensor-core packing (impl auto / tc3h / tc1h, Cin % 64 == 0)')
         if use_tc:
             if self.tc == 'f16':
-                d.impl = _lib.HD_IMPL_TC_3XF16
+                d.impl = _lib.HD_IMPL_TC_1XF16 if heads else _lib.HD_IMPL_TC_3XF16
             else:
-                d.impl = _lib.HD_IMPL_TC_1XTF32 if impl == 'tc1' else _lib.HD_IMPL_TC_3XTF32
-            d.w_nk_hi, d.w_nk_lo = self.w_nk_hi.data_ptr(), self.w_nk_lo.data_ptr()
+                d.impl = _lib.HD_IMPL_TC_1XTF32 if impl in ('tc1', 'tc1h') else _lib.HD_IMPL_TC_3XTF32
+            d.w_nk_hi = self.w_nk_hi.data_ptr()
             d.tmap_hi = C.cast(self.tmap_hi, C.c_void_p)
-            d.tmap_lo = C.cast(self.tmap_lo, C.c_void_p)
+            if not heads:
+                d.w_nk_lo = self.w_nk_lo.data_ptr()
+                d.tmap_lo = C.cast(self.tmap_lo, C.c_void_p)
         else:
             d.impl = _lib.HD_IMPL_SIMT
         op = ConvOp(d, (self, inp, out, pre, res, inp_split, out_split, post2, post), (Ho, Wo))
@@ -237,7 +271,7 @@ class ConvOp(object):
         the C-ABI rule of hd_b200.h.  Layers that qualify: fp16-split input, Cout % 32 == 0, residual row == output row."""
         d = self.d
         K = d.KH * d.KW * d.Cin
-        ok = (d.impl == _lib.HD_IMPL_TC_3XF16 and d.in_hi and d.Cout % 32 == 0 and
+        ok = (d.impl in (_lib.HD_IMPL_TC_3XF16, _lib.HD_IMPL_TC_1XF16) and d.in_hi and d.Cout % 32 == 0 and
               (not d.res or (d.res_stride == 1 and d.res_H == d.Ho and d.res_W == d.Wo)))
         for f in ('tmap_res', 'tmap_out', 'tmap_out_hi', 'tmap_out_lo'):
             setattr(d, f, None)
@@ -303,15 +337,20 @@ class PackedConv1Planes(object):
     def plane_width(size):
         return (size + 8 + 1) // 2 * 2
 
-    def alloc_planes(self, n, size):
-        """Zero-initialised planes: the 3-pixel border (and the spare columns) must be zero and is never written again."""
+    def alloc_planes(self, n, size, impl='auto'):
+        """Zero-initialised planes: the 3-pixel border (and the spare columns) must be zero and is never written again.  'tc1h': the
+        head plane alone, (hi, None)."""
         shape = (n, size + 6, self.plane_width(size), 4)
-        return (torch.zeros(shape, dtype=torch.float16, device=self.device), torch.zeros(shape, dtype=torch.float16, device=self.device))
+        hi = torch.zeros(shape, dtype=torch.float16, device=self.device)
+        return (hi, None) if heads_only(impl) else (hi, torch.zeros(shape, dtype=torch.float16, device=self.device))
 
-    def bind(self, planes, n, size, out):
+    def bind(self, planes, n, size, out, impl='auto'):
         d = ConvDesc()
         WP = self.plane_width(size)
-        d.in_hi, d.in_lo = planes[0].data_ptr(), planes[1].data_ptr()
+        heads = heads_only(impl)
+        d.in_hi = planes[0].data_ptr()
+        if not heads:
+            d.in_lo = planes[1].data_ptr()
         d.in_ld = 4
         d.n_img, d.H, d.W, d.Cin = n, size + 6, WP, 32
         d.Ho = d.Wo = size // 2
@@ -319,9 +358,10 @@ class PackedConv1Planes(object):
         d.Cout, d.K_pad = 64, 256
         d.post_shift = self.bias.data_ptr()
         d.out, d.out_ld = out.data_ptr(), 64
-        d.impl = _lib.HD_IMPL_TC_3XF16
-        d.w_nk_hi, d.w_nk_lo = self.w_nk_hi.data_ptr(), self.w_nk_lo.data_ptr()
-        d.tmap_hi, d.tmap_lo = C.cast(self.tmap_hi, C.c_void_p), C.cast(self.tmap_lo, C.c_void_p)
+        d.impl = _lib.HD_IMPL_TC_1XF16 if heads else _lib.HD_IMPL_TC_3XF16
+        d.w_nk_hi, d.tmap_hi = self.w_nk_hi.data_ptr(), C.cast(self.tmap_hi, C.c_void_p)
+        if not heads:
+            d.w_nk_lo, d.tmap_lo = self.w_nk_lo.data_ptr(), C.cast(self.tmap_lo, C.c_void_p)
         d.flags = _lib.HD_CONV_INPUT_PLANES | (0 if TMA_EPILOGUE else _lib.HD_CONV_NO_TMA_EPILOGUE)
         op = ConvOp(d, (self, planes, out), (size // 2, size // 2))
         op.encode_act_maps()
@@ -341,7 +381,7 @@ class PackedResNet(object):
         self.conv1_b = _dev(w[p + '/conv1/biases'], device)
         # conv2d_same(7x7, stride 2): explicit pad 3+3 then VALID (A.2); tensor-core path gathers the ragged K=147 element-wise
         self.conv1 = PackedConv(w[p + '/conv1/weights'], device, post_shift=w[p + '/conv1/biases'], stride=2, pad=(3, 3), tc=tc)
-        want = {True: 'f16', 'auto': 'f16', 'tc3h': 'f16'}.get(tc, None)
+        want = {True: 'f16', 'auto': 'f16', 'tc3h': 'f16', 'tc1h': 'f16'}.get(tc, None)
         self.conv1_planes = PackedConv1Planes(w[p + '/conv1/weights'], w[p + '/conv1/biases'], device) if want == 'f16' else None
         self.units = []
         d_in = 64
@@ -410,7 +450,8 @@ class ResNetPlan(object):
         f16 = dict(dtype=torch.float16, device=dev)
         # split mode: every conv reads its A operand as a pre-activated fp16 head/remainder pair written by the producing
         # epilogue (cp.async straight into the swizzled tile, DESIGN.md 4.1); fp32 copies exist only where a residual needs them
-        self.split = impl in ('auto', 'tc3h') and all(
+        self.impl = impl
+        self.split = impl in F16_IMPLS and all(
             c.tc == 'f16' and not c.gather for u in packed.units[lo:hi] for k, c in u.items() if isinstance(c, PackedConv))
         self.bufA = torch.empty(n * mx_io, **f32)
         self.bufB = torch.empty(n * mx_io, **f32)
@@ -418,9 +459,9 @@ class ResNetPlan(object):
         self.ops = []
         self.conv1_op = None
         self.planes = None
-        if root and packed.conv1_planes is not None and impl in ('auto', 'tc3h') and CONV1_PLANES and size % 2 == 0:
-            self.planes = packed.conv1_planes.alloc_planes(n, size)
-            self.conv1_op = packed.conv1_planes.bind(self.planes, n, size, self.bufS)
+        if root and packed.conv1_planes is not None and impl in F16_IMPLS and CONV1_PLANES and size % 2 == 0:
+            self.planes = packed.conv1_planes.alloc_planes(n, size, impl)
+            self.conv1_op = packed.conv1_planes.bind(self.planes, n, size, self.bufS, impl)
         elif root and packed.conv1.tc and impl != 'simt':
             self.conv1_op = packed.conv1.bind(self.bufS, n, size, size, self.bufS, in_ld=3, impl=impl)   # `in_` is set per run
         self.in_refs = []                     # (op, field) descriptor fields that read the stage input
@@ -429,8 +470,8 @@ class ResNetPlan(object):
         x, y = self.bufA, self.bufB
         units = packed.units[lo:hi]
         if self.split:
-            def pair(count):
-                return (torch.empty(max(1, count), **f16), torch.empty(max(1, count), **f16))
+            def pair(count):                  # 'tc1h': heads only, (hi, None)
+                return f16_pair(max(1, count), dev, impl)
             xs, ys = pair(n * mx_io), pair(n * mx_io)
             r1, r2 = pair(n * mx_r), pair(n * mx_r)
             self.in_split = xs
@@ -445,7 +486,7 @@ class ResNetPlan(object):
                 if 'shortcut' in unit:
                     self.ops.append(unit['shortcut'].bind(None, n, H, H, self.bufS, inp_split=xs, impl=impl))
                     if ui == 0:
-                        self.in_refs += [(self.ops[-1], 'in_hi', 0), (self.ops[-1], 'in_lo', 1)]
+                        self.in_refs += self._split_refs(self.ops[-1])
                     res, res_geom = self.bufS, (unit['depth'], Ho, Ho, 1)
                 elif s > 1 and SUBSAMPLE_RES:
                     # strided identity shortcut: a dense subsampled copy so conv3's residual is row-aligned (TMA slab loads) -- written by
@@ -459,7 +500,7 @@ class ResNetPlan(object):
                     res, res_geom = x, (unit['depth'], H, H, s)
                 self.ops.append(unit['conv1'].bind(None, n, H, H, None, inp_split=xs, out_split=r1, impl=impl))
                 if ui == 0:
-                    self.in_refs += [(self.ops[-1], 'in_hi', 0), (self.ops[-1], 'in_lo', 1)]
+                    self.in_refs += self._split_refs(self.ops[-1])
                 self.ops.append(unit['conv2'].bind(None, n, H, H, None, inp_split=r1, out_split=r2, impl=impl))
                 last = ui == len(units) - 1
                 nxt = units[ui + 1]['pre'] if not last else next_pre        # the next unit's pre-activation BN (+ReLU)
@@ -515,6 +556,10 @@ class ResNetPlan(object):
         self.out_hw, self.out_depth = H, d_in
         self.in_buf = self.bufA               # stage input when root=False
 
+    def _split_refs(self, op):
+        """in_refs entries of a conv that reads the stage input's pair (its head only in the 'tc1h' mode)."""
+        return [(op, 'in_hi', 0)] + ([] if heads_only(self.impl) else [(op, 'in_lo', 1)])
+
     def set_input(self, t, t_split=None):
         """Point the stage at an external input feature map [n, in_hw, in_hw, in_depth] (fp32 `t`, and in split mode its
         pre-activated fp16 pair `t_split`); no copy."""
@@ -535,7 +580,8 @@ class ResNetPlan(object):
             op.rebind('out', t)
         if t_split is not None:
             op.rebind('out_hi', t_split[0])
-            op.rebind('out_lo', t_split[1])
+            if t_split[1] is not None:
+                op.rebind('out_lo', t_split[1])
         op.encode_act_maps()
         self.final = t
 
@@ -548,7 +594,7 @@ class ResNetPlan(object):
         if self.root:
             if self.planes is not None:
                 if images is not None:        # None: the planes were filled by the caller (uint8 frames through hd_process_image_planes)
-                    check(lib.hd_pack_conv1_planes(fptr(images), C.c_void_p(self.planes[0].data_ptr()), C.c_void_p(self.planes[1].data_ptr()),
+                    check(lib.hd_pack_conv1_planes(fptr(images), _vp(self.planes[0]), _vp(self.planes[1]),
                                                    n, self.size, self.size, self.planes[0].shape[2], st), 'hd_pack_conv1_planes')
                 self.conv1_op.run(st)
             elif self.conv1_op is not None:
@@ -560,8 +606,7 @@ class ResNetPlan(object):
             ps = self.pool_split
             check(lib.hd_maxpool3x3s2_same(fptr(self.bufS), None if self.pool_f32_dead else fptr(self.bufA), n, self.H1, self.H1, 64,
                                            fptr(ps[0]) if ps else None, fptr(ps[1]) if ps else None,
-                                           C.c_void_p(ps[2][0].data_ptr()) if ps else None,
-                                           C.c_void_p(ps[2][1].data_ptr()) if ps else None, st), 'hd_maxpool3x3s2_same')
+                                           _vp(ps[2][0]) if ps else None, _vp(ps[2][1]) if ps else None, st), 'hd_maxpool3x3s2_same')
         for op in self.ops:
             op.run(st)
         if self.tail:
@@ -660,6 +705,7 @@ class ResNetTrainPlan(object):
     root's (trunk.TrainableResNet sets them)."""
 
     def __init__(self, packed: PackedResNet, bn: ResNetBatchNorm, n, size=224, impl='auto', keep=False):
+        require_training_impl(impl, 'ResNetTrainPlan')
         self.p, self.bn, self.n, self.size, self.keep = packed, bn, n, size, bool(keep)
         self.generation = 0                   # runs so far: a recorded graph checks that its saved maps are still the plan's
         dev = packed.device
@@ -962,12 +1008,12 @@ class FMoviePlan(object):
         self._bound_for = None
 
     def _bind_fast(self, x):
-        """impl auto / tc3h: GroupNorm + ReLU + split in one kernel (hd_groupnorm_relu_split), then the temporal conv reads its A
+        """impl auto / tc3h / tc1h: GroupNorm + ReLU + split in one kernel (hd_groupnorm_relu_split), then the temporal conv reads its A
         operand as the pre-split pair (cp.async producer) instead of running GroupNorm in the register-staged producer."""
         dev, Cc = self.p.device, self.p.C
         B, T = self.B, self.T
         if not hasattr(self, 'act'):
-            self.act = (torch.empty((B * T, Cc), dtype=torch.float16, device=dev), torch.empty((B * T, Cc), dtype=torch.float16, device=dev))
+            self.act = f16_pair((B * T, Cc), dev, self.impl)
         steps, cur = [], x
         for i, blk in enumerate(self.p.blocks):
             out = self.bufs[i % 2]
@@ -980,7 +1026,7 @@ class FMoviePlan(object):
         self._bound_for = x.data_ptr()
 
     def _bind(self, x):
-        if self.impl in ('auto', 'tc3h') and self.p.blocks and all(b[k].tc == 'f16' for b in self.p.blocks for k in ('conv1', 'conv2')) \
+        if self.impl in F16_IMPLS and self.p.blocks and all(b[k].tc == 'f16' for b in self.p.blocks for k in ('conv1', 'conv2')) \
                 and self.T * (self.p.C // GN_GROUPS) <= 1280 and FAST_HEADS:
             return self._bind_fast(x)
         steps = []
@@ -1008,8 +1054,8 @@ class FMoviePlan(object):
                 check(lib.hd_groupnorm_stats(fptr(s[1]), fptr(s[2][0]), fptr(s[2][1]), fptr(self.gain), fptr(self.offset),
                                              self.B, self.T, self.p.C, GN_GROUPS, GN_EPS, st), 'hd_groupnorm_stats')
             elif s[0] == 'gns':
-                check(lib.hd_groupnorm_relu_split(fptr(s[1]), fptr(s[2][0]), fptr(s[2][1]), C.c_void_p(self.act[0].data_ptr()),
-                                                  C.c_void_p(self.act[1].data_ptr()), self.B, self.T, self.p.C, GN_GROUPS, GN_EPS, st),
+                check(lib.hd_groupnorm_relu_split(fptr(s[1]), fptr(s[2][0]), fptr(s[2][1]), _vp(self.act[0]), _vp(self.act[1]),
+                                                  self.B, self.T, self.p.C, GN_GROUPS, GN_EPS, st),
                       'hd_groupnorm_relu_split')
             else:
                 s[1].run(st)
@@ -1070,14 +1116,13 @@ class IEFPlan(object):
         self.impl = impl
         self._bound_for = None
         heads = [packed.main] + [packed.deltas[k] for k in self.delta_keys]
-        self.fast = FAST_HEADS and impl in ('auto', 'tc3h') and all(h.fc1_phi.tc == 'f16' and h.fc2.tc == 'f16' for h in heads)
+        self.fast = FAST_HEADS and impl in F16_IMPLS and all(h.fc1_phi.tc == 'f16' and h.fc2.tc == 'f16' for h in heads)
         if self.fast:
-            f16 = dict(dtype=torch.float16, device=dev)
-            self.phi_split = (torch.empty((N, heads[0].feat), **f16), torch.empty((N, heads[0].feat), **f16))
-            self.h1_split = (torch.empty((N, 1024), **f16), torch.empty((N, 1024), **f16))
+            self.phi_split = f16_pair((N, heads[0].feat), dev, impl)
+            self.h1_split = f16_pair((N, 1024), dev, impl)
 
     def _head_ops_fast(self, head, start_view, state_view, ld):
-        """impl auto / tc3h.  phi arrives once as a pre-split pair (hd_split_f16); per stage: hd_ief_fc1_theta (K = 85 / 72, writes h1
+        """impl auto / tc3h / tc1h.  phi arrives once as a pre-split pair (hd_split_f16); per stage: hd_ief_fc1_theta (K = 85 / 72, writes h1
         pre-split) -> fc2 on the tensor cores (cp.async producer) -> hd_ief_fc3 (D = 85 / 72 + the IEF update).  The
         generic kernels ran fc1-theta on 40 SIMT blocks (50 us) and fc3 as ONE 128-row tile per 128 poses on 5 CTAs (80 us)."""
         N = self.N
@@ -1101,7 +1146,7 @@ class IEFPlan(object):
             elif kind == 'fc1t':
                 _, prev, prev_ld, head = op
                 check(lib.hd_ief_fc1_theta(fptr(self.P), fptr(prev), prev_ld, fptr(head.fc1_theta.w_kn), head.d, 1024,
-                                           C.c_void_p(self.h1_split[0].data_ptr()), C.c_void_p(self.h1_split[1].data_ptr()), None, N, st),
+                                           _vp(self.h1_split[0]), _vp(self.h1_split[1]), None, N, st),
                       'hd_ief_fc1_theta')
             else:
                 _, prev, prev_ld, out, out_ld, head = op
@@ -1136,8 +1181,7 @@ class IEFPlan(object):
         if self._bound_for != (phi.data_ptr(), theta0.data_ptr()):
             self._bind(phi, theta0)
         if self.fast:
-            check(lib.hd_split_f16(fptr(phi), C.c_void_p(self.phi_split[0].data_ptr()), C.c_void_p(self.phi_split[1].data_ptr()),
-                                   phi.numel(), st), 'hd_split_f16')
+            check(lib.hd_split_f16(fptr(phi), _vp(self.phi_split[0]), _vp(self.phi_split[1]), phi.numel(), st), 'hd_split_f16')
         self._run_ops(self.main_ops, st)
         return self.theta
 

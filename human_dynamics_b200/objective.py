@@ -38,7 +38,7 @@ from torch.autograd.function import once_differentiable
 from . import _lib
 from ._lib import lib, check, current_stream
 from .config import HMMRConfig
-from .nets import RESNET_BLOCKS
+from .nets import RESNET_BLOCKS, require_training_impl
 
 F32 = torch.float32
 
@@ -338,6 +338,7 @@ class HMMRTrainer(object):
         from .trainable import TemporalModel
         from src.tf_smpl.batch_smpl import SMPL
         self.config = config
+        require_training_impl(config.impl, 'HMMRTrainer')
         if config.do_hallucinate and not config.predict_delta:
             raise _lib.HDError('do_hallucinate needs predict_delta (the reference asserts it, src/config.py:271)')
         if not config.freeze_phi and config.precomputed_phi:

@@ -28,7 +28,7 @@ from torch.autograd.function import once_differentiable
 
 from . import _lib
 from ._lib import lib, check, fptr, current_stream, ConvDesc
-from .nets import FAST_HEADS, GN_EPS, GN_GROUPS, PackedConv, sync_packing, weight_tmap
+from .nets import FAST_HEADS, GN_EPS, GN_GROUPS, PackedConv, require_training_impl, sync_packing, weight_tmap
 
 F32 = torch.float32
 
@@ -493,9 +493,10 @@ class TemporalModel(nn.Module):
         super().__init__()
         from .config import HMMRConfig
         from .engine import load_weights
+        self.config = config or HMMRConfig()
+        require_training_impl(self.config.impl, 'TemporalModel')
         if not torch.cuda.is_available():
             raise _lib.HDError('TemporalModel needs a CUDA device: the hot path has no CPU fallback')
-        self.config = config or HMMRConfig()
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         w = load_weights(weights)
         self._source = w                                       # frozen variables (the ResNet) for tf_variables / save_checkpoint

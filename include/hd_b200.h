@@ -53,7 +53,12 @@ void hd_launch_count_reset(void);
  *   if post_relu: v = max(v,0)
  *   out[(n*Ho+oy)*Wo+ox][co] = v          (out may be NULL when out_hi/out_lo are given, see below)
  * ------------------------------------------------------------------------------------------ */
-enum { HD_IMPL_SIMT = 0, HD_IMPL_TC_3XTF32 = 1, HD_IMPL_TC_1XTF32 = 2, HD_IMPL_TC_3XF16 = 3 };
+/* impl 3 (3xFP16) is FP32-class: A_hi*B_hi + (A_lo*B_hi + A_hi*B_lo) per product.  impl 4 (1xFP16) is its half-precision
+ * inference mode: A_hi*B_hi alone, one MMA per product, on the same formats -- w_nk_hi / tmap_hi (and tmap_hi_n64) are the heads of
+ * the fp16 packs, in_hi (or the conv1 planes' plane_hi) is read without in_lo, out_hi is written without out_lo -- with the same
+ * two-level accumulation, so impl 4 computes what impl 3 computes from zero remainders.  With impl 4, w_nk_lo, tmap_lo,
+ * tmap_lo_n64, in_lo and out_lo must be NULL (HD_ERR_INVALID otherwise), and out_subsample does not need tmap_out_lo. */
+enum { HD_IMPL_SIMT = 0, HD_IMPL_TC_3XTF32 = 1, HD_IMPL_TC_1XTF32 = 2, HD_IMPL_TC_3XF16 = 3, HD_IMPL_TC_1XF16 = 4 };
 
 typedef struct {
   const float *in;  long long in_ld;          /* floats between consecutive pixels (>= Cin) */
@@ -61,8 +66,8 @@ typedef struct {
   int Ho, Wo, KH, KW, stride, pad_t, pad_l;
   const float *w_kn;                          /* [K, Cout] row-major, K=(ky,kx,ci) (TF HWIO flattened) */
   const void *w_nk_hi;                        /* [Cout_pad, K] K-major head of the split weights: fp32 holding TF32 values (impl 1,2)
-                                                 or fp16 (impl 3) */
-  const void *w_nk_lo;                        /* remainder, same layout: RN_tf32(w - hi), or RN_f16((w - hi) * 2^11) */
+                                                 or fp16 (impl 3, 4) */
+  const void *w_nk_lo;                        /* remainder, same layout: RN_tf32(w - hi), or RN_f16((w - hi) * 2^11); NULL for impl 4 */
   int Cout;  int K_pad;
   const float *pre_scale, *pre_shift;  int pre_img_stride;  int pre_relu;
   const float *post_scale, *post_shift;  int post_relu;
@@ -70,7 +75,7 @@ typedef struct {
   float *out;  long long out_ld;
   int impl;
   const void *tmap_hi, *tmap_lo;              /* HOST pointers to 128-byte CUtensorMap blobs from hd_make_weight_tmap */
-  /* Pre-split activations (impl 3 only).  When in_hi/in_lo are set the A operand is read from two fp16 arrays of the
+  /* Pre-split activations (impl 3; impl 4 with the heads alone).  When in_hi/in_lo are set the A operand is read from two fp16 arrays of the
    * same [pixels, in_ld] geometry as `in` (hi = RN_f16(a), lo = RN_f16((a - hi) * 2^11), a = the ALREADY pre-activated
    * input) with cp.async straight into the swizzled tile -- no register staging, no prologue (pre_scale must be NULL).
    * When out_hi/out_lo are set the epilogue additionally (or, with out == NULL, only) writes
@@ -124,12 +129,13 @@ int hd_make_act_tmap(const void *base, long long rows, int cols, long long ld_el
 /* ---- ResNet root / tail pieces (slim resnet_v2_50, called from src/models.py:65-74) ---- */
 /* Input of the tensor-core conv1 (HD_CONV_INPUT_PLANES): img fp32 [N,H,W,3] -> two fp16 planes [N, H+6, WP, 4] (head and
  * 2^11-scaled remainder of every sample, channel 3 = 0), the image at row/column offset 3 inside a zero border that the
- * caller clears ONCE (the kernel writes the interior only).  WP = plane row length in pixels (even, >= W + 8). */
+ * caller clears ONCE (the kernel writes the interior only).  WP = plane row length in pixels (even, >= W + 8).
+ * plane_lo may be NULL: the head plane alone (impl 4). */
 int hd_pack_conv1_planes(const float *img, void *plane_hi, void *plane_lo, int N, int H, int W, int WP, void *stream);
 /* conv1: 7x7 stride 2, explicit zero pad 3+3, + bias.  in [N,H,W,3] -> out [N,H/2,W/2,64]; w [7*7*3,64]. */
 int hd_conv1_7x7s2(const float *in, const float *w, const float *bias, float *out, int N, int H, int W, void *stream);
 /* pool1: 3x3 stride 2 max pool, TF SAME padding (pad 0 top/left, 1 bottom/right for even sizes).
- * Optional second output (out_hi/out_lo non-NULL): relu(v*scale[c] + shift[c]) as an fp16 head/remainder pair
+ * Optional second output (out_hi non-NULL): relu(v*scale[c] + shift[c]) as an fp16 head/remainder pair (out_lo NULL: the head alone)
  * (the first bottleneck unit's pre-activation, pre-split for the tensor-core kernel); `out` may then be NULL (the first unit's
  * shortcut is a conv of the pre-activation, so nobody reads the fp32 pool output). */
 int hd_maxpool3x3s2_same(const float *in, float *out, int N, int H, int W, int C, const float *scale, const float *shift,
@@ -202,8 +208,9 @@ int hd_zero_insert(const float *in, float *out, int N, int Hi, int Wi, int C, in
  * (src/util/common.py:7-14), batched.  frames uint8 [N,H,W,3]; geom int32 [N,4] (16-byte aligned) = {Hs, Ws, x0, y0}: size of the
  * cv2.resize'd frame and the top-left corner of the SxS crop in its coordinates (may lie outside: edge replication = the
  * reference's np.pad(mode='edge')); out fp32 [N,S,S,3] = crop of resize(2*(frame/255 - 0.5)) (bilinear, cv2 conventions).
- * plane_hi / plane_lo (optional, both or neither; then `out` may be NULL): the same crop written directly as the padded RGBX
- * fp16 planes [N,S+6,WP,4] the tensor-core conv1 reads (hd_pack_conv1_planes layout; border cleared once by the caller). */
+ * plane_hi / plane_lo (optional; then `out` may be NULL): the same crop written directly as the padded RGBX fp16 planes
+ * [N,S+6,WP,4] the tensor-core conv1 reads (hd_pack_conv1_planes layout; border cleared once by the caller).  plane_lo needs
+ * plane_hi; plane_hi alone writes the head plane (impl 4). */
 int hd_process_image(const unsigned char *frames, int N, int H, int W, const int *geom, float *out, int S, void *plane_hi,
                      void *plane_lo, int WP, void *stream);
 /* Host bookkeeping of process_image for one frame (no CUDA call): bbox = {cx, cy, scale} as float64 -> geom = the {Hs, Ws, x0, y0} row
@@ -265,15 +272,16 @@ int hd_groupnorm_stats(const float *x, const float *gamma, const float *beta, fl
                        int B, int T, int C, int groups, float eps, void *stream);
 
 /* GroupNorm + ReLU straight to the tensor-core conv's A operand format: y = relu(group_norm(x)) as an fp16 head / 2^11-scaled
- * remainder pair [B*T, C] (same statistics and affine as hd_groupnorm_stats + the conv prologue).  T * C/groups <= 1280. */
+ * remainder pair [B*T, C] (same statistics and affine as hd_groupnorm_stats + the conv prologue).  T * C/groups <= 1280.
+ * out_lo may be NULL: the head alone (impl 4). */
 int hd_groupnorm_relu_split(const float *x, const float *gamma, const float *beta, void *out_hi, void *out_lo, int B, int T, int C,
                             int groups, float eps, void *stream);
-/* fp32 [n] -> fp16 head / remainder pair (n % 4 == 0, 16-byte aligned). */
+/* fp32 [n] -> fp16 head / remainder pair (n % 4 == 0, 16-byte aligned); lo may be NULL: the head alone (impl 4). */
 int hd_split_f16(const float *x, void *hi, void *lo, long long n, void *stream);
 
 /* ---- IEF pieces too small / too narrow for the tensor-core tile (src/models.py:101-113,400-413) ----
  * fc1, theta part: h1 = relu(P + theta . W) with P [N,C] = phi . W1[:2048] + b1 (hoisted), theta rows of K <= 96 at stride theta_ld,
- * W [K,C]; writes h1 as an fp16 head / remainder pair (fc2's A operand) and / or fp32. */
+ * W [K,C]; writes h1 as an fp16 head / remainder pair (fc2's A operand; out_lo NULL: the head alone) and / or fp32. */
 int hd_ief_fc1_theta(const float *P, const float *theta, int theta_ld, const float *W, int K, int C, void *out_hi, void *out_lo,
                      float *out_f32, int N, void *stream);
 /* fc3 + IEF update: out[n, :D] = prev[n, :D] + h2[n] . W + bias, h2 [N,K] (K % 64 == 0), W [K,D], D <= 96; fixed summation order. */
@@ -287,7 +295,8 @@ int hd_ief_delta_init(const float *theta, float *dst, int dst_ld, int N, void *s
  * A plan packs the TF-named weights once (BatchNorm folded, K-major fp16 head / remainder split, TMA descriptors) and owns its
  * activation buffers: `*_create` allocates device memory and copies weights (synchronous, once); `*_forward` is a fixed sequence of
  * the per-layer entries above on `stream` -- no allocation, no synchronisation -- and is bit-identical to the Python host plans
- * (human_dynamics_b200/nets.py).  Precision mode: HD_IMPL_TC_3XF16 (FP32-class).
+ * (human_dynamics_b200/nets.py).  Precision mode: HD_IMPL_TC_3XF16 (FP32-class); the half-precision mode (impl 4) is only
+ * reachable through the per-layer entries above.
  * Weights are pulled through a callback: get(user, "<TF variable name>", &numel) returns a HOST pointer to the fp32 array in the
  * TensorFlow layout (conv HWIO, FC [in,out]) -- e.g. "resnet_v2_50/block1/unit_1/bottleneck_v2/conv1/weights" -- or NULL if absent
  * (then create fails with HD_ERR_INVALID and hd_net_error names the variable); the arrays only have to stay valid during `*_create`.

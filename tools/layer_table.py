@@ -1,14 +1,18 @@
-"""Per-layer table of one C3 trunk pass: time, TFLOP/s, and the layer's compulsory HBM traffic / time (GB/s)."""
-import sys, os, ctypes
+"""Per-layer table of one C3 trunk pass: time, TFLOP/s, and the layer's compulsory HBM traffic / time (GB/s).
+--impl picks the precision mode of the trunk (default 'auto'; 'tc1h' = the half-precision inference mode)."""
+import argparse, sys, os, ctypes
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from human_dynamics_b200 import synthetic, HMMRConfig, _lib
 from human_dynamics_b200.engine import HMMREngine
+ap = argparse.ArgumentParser()
+ap.add_argument('--impl', default='auto', help="HMMRConfig.impl of the engine: auto | tc3h | tc1h | tc3 | tc1 | simt")
+args = ap.parse_args()
 B, T = 32, 20
 N = B * T
 w = synthetic.make_synthetic_weights(seed=1)
 smpl = synthetic.make_synthetic_smpl(seed=2)
-eng = HMMREngine(w, smpl, HMMRConfig(batch_size=B, sequence_length=T))
+eng = HMMREngine(w, smpl, HMMRConfig(batch_size=B, sequence_length=T, impl=args.impl))
 img = torch.from_numpy(synthetic.make_images(N, seed=0)).cuda()
 phi = eng.encode_images(img)
 torch.cuda.synchronize()
