@@ -152,6 +152,7 @@ SIGNATURES = {
     'hd_bn_moving_update': (_i, [_vp, _vp, _ll, _i, C.c_double, _vp, _vp, _vp]),
     'hd_conv_wgrad_workspace_bytes': (_sz, [_ll, _i, _i, _i]),
     'hd_conv_wgrad': (_i, [_vp, _ll] + [_i] * 11 + [_vp, _vp, _vp, _ll, _i, _vp, _vp, _vp, _sz, _vp]),
+    'hd_conv_wgrad_ex': (_i, [_vp, _ll] + [_i] * 11 + [_vp, _vp, _vp, _ll, _i, _vp, _vp, _vp, _sz, _i, _vp]),
     'hd_bn_relu_backward_workspace_bytes': (_sz, [_ll, _i]),
     'hd_bn_relu_backward': (_i, [_vp, _vp, _i, _ll, _i, _vp, _vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _sz, _vp]),
     'hd_maxpool3x3s2_same_backward': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),

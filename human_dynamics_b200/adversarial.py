@@ -13,7 +13,7 @@ encoder), which are ordinary torch code:
     e_loss = compute_loss_e_fake(disc(batch_rodrigues(theta)[:, 1:]))
 
 The forward and backward run csrc/dpose.cu and hd_conv_gemm (the FC layers: 3xTF32 for fc1, whose K = 736 is not a multiple of 64, the
-fp16-split pack for fc2 (impl 'auto'); the backward's GEMMs are 3xTF32).  Results are deterministic: a pose's logits and input gradient
+fp16-split pack for fc2 (impl 'auto'); the backward's GEMMs are 3xTF32, or 1xTF32 with grad_precision='tf32').  Results are deterministic: a pose's logits and input gradient
 depend on that pose only, and the weight gradients are fixed-order sums.  No weight decay: the reference's l2_regularizer terms go into a
 collection its trainer never reads.
 """
@@ -26,7 +26,7 @@ from torch.autograd.function import once_differentiable
 
 from . import _lib
 from ._lib import lib, check, fptr, current_stream
-from .nets import PackedConv, sync_packing
+from .nets import PackedConv, grad_one_pass, sync_packing
 from .trainable import BackwardDataPack, _col_sum, _round, _tf32_gemm, _vp, _wgrad, _xt, repack_stale
 
 F32 = torch.float32
@@ -86,9 +86,9 @@ def dpose_backward(d, x, saved, g, want_dx, want_dw):
     dflat = torch.empty((N, FLAT), dtype=F32, device=dev)
     # df2 = g[:, 23] w_out^T * (f2 > 0);  df1 = (df2 . Wfc2^T) * (f1 > 0);  dflat = df1 . Wfc1^T
     check(lib.hd_fc_small_dgrad(_vp(g, J * 4), J + 1, fptr(P[10]), HID, 1, fptr(f2), fptr(df2), N, st), 'hd_fc_small_dgrad')
-    _tf32_gemm(df2, N, HID, HID, d.fc2_bwd, df1, HID, stream=st)
+    _tf32_gemm(df2, N, HID, HID, d.fc2_bwd, df1, HID, stream=st, one_pass=d.one_pass)
     check(lib.hd_relu_backward(fptr(f1), fptr(df1), fptr(df1), N * HID, st), 'hd_relu_backward')
-    _tf32_gemm(df1, N, HID, HID, d.fc1_bwd, dflat, FLAT, stream=st)
+    _tf32_gemm(df1, N, HID, HID, d.fc1_bwd, dflat, FLAT, stream=st, one_pass=d.one_pass)
     dx = torch.empty((N, J, 9), dtype=F32, device=dev) if want_dx else None
     ws_bytes = int(lib.hd_dpose_workspace_bytes(N)) if want_dw else 0
     ws = torch.empty(ws_bytes // 4, dtype=F32, device=dev) if want_dw else None
@@ -104,7 +104,7 @@ def dpose_backward(d, x, saved, g, want_dx, want_dw):
     kp = _round(N, 32)
     for i, inp, gin, cin in ((6, h2, df1, FLAT), (8, f1, df2, HID)):
         W, bias = torch.empty((cin, HID), dtype=F32, device=dev), torch.empty(HID, dtype=F32, device=dev)
-        _wgrad(_xt([(inp, N, cin)], cin, kp, st), cin, kp, [(gin, N, HID)], HID, W, st)
+        _wgrad(_xt([(inp, N, cin)], cin, kp, st), cin, kp, [(gin, N, HID)], HID, W, st, d.one_pass)
         _col_sum(gin, N, HID, HID, bias, st)
         grads[i], grads[i + 1] = W, bias
     return dx, grads
@@ -141,11 +141,13 @@ class PoseDiscriminator(nn.Module):
 
     Parameters are addressable by PARAM_NAMES (`disc.param('D_pose/D_conv1/weights')`); the 23 heads pose_out_j<j> are stacked into
     'D_pose/pose_out_j/weights' [23, 32] and '.../biases' [23].  A parameter changed in place (optimizer.step()) is repacked before the
-    next forward / backward.  Under torch.no_grad(), or when nothing requires grad, the forward builds no graph."""
+    next forward / backward.  Under torch.no_grad(), or when nothing requires grad, the forward builds no graph.  grad_precision: 'fp32'
+    (3xTF32 backward GEMMs) or 'tf32' (1xTF32, nets.GRAD_PRECISIONS); the forward is the same in both."""
 
-    def __init__(self, weights=None, seed=0, device=None):
+    def __init__(self, weights=None, seed=0, device=None, grad_precision='fp32'):
         super().__init__()
         from .synthetic import make_dpose_weights
+        self.one_pass = grad_one_pass(grad_precision, 'PoseDiscriminator')
         if not torch.cuda.is_available():
             raise _lib.HDError('PoseDiscriminator needs a CUDA device: the hot path has no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)

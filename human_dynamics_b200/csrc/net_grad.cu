@@ -24,7 +24,7 @@ __device__ __forceinline__ void store_split(float v, int mode, void *hi, void *l
   } else if (mode == 1) {
     const float h = rn_tf32(v);
     reinterpret_cast<float *>(hi)[o] = h;
-    reinterpret_cast<float *>(lo)[o] = rn_tf32(__fsub_rn(v, h));
+    if (lo) reinterpret_cast<float *>(lo)[o] = rn_tf32(__fsub_rn(v, h));         // lo NULL: the head alone (1xTF32)
   } else {
     reinterpret_cast<float *>(hi)[o] = v;
   }
@@ -257,9 +257,9 @@ extern "C" {
 
 int hd_transpose_split(const float *x, long long rows, int cols, long long ld, int mode, void *hi, void *lo, long long out_ld, int out_rows,
                        long long out_cols, void *stream) {
-  HD_REQUIRE(x && hi && rows > 0 && cols > 0 && ld >= cols && (mode == 0 || mode == 1 || mode == 2) && ((mode == 0) == (lo == nullptr)) &&
+  HD_REQUIRE(x && hi && rows > 0 && cols > 0 && ld >= cols && (mode == 0 || mode == 1 || mode == 2) && (mode == 0 ? lo == nullptr : (mode == 1 || lo != nullptr)) &&
                  out_rows >= cols && out_cols >= rows && out_ld >= out_cols,
-             "hd_transpose_split: bad arguments (mode 0 = fp32 with lo NULL, 1 = tf32 pair, 2 = fp16 pair; out_rows >= cols, out_cols >= rows)");
+             "hd_transpose_split: bad arguments (mode 0 = fp32 with lo NULL, 1 = tf32 pair or head, 2 = fp16 pair; out_rows >= cols, out_cols >= rows)");
   dim3 grid((unsigned)hd::ceil_div(out_cols, 32), (unsigned)hd::ceil_div(out_rows, 32));
   HD_REQUIRE(grid.y <= 65535u, "hd_transpose_split: out_rows too large");
   transpose_split_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, rows, cols, ld, mode, hi, lo, out_ld, out_rows, out_cols);

@@ -1,7 +1,7 @@
 // Backward of the training-mode ResNet trunk (slim resnet_v2_50 with is_training=True): the convolutions' weight gradients, the
 // training-mode batch norm + ReLU backward, pool1's backward and the zero-insertion that turns the data gradient of a stride-2 3x3 conv
-// into a stride-1 conv for hd_conv_gemm.  The other data gradients are hd_conv_gemm itself (3xTF32, in = dY) over
-// hd_pack_weight(HD_PACK_BACKWARD_DATA).
+// into a stride-1 conv for hd_conv_gemm.  The other data gradients are hd_conv_gemm itself (3xTF32, or 1xTF32 in the TF32 gradient
+// mode; in = dY) over hd_pack_weight(HD_PACK_BACKWARD_DATA).
 //
 // Nothing here uses atomics: every sum runs over a partition that depends only on the shapes, and partials are merged in a fixed order,
 // so results are bit-identical from run to run and do not depend on the GPU's SM count.
@@ -15,21 +15,30 @@ namespace {
 // ------------------------------------------------------------------------------------------------------------------------------------
 // hd_conv_wgrad: dW[(ky,kx,ci), co] = sum_p a[p, (ky,kx,ci)] * dY[p, co] as an implicit GEMM, M = KH*KW*Cin, N = Cout, reduced over the
 // pixels p in chunks of kChunk.  A CTA owns a 64 x 64 tile of dW and one chunk, and is split into two warpgroups:
-//   producer  gathers 32 pixels of A (from the input, the prologue applied) and of dY per stage, splits every value into a TF32 head and
-//             remainder in registers and writes the four 64-row x 128-byte tiles (A hi / lo, dY hi / lo, both K-major: the pixels are
-//             the GEMM's K) in the 128-byte swizzle wgmma reads; kStages stages in flight on full / empty mbarriers.  The CTAs of the
-//             first M tile also sum the dY values they load per column in fp64: the bias gradient, without a padding tile.
-//   consumer  per stage, 4 K steps of wgmma m64n64k8 in the 3xTF32 split (a_lo b_hi + a_hi b_lo + a_hi b_hi: gradients have an
-//             arbitrary scale, so no fp16 operand).  The tensor cores' own fp32 accumulation does not round to nearest, so each stage
-//             is accumulated from zero and added to the running sums with ordinary round-to-nearest adds.
+//   producer  gathers 32 pixels of A (from the input, the prologue applied) and of dY per stage, rounds every value to a TF32 head (and,
+//             with SPLIT, its remainder) in registers and writes the 64-row x 128-byte tiles (SPLIT: A hi / lo, dY hi / lo; else A hi,
+//             dY hi; K-major: the pixels are the GEMM's K) in the 128-byte swizzle wgmma reads; WgradCfg<SPLIT>::kStages stages in flight on
+//             full / empty mbarriers.  The CTAs of the first M tile also sum the loaded fp32 dY values per column in fp64: the bias gradient,
+//             without a padding tile, and the same in both modes.
+//   consumer  per stage, 4 K steps of wgmma m64n64k8: SPLIT (3xTF32, impl 1) a_lo b_hi + a_hi b_lo + a_hi b_hi (gradients have an
+//             arbitrary scale, so no fp16 operand); !SPLIT (1xTF32, impl 2) a_hi b_hi alone.  The tensor cores' own fp32 accumulation
+//             does not round to nearest, so each stage is accumulated from zero and added to the running sums with ordinary
+//             round-to-nearest adds.
 // Tile partials go to the workspace [chunks, K + bias, Cout] and wgrad_merge_kernel adds them in chunk order in fp64.
 // ------------------------------------------------------------------------------------------------------------------------------------
 constexpr int kChunk = 2048;           // pixels per partial sum: fixed, so the rounding depends on the shapes alone
 constexpr int kBM = 64, kBN = 64, kBP = 32;
-constexpr int kStages = 3;
 constexpr int kTileBytes = 64 * 128;                  // 64 rows x one 128-byte swizzle row (32 tf32 pixels)
-constexpr int kStageBytes = 4 * kTileBytes;           // A hi, A lo, dY hi, dY lo
-constexpr int kWgradSmem = kStages * kStageBytes + 1024;
+template <bool SPLIT>
+struct WgradCfg {
+  static constexpr int kTiles = SPLIT ? 4 : 2;        // A hi (, A lo), dY hi (, dY lo)
+  static constexpr int kBOffset = (kTiles / 2) * kTileBytes;
+  static constexpr int kStageBytes = kTiles * kTileBytes;
+  // 1xTF32: a stage is half as large.  Measured on an H100 80GB HBM3 (700 W), one n = 160 trunk backward's weight gradients take
+  // 65.5 / 65.2 / 65.5 ms with 3 / 4 / 6 stages (3xTF32: 68.6 ms): the gather, not the ring, bounds the kernel; 4 is the fastest.
+  static constexpr int kStages = SPLIT ? 3 : 4;
+  static constexpr int kSmem = kStages * kStageBytes + 1024;
+};
 constexpr int kWgradThreads = 256;
 
 struct WgradArgs {
@@ -45,20 +54,25 @@ struct WgradArgs {
   float *part;                         // [chunks, M, Cout]
 };
 
-__device__ __forceinline__ void split4(const float *v, uint4 &hi, uint4 &lo) {
+// Four K-consecutive values of one tile row -> their TF32 heads at `hi` (and, with SPLIT, the remainders one tile further on).
+template <bool SPLIT>
+__device__ __forceinline__ void store4(uint8_t *hi, const float *v) {
   uint32_t h[4], l[4];
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
     const float hf = hd::ptx::rn_tf32(v[e]);
     h[e] = __float_as_uint(hf);
-    l[e] = __float_as_uint(hd::ptx::rn_tf32(v[e] - hf));
+    if (SPLIT) l[e] = __float_as_uint(hd::ptx::rn_tf32(v[e] - hf));
   }
-  hi = make_uint4(h[0], h[1], h[2], h[3]);
-  lo = make_uint4(l[0], l[1], l[2], l[3]);
+  *reinterpret_cast<uint4 *>(hi) = make_uint4(h[0], h[1], h[2], h[3]);
+  if (SPLIT) *reinterpret_cast<uint4 *>(hi + kTileBytes) = make_uint4(l[0], l[1], l[2], l[3]);
 }
 
+template <bool SPLIT>
 __global__ void __launch_bounds__(kWgradThreads, 2) wgrad_kernel(const WgradArgs a) {
   namespace P = hd::ptx;
+  using Cfg = WgradCfg<SPLIT>;
+  constexpr int kStages = Cfg::kStages, kStageBytes = Cfg::kStageBytes;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kStages], empty_bar[kStages];
   __shared__ int pix_n[kBP], pix_y[kBP], pix_x[kBP];       // per staged pixel: image, top-left input row / column (n = -1: past the chunk)
@@ -163,13 +177,8 @@ __global__ void __launch_bounds__(kWgradThreads, 2) wgrad_kernel(const WgradArgs
         for (int c4 = 0; c4 < 4; ++c4) {
           const int rr = 4 * vrg + c4;
           const uint32_t off = (uint32_t)rr * 128u + ((uint32_t)(vj ^ (rr & 7)) << 4);
-          uint4 h, l;
-          split4(av[c4], h, l);
-          *reinterpret_cast<uint4 *>(st + off) = h;
-          *reinterpret_cast<uint4 *>(st + kTileBytes + off) = l;
-          split4(bv[c4], h, l);
-          *reinterpret_cast<uint4 *>(st + 2 * kTileBytes + off) = h;
-          *reinterpret_cast<uint4 *>(st + 3 * kTileBytes + off) = l;
+          store4<SPLIT>(st + off, av[c4]);
+          store4<SPLIT>(st + Cfg::kBOffset + off, bv[c4]);
           if (bias) vbsum[c4] += ((double)bv[c4][0] + (double)bv[c4][1]) + ((double)bv[c4][2] + (double)bv[c4][3]);
         }
       } else {
@@ -200,13 +209,8 @@ __global__ void __launch_bounds__(kWgradThreads, 2) wgrad_kernel(const WgradArgs
           for (int e = 0; e < 4; ++e) bsum += (double)bv[e];
         }
         const uint32_t off = (uint32_t)r * 128u + ((uint32_t)(j ^ (r & 7)) << 4);
-        uint4 h, l;
-        split4(av, h, l);
-        *reinterpret_cast<uint4 *>(st + off) = h;
-        *reinterpret_cast<uint4 *>(st + kTileBytes + off) = l;
-        split4(bv, h, l);
-        *reinterpret_cast<uint4 *>(st + 2 * kTileBytes + off) = h;
-        *reinterpret_cast<uint4 *>(st + 3 * kTileBytes + off) = l;
+        store4<SPLIT>(st + off, av);
+        store4<SPLIT>(st + Cfg::kBOffset + off, bv);
       }
       }
       P::fence_proxy_async();                                // generic-proxy stores -> visible to wgmma (async proxy)
@@ -240,16 +244,18 @@ __global__ void __launch_bounds__(kWgradThreads, 2) wgrad_kernel(const WgradArgs
       const int s = q % kStages;
       P::mbar_wait(P::smem_u32(&full_bar[s]), (uint32_t)(q / kStages) & 1u);
       const uint32_t sa = base + s * kStageBytes;
-      const uint64_t da_hi = P::make_smem_desc(sa), da_lo = P::make_smem_desc(sa + kTileBytes);
-      const uint64_t db_hi = P::make_smem_desc(sa + 2 * kTileBytes), db_lo = P::make_smem_desc(sa + 3 * kTileBytes);
+      const uint64_t da_hi = P::make_smem_desc(sa), db_hi = P::make_smem_desc(sa + Cfg::kBOffset);
       P::fence_regs(tmp);
       P::wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {                       // K = 8 tf32 = 32 bytes per wgmma: advance inside the swizzle row
         const uint64_t adv = (uint64_t)((kk * 32) >> 4);
-        P::wgmma_m64n64k8_tf32(tmp, da_lo + adv, db_hi + adv, kk != 0);     // small products first, then the head product
-        P::wgmma_m64n64k8_tf32(tmp, da_hi + adv, db_lo + adv, 1u);
-        P::wgmma_m64n64k8_tf32(tmp, da_hi + adv, db_hi + adv, 1u);
+        if constexpr (SPLIT) {
+          const uint64_t da_lo = P::make_smem_desc(sa + kTileBytes), db_lo = P::make_smem_desc(sa + Cfg::kBOffset + kTileBytes);
+          P::wgmma_m64n64k8_tf32(tmp, da_lo + adv, db_hi + adv, kk != 0);     // small products first, then the head product
+          P::wgmma_m64n64k8_tf32(tmp, da_hi + adv, db_lo + adv, 1u);
+        }
+        P::wgmma_m64n64k8_tf32(tmp, da_hi + adv, db_hi + adv, SPLIT || kk != 0);
       }
       P::wgmma_commit();
       P::wgmma_wait<0>();
@@ -514,9 +520,29 @@ extern "C" size_t hd_conv_wgrad_workspace_bytes(long long pixels, int K, int Cou
   return (size_t)chunks * (size_t)(K + (bias ? 1 : 0)) * (size_t)Cout * sizeof(float);
 }
 
-extern "C" int hd_conv_wgrad(const float *x, long long x_ld, int n_img, int H, int W, int Cin, int Ho, int Wo, int KH, int KW, int stride,
-                             int pad_t, int pad_l, const float *pre_scale, const float *pre_shift, const float *dy, long long dy_ld, int Cout,
-                             float *dw, float *db, void *workspace, size_t workspace_bytes, void *stream) {
+namespace {
+
+template <bool SPLIT>
+int launch_wgrad(const WgradArgs &a, dim3 grid, cudaStream_t st) {
+  static bool smem_set = false;               // (benign race: every caller sets the same value)
+  if (!smem_set) {
+    const cudaError_t e = cudaFuncSetAttribute(wgrad_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgradCfg<SPLIT>::kSmem);
+    if (e != cudaSuccess) {
+      hd::set_last_error("hd_conv_wgrad: cudaFuncSetAttribute", e);
+      return HD_ERR_CUDA;
+    }
+    smem_set = true;
+  }
+  wgrad_kernel<SPLIT><<<grid, kWgradThreads, WgradCfg<SPLIT>::kSmem, st>>>(a);
+  return hd::check_launch("wgrad_kernel");
+}
+
+}  // namespace
+
+extern "C" int hd_conv_wgrad_ex(const float *x, long long x_ld, int n_img, int H, int W, int Cin, int Ho, int Wo, int KH, int KW, int stride,
+                                int pad_t, int pad_l, const float *pre_scale, const float *pre_shift, const float *dy, long long dy_ld,
+                                int Cout, float *dw, float *db, void *workspace, size_t workspace_bytes, int impl, void *stream) {
+  HD_REQUIRE(impl == HD_IMPL_TC_3XTF32 || impl == HD_IMPL_TC_1XTF32, "hd_conv_wgrad_ex: impl must be HD_IMPL_TC_3XTF32 or HD_IMPL_TC_1XTF32");
   HD_REQUIRE(x && dy && dw && workspace, "hd_conv_wgrad: null pointer");
   HD_REQUIRE(n_img > 0 && H > 0 && W > 0 && Cin > 0 && Ho > 0 && Wo > 0 && KH > 0 && KW > 0 && stride > 0 && Cout > 0 && pad_t >= 0 &&
                  pad_l >= 0 && x_ld >= Cin && dy_ld >= Cout,
@@ -536,20 +562,18 @@ extern "C" int hd_conv_wgrad(const float *x, long long x_ld, int n_img, int H, i
   a.part = reinterpret_cast<float *>(workspace);
   const int chunks = (int)((P + kChunk - 1) / kChunk);
   cudaStream_t st = (cudaStream_t)stream;
-  static bool smem_set = false;               // (benign race: every caller sets the same value)
-  if (!smem_set) {
-    const cudaError_t e = cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgradSmem);
-    if (e != cudaSuccess) {
-      hd::set_last_error("hd_conv_wgrad: cudaFuncSetAttribute", e);
-      return HD_ERR_CUDA;
-    }
-    smem_set = true;
-  }
-  wgrad_kernel<<<dim3(chunks, hd::ceil_div(K, kBM), hd::ceil_div(Cout, kBN)), kWgradThreads, kWgradSmem, st>>>(a);
-  int rc = hd::check_launch("wgrad_kernel");
+  const dim3 grid(chunks, hd::ceil_div(K, kBM), hd::ceil_div(Cout, kBN));
+  int rc = impl == HD_IMPL_TC_3XTF32 ? launch_wgrad<true>(a, grid, st) : launch_wgrad<false>(a, grid, st);
   if (rc) return rc;
   wgrad_merge_kernel<<<hd::ceil_div((long long)a.M * Cout, 256), 256, 0, st>>>(a.part, chunks, K, a.M, Cout, dw, db);
   return hd::check_launch("wgrad_merge_kernel");
+}
+
+extern "C" int hd_conv_wgrad(const float *x, long long x_ld, int n_img, int H, int W, int Cin, int Ho, int Wo, int KH, int KW, int stride,
+                             int pad_t, int pad_l, const float *pre_scale, const float *pre_shift, const float *dy, long long dy_ld, int Cout,
+                             float *dw, float *db, void *workspace, size_t workspace_bytes, void *stream) {
+  return hd_conv_wgrad_ex(x, x_ld, n_img, H, W, Cin, Ho, Wo, KH, KW, stride, pad_t, pad_l, pre_scale, pre_shift, dy, dy_ld, Cout, dw, db,
+                          workspace, workspace_bytes, HD_IMPL_TC_3XTF32, stream);
 }
 
 extern "C" size_t hd_bn_relu_backward_workspace_bytes(long long rows, int C) {

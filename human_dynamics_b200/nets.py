@@ -55,6 +55,19 @@ def require_training_impl(impl, who):
         raise _lib.HDError("%s: impl 'tc1h' is an inference-only half-precision mode; training runs FP32-class ('auto' / 'tc3h')" % who)
 
 
+# Precision of the training backward passes' tensor-core GEMMs (weight and data gradients; the forward passes never change):
+#   'fp32'  3xTF32 (HD_IMPL_TC_3XTF32), FP32-class
+#   'tf32'  1xTF32 (HD_IMPL_TC_1XTF32): one TF32 MMA per product on round-to-nearest heads, no remainder operand (DESIGN.md section 2)
+GRAD_PRECISIONS = ('fp32', 'tf32')
+
+
+def grad_one_pass(grad_precision, who):
+    """True for 'tf32' (single-pass TF32 gradients), False for 'fp32'; any other value raises HDError."""
+    if not isinstance(grad_precision, str) or grad_precision not in GRAD_PRECISIONS:
+        raise _lib.HDError("%s: grad_precision must be 'fp32' or 'tf32', got %r" % (who, grad_precision))
+    return grad_precision == 'tf32'
+
+
 def _dev(a, device, dtype=np.float32):
     if isinstance(a, torch.Tensor):           # already on the device (TemporalModel's parameters): used in place
         return a
@@ -702,10 +715,13 @@ class ResNetTrainPlan(object):
     conv1 output, each unit's input and its raw conv1 / conv2 outputs -- instead of ping-ponging (about 32 MB per frame at 224 x 224);
     the kernels, descriptors and arithmetic are the same, so the phis are bit-identical to keep=False.  `backward(dphi, images)` then
     walks the units in reverse (csrc/resnet_grad.cu + hd_conv_gemm 3xTF32); it needs a `bwd` data-gradient pack on every conv but the
-    root's (trunk.TrainableResNet sets them)."""
+    root's (trunk.TrainableResNet sets them).  grad_precision='tf32' runs the backward's weight and data gradients in 1xTF32 instead
+    (GRAD_PRECISIONS); the forward is the same either way."""
 
-    def __init__(self, packed: PackedResNet, bn: ResNetBatchNorm, n, size=224, impl='auto', keep=False):
+    def __init__(self, packed: PackedResNet, bn: ResNetBatchNorm, n, size=224, impl='auto', keep=False, grad_precision='fp32'):
         require_training_impl(impl, 'ResNetTrainPlan')
+        self.one_pass = grad_one_pass(grad_precision, 'ResNetTrainPlan')
+        self.grad_precision = grad_precision
         self.p, self.bn, self.n, self.size, self.keep = packed, bn, n, size, bool(keep)
         self.generation = 0                   # runs so far: a recorded graph checks that its saved maps are still the plan's
         dev = packed.device
@@ -846,7 +862,7 @@ class ResNetTrainPlan(object):
         return out
 
     def _backward_state(self):
-        """Scratch maps, workspaces and the data-gradient descriptors of `backward` (3xTF32 hd_conv_gemm over each conv's `bwd` pack),
+        """Scratch maps, workspaces and the data-gradient descriptors of `backward` (hd_conv_gemm over each conv's `bwd` pack),
         made on the first call; every pointer is plan-owned, so the descriptors never change."""
         if self._bwd is not None:
             return self._bwd
@@ -874,13 +890,14 @@ class ResNetTrainPlan(object):
                                        (H * H, d_in, depth, 1)):
                 ws_w = max(ws_w, lib.hd_conv_wgrad_workspace_bytes(n * pix, K, Cout, bias))
             u = {'gy': gy, 'gx': gx, 'H': H, 'Ho': Ho}
-            u['conv3'] = _dgrad_op(unit['conv3'], gy, n, Ho, Ho, 1, D1)
-            u['conv2'] = _dgrad_op(unit['conv2'], D2 if s == 1 else Z, n, H, H, 3, D1)
+            op = self.one_pass
+            u['conv3'] = _dgrad_op(unit['conv3'], gy, n, Ho, Ho, 1, D1, one_pass=op)
+            u['conv2'] = _dgrad_op(unit['conv2'], D2 if s == 1 else Z, n, H, H, 3, D1, one_pass=op)
             if 'shortcut' in unit:
-                u['shortcut'] = _dgrad_op(unit['shortcut'], gy, n, H, H, 1, P)
-                u['conv1'] = _dgrad_op(unit['conv1'], D2, n, H, H, 1, P, res=P)
+                u['shortcut'] = _dgrad_op(unit['shortcut'], gy, n, H, H, 1, P, one_pass=op)
+                u['conv1'] = _dgrad_op(unit['conv1'], D2, n, H, H, 1, P, res=P, one_pass=op)
             else:
-                u['conv1'] = _dgrad_op(unit['conv1'], D2, n, H, H, 1, P)
+                u['conv1'] = _dgrad_op(unit['conv1'], D2, n, H, H, 1, P, one_pass=op)
             ops.append(u)
             H = Ho
         self._bwd = dict(G=G, D1=D1, D2=D2, Z=Z, P=P, units=ops, ws_w=torch.empty(max(16, int(ws_w)), dtype=torch.uint8, device=p.device),
@@ -894,13 +911,18 @@ class ResNetTrainPlan(object):
                                       add_geom[2], fptr(out), fptr(bn.view(dgamma, i)), fptr(bn.view(dbeta, i)),
                                       C.c_void_p(ws.data_ptr()), ws.numel(), stream), 'hd_bn_relu_backward')
 
-    def _wgrad(self, x, geom, pre, dy, Cout, dw, db, stream):
-        """hd_conv_wgrad; geom = (n, H, W, Cin, Ho, Wo, KH, KW, stride, pad_t, pad_l); pre = a stats op (relu(bn(x))) or None."""
+    def _wgrad(self, x, geom, pre, dy, Cout, dw, db, stream, one_pass=False):
+        """hd_conv_wgrad (one_pass: hd_conv_wgrad_ex in 1xTF32); geom = (n, H, W, Cin, Ho, Wo, KH, KW, stride, pad_t, pad_l); pre = a
+        stats op (relu(bn(x))) or None."""
         n, H, W, Cin, Ho, Wo, KH, KW, s, pt, pl = geom
         ws = self._bwd['ws_w']
-        check(lib.hd_conv_wgrad(fptr(x), Cin, n, H, W, Cin, Ho, Wo, KH, KW, s, pt, pl, fptr(pre.scale) if pre is not None else None,
-                                fptr(pre.shift) if pre is not None else None, fptr(dy), Cout, Cout, fptr(dw),
-                                fptr(db) if db is not None else None, C.c_void_p(ws.data_ptr()), ws.numel(), stream), 'hd_conv_wgrad')
+        args = (fptr(x), Cin, n, H, W, Cin, Ho, Wo, KH, KW, s, pt, pl, fptr(pre.scale) if pre is not None else None,
+                fptr(pre.shift) if pre is not None else None, fptr(dy), Cout, Cout, fptr(dw), fptr(db) if db is not None else None,
+                C.c_void_p(ws.data_ptr()), ws.numel())
+        if one_pass:
+            check(lib.hd_conv_wgrad_ex(*args, _lib.HD_IMPL_TC_1XTF32, stream), 'hd_conv_wgrad_ex')
+        else:
+            check(lib.hd_conv_wgrad(*args, stream), 'hd_conv_wgrad')
 
     def backward(self, dphi, images, stream=None):
         """Gradients of sum(phis * dphi) after the last `run` (keep=True), images (n,size,size,3) being that run's input: returns
@@ -925,21 +947,21 @@ class ResNetTrainPlan(object):
             gy, gx = u['gy'], u['gx']
             st0, st1, st2 = self.stats[3 * ui], self.stats[3 * ui + 1], self.stats[3 * ui + 2]
             dW3, db3 = torch.empty((1, 1, base, depth), **f32), torch.empty(depth, **f32)
-            self._wgrad(self.r2s[ui], (n, Ho, Ho, base, Ho, Ho, 1, 1, 1, 0, 0), st2, gy, depth, dW3, db3, st)
+            self._wgrad(self.r2s[ui], (n, Ho, Ho, base, Ho, Ho, 1, 1, 1, 0, 0), st2, gy, depth, dW3, db3, st, self.one_pass)
             u['conv3'].run(st)                                                          # d relu(bn(conv2 out)) -> D1
             self._bn_backward(3 * ui + 2, D1, D2, dgamma, dbeta, stream=st)             # d conv2 out -> D2
             dW2 = torch.empty((3, 3, base, base), **f32)
-            self._wgrad(self.r1s[ui], (n, H, H, base, Ho, Ho, 3, 3, s, 1, 1), st1, D2, base, dW2, None, st)
+            self._wgrad(self.r1s[ui], (n, H, H, base, Ho, Ho, 3, 3, s, 1, 1), st1, D2, base, dW2, None, st, self.one_pass)
             if s > 1:
                 check(lib.hd_zero_insert(fptr(D2), fptr(Z), n, Ho, Ho, base, s, H, H, st), 'hd_zero_insert')
             u['conv2'].run(st)                                                          # d relu(bn(conv1 out)) -> D1
             self._bn_backward(3 * ui + 1, D1, D2, dgamma, dbeta, stream=st)             # d conv1 out -> D2
             dW1 = torch.empty((1, 1, d_in, base), **f32)
-            self._wgrad(self.xs[ui], (n, H, H, d_in, H, H, 1, 1, 1, 0, 0), st0, D2, base, dW1, None, st)
+            self._wgrad(self.xs[ui], (n, H, H, d_in, H, H, 1, 1, 1, 0, 0), st0, D2, base, dW1, None, st, self.one_pass)
             addend, geom = None, (0, 0, 0)
             if 'shortcut' in unit:
                 dWs, dbs = torch.empty((1, 1, d_in, depth), **f32), torch.empty(depth, **f32)
-                self._wgrad(self.xs[ui], (n, H, H, d_in, H, H, 1, 1, 1, 0, 0), st0, gy, depth, dWs, dbs, st)
+                self._wgrad(self.xs[ui], (n, H, H, d_in, H, H, 1, 1, 1, 0, 0), st0, gy, depth, dWs, dbs, st, self.one_pass)
                 u['shortcut'].run(st)                                                   # d preact, shortcut path -> P
                 grads[q + '/shortcut/weights'], grads[q + '/shortcut/biases'] = dWs, dbs
             else:
@@ -952,27 +974,32 @@ class ResNetTrainPlan(object):
         check(lib.hd_maxpool3x3s2_same_backward(fptr(self.root_buf), fptr(G[U % 2]), fptr(P), n, self.H1, self.H1, 64, st),
               'hd_maxpool3x3s2_same_backward')
         dW, db = torch.empty((7, 7, 3, 64), **f32), torch.empty(64, **f32)
-        self._wgrad(images, (n, self.size, self.size, 3, self.H1, self.H1, 7, 7, 2, 3, 3), None, P, 64, dW, db, st)
+        self._wgrad(images, (n, self.size, self.size, 3, self.H1, self.H1, 7, 7, 2, 3, 3), None, P, 64, dW, db, st, self.one_pass)
         grads['resnet_v2_50/conv1/weights'], grads['resnet_v2_50/conv1/biases'] = dW, db
         return grads
 
 
-def _dgrad_op(conv, inp, n, H, W, KH, out, res=None):
+def _dgrad_op(conv, inp, n, H, W, KH, out, res=None, one_pass=False):
     """The data gradient of a stride-1 KH x KH SAME conv (or, over the zero-inserted gradient, of a strided conv2d_same 3x3) as an
-    hd_conv_gemm op in its 3xTF32 mode: out[n, H, W, Cin] (+ res) = conv(inp [n, H, W, Cout], tap-flipped W^T = conv.bwd)."""
+    hd_conv_gemm op in its 3xTF32 mode (one_pass: 1xTF32 on the pack's head alone): out[n, H, W, Cin] (+ res) = conv(inp [n, H, W, Cout],
+    tap-flipped W^T = conv.bwd)."""
     bwd = conv.bwd
     d = ConvDesc()
     d.in_, d.in_ld = inp.data_ptr(), conv.Cout
     d.n_img, d.H, d.W, d.Cin = n, H, W, conv.Cout
     d.Ho, d.Wo, d.KH, d.KW, d.stride, d.pad_t, d.pad_l = H, W, KH, KH, 1, KH // 2, KH // 2
     d.w_kn = bwd.w_nk_hi.data_ptr()
-    d.w_nk_hi, d.w_nk_lo = bwd.w_nk_hi.data_ptr(), bwd.w_nk_lo.data_ptr()
+    d.w_nk_hi = bwd.w_nk_hi.data_ptr()
     d.Cout, d.K_pad = conv.Cin, KH * KH * conv.Cout
     if res is not None:
         d.res, d.res_ld, d.res_H, d.res_W, d.res_stride = res.data_ptr(), conv.Cin, H, W, 1
     d.out, d.out_ld = out.data_ptr(), conv.Cin
-    d.impl = _lib.HD_IMPL_TC_3XTF32
-    d.tmap_hi, d.tmap_lo = C.cast(bwd.tmap_hi, C.c_void_p), C.cast(bwd.tmap_lo, C.c_void_p)
+    d.tmap_hi = C.cast(bwd.tmap_hi, C.c_void_p)
+    if one_pass:
+        d.impl = _lib.HD_IMPL_TC_1XTF32
+    else:
+        d.impl = _lib.HD_IMPL_TC_3XTF32
+        d.w_nk_lo, d.tmap_lo = bwd.w_nk_lo.data_ptr(), C.cast(bwd.tmap_lo, C.c_void_p)
     return ConvOp(d, (conv, bwd, inp, out, res), (H, W))
 
 

@@ -38,7 +38,7 @@ from torch.autograd.function import once_differentiable
 from . import _lib
 from ._lib import lib, check, current_stream
 from .config import HMMRConfig
-from .nets import RESNET_BLOCKS, require_training_impl
+from .nets import RESNET_BLOCKS, grad_one_pass, require_training_impl
 
 F32 = torch.float32
 
@@ -63,6 +63,13 @@ class TrainConfig(HMMRConfig):
     do_hallucinate_preds: bool = False
     precomputed_phi: bool = True
     freeze_phi: bool = True
+    # Precision of every backward GEMM (the trunk's, the temporal model's and D_pose's weight and data gradients): 'fp32' (3xTF32,
+    # FP32-class) or 'tf32' (one TF32 MMA per product on round-to-nearest heads).  The forward passes, losses and optimizers are the
+    # same in both (DESIGN.md section 2).
+    grad_precision: str = 'fp32'
+
+    def __post_init__(self):
+        grad_one_pass(self.grad_precision, 'TrainConfig')
 
 
 def loss_weights(config):
@@ -339,17 +346,19 @@ class HMMRTrainer(object):
         from src.tf_smpl.batch_smpl import SMPL
         self.config = config
         require_training_impl(config.impl, 'HMMRTrainer')
+        grad_one_pass(config.grad_precision, 'HMMRTrainer')
         if config.do_hallucinate and not config.predict_delta:
             raise _lib.HDError('do_hallucinate needs predict_delta (the reference asserts it, src/config.py:271)')
         if not config.freeze_phi and config.precomputed_phi:
             raise _lib.HDError('freeze_phi=False trains the ResNet, which needs image input: set precomputed_phi=False (precomputed '
                                'phis have no trunk to train)')
         self.model = TemporalModel(weights, config, device=device)
+        gp = config.grad_precision
         self.trunk = None if config.precomputed_phi else _TrainTrunk(self.model._source, self.model.device,
-                                                                     trainable=not config.freeze_phi)
+                                                                     trainable=not config.freeze_phi, grad_precision=gp)
         self._pending = None                  # the trunk plan of the last forward: step applies its update ops
-        self.disc = PoseDiscriminator(disc_weights, device=self.model.device) if disc_weights is not None else \
-            PoseDiscriminator(seed=0, device=self.model.device)
+        self.disc = PoseDiscriminator(disc_weights, device=self.model.device, grad_precision=gp) if disc_weights is not None else \
+            PoseDiscriminator(seed=0, device=self.model.device, grad_precision=gp)
         self.smpl = smpl_model if hasattr(smpl_model, 'consts') else SMPL(smpl_model)
         make = optimizer or (lambda params, lr: torch.optim.Adam(params, lr))
         self.e_params = list(self.model.parameters())
@@ -467,7 +476,7 @@ class _TrainTrunk(object):
     them.  Called with images (B, T, S, S, 3) -> (phis (B, T, 2048), the plan that made them): frozen, without autograd; trainable
     (freeze_phi=False), on the graph of trunk.TrainableResNet."""
 
-    def __init__(self, w, device, trainable=False):
+    def __init__(self, w, device, trainable=False, grad_precision='fp32'):
         from .nets import PackedResNet, ResNetBatchNorm
         p = 'resnet_v2_50'
         need = [p + '/conv1/weights', p + '/conv1/biases']
@@ -482,11 +491,12 @@ class _TrainTrunk(object):
             raise _lib.HDError('precomputed_phi=False runs the ResNet: weights lack %d resnet_v2_50 variables, e.g. %s'
                                % (len(missing), missing[0]))
         self.device = device
+        self.grad_precision = grad_precision
         self._plans = {}
         self.net = None
         if trainable:
             from .trunk import TrainableResNet
-            self.net = TrainableResNet(w, device)
+            self.net = TrainableResNet(w, device, grad_precision=grad_precision)
             self.bn = self.net.bn
             return
         with torch.cuda.device(device):
@@ -498,7 +508,7 @@ class _TrainTrunk(object):
         key = (n, size)
         if key not in self._plans:
             self._plans.clear()                   # one batch shape at a time: a plan holds gigabytes of activations at 224 x 224
-            self._plans[key] = ResNetTrainPlan(self.packed, self.bn, n, size)
+            self._plans[key] = ResNetTrainPlan(self.packed, self.bn, n, size, grad_precision=self.grad_precision)
         return self._plans[key]
 
     def __call__(self, images):

@@ -5,7 +5,7 @@ This is what the reference trains in its default configuration (freeze_phi=True,
 after the ResNet.  Each forward runs the kernels and the packing of the inference plans (nets.FMoviePlan / IEFPlan fast heads,
 engine.PackedHal), so its outputs are bit-identical to HMMREngine's; the weights are packed on the device (hd_pack_weight) and repacked
 before a forward whenever a parameter was changed in place (optimizer.step()).  The backward (csrc/net_grad.cu + hd_conv_gemm in its
-3xTF32 mode) is first-order, deterministic and follows the inference graph: dropout is the identity (is_training=False).
+3xTF32 mode, or 1xTF32 with TrainConfig.grad_precision='tf32') is first-order, deterministic and follows the inference graph: dropout is the identity (is_training=False).
 
 All arithmetic goes through libhd_b200.so; torch provides buffers, streams and the autograd plumbing.  The user's loss and optimizer
 are ordinary torch code:
@@ -28,7 +28,7 @@ from torch.autograd.function import once_differentiable
 
 from . import _lib
 from ._lib import lib, check, fptr, current_stream, ConvDesc
-from .nets import FAST_HEADS, GN_EPS, GN_GROUPS, PackedConv, require_training_impl, sync_packing, weight_tmap
+from .nets import FAST_HEADS, GN_EPS, GN_GROUPS, PackedConv, grad_one_pass, require_training_impl, sync_packing, weight_tmap
 
 F32 = torch.float32
 
@@ -85,9 +85,10 @@ def repack_stale(packs, seen, param):
     return len(stale)
 
 
-def _tf32_gemm(a, M, K, a_ld, b, out, out_ld, res=None, T=1, KH=1, pad=0, stream=None):
-    """out[M', Cout] = (implicit conv of) a . B on the 3xTF32 tensor-core kernel.  b: a BackwardDataPack or an operand tuple
-    (hi, lo, tmap_hi, tmap_lo, Cout) from _bt_operand.  T / KH / pad > 1: a KH x 1 conv over T of M = B clips."""
+def _tf32_gemm(a, M, K, a_ld, b, out, out_ld, res=None, T=1, KH=1, pad=0, stream=None, one_pass=False):
+    """out[M', Cout] = (implicit conv of) a . B on the 3xTF32 tensor-core kernel (one_pass: 1xTF32, B's head alone).  b: a
+    BackwardDataPack or an operand tuple (hi, lo, tmap_hi, tmap_lo, Cout) from _bt_operand.  T / KH / pad > 1: a KH x 1 conv over T of
+    M = B clips."""
     d = ConvDesc()
     d.in_, d.in_ld = a.data_ptr(), a_ld
     d.n_img, d.H, d.W, d.Cin = M, T, 1, K
@@ -97,24 +98,30 @@ def _tf32_gemm(a, M, K, a_ld, b, out, out_ld, res=None, T=1, KH=1, pad=0, stream
     else:
         hi, lo, th, tl, Cout = b
     d.w_kn = hi.data_ptr()
-    d.w_nk_hi, d.w_nk_lo = hi.data_ptr(), lo.data_ptr()
+    d.w_nk_hi = hi.data_ptr()
     d.Cout, d.K_pad = Cout, KH * K
     if res is not None:
         d.res, d.res_ld, d.res_H, d.res_W, d.res_stride = res.data_ptr(), out_ld, T, 1, 1
     d.out, d.out_ld = out.data_ptr(), out_ld
-    d.impl = _lib.HD_IMPL_TC_3XTF32
-    d.tmap_hi, d.tmap_lo = C.cast(th, C.c_void_p), C.cast(tl, C.c_void_p)
-    check(lib.hd_conv_gemm(C.byref(d), current_stream() if stream is None else stream), 'hd_conv_gemm (backward, 3xTF32)')
+    d.tmap_hi = C.cast(th, C.c_void_p)
+    if one_pass:
+        d.impl = _lib.HD_IMPL_TC_1XTF32
+    else:
+        d.impl = _lib.HD_IMPL_TC_3XTF32
+        d.w_nk_lo, d.tmap_lo = lo.data_ptr(), C.cast(tl, C.c_void_p)
+    check(lib.hd_conv_gemm(C.byref(d), current_stream() if stream is None else stream),
+          'hd_conv_gemm (backward, %s)' % ('1xTF32' if one_pass else '3xTF32'))
 
 
-def _bt_operand(pieces, cols, k_pad, st):
+def _bt_operand(pieces, cols, k_pad, st, one_pass=False):
     """B operand of a weight-gradient GEMM: the row blocks `pieces` = [(x, rows, ld)] of an upstream gradient stacked along K,
-    transposed and TF32-split into [roundup64(cols), k_pad] (zero past the real rows / columns)."""
+    transposed and TF32-split into [roundup64(cols), k_pad] (zero past the real rows / columns).  one_pass: the round-to-nearest TF32
+    head alone (lo and its map are None)."""
     rows = _round(cols, 64)
     hi = torch.empty((rows, k_pad), dtype=F32, device=pieces[0][0].device)
-    lo = torch.empty_like(hi)
+    lo = None if one_pass else torch.empty_like(hi)
     _stack_t(pieces, cols, k_pad, 1, hi, lo, rows, st)
-    return (hi, lo, weight_tmap(hi), weight_tmap(lo), cols), (hi, lo)
+    return (hi, lo, weight_tmap(hi), None if one_pass else weight_tmap(lo), cols), (hi, lo)
 
 
 def _stack_t(pieces, cols, k_pad, mode, hi, lo, out_rows, st):
@@ -137,10 +144,10 @@ def _col_sum(x, rows, cols, ld, out, st):
     check(lib.hd_col_sum(fptr(x), rows, cols, ld, fptr(out), st), 'hd_col_sum')
 
 
-def _wgrad(xt, M, k_pad, g_pieces, cols, out, st):
-    """out[M, cols] = xt . (stacked g) : the weight gradient, 3xTF32."""
-    op, _keep = _bt_operand(g_pieces, cols, k_pad, st)
-    _tf32_gemm(xt, M, k_pad, k_pad, op, out, cols, stream=st)
+def _wgrad(xt, M, k_pad, g_pieces, cols, out, st, one_pass=False):
+    """out[M, cols] = xt . (stacked g) : the weight gradient, 3xTF32 (one_pass: 1xTF32)."""
+    op, _keep = _bt_operand(g_pieces, cols, k_pad, st, one_pass)
+    _tf32_gemm(xt, M, k_pad, k_pad, op, out, cols, stream=st, one_pass=one_pass)
 
 
 # ------------------------------------------------------------------------------------------------------------------------------------
@@ -205,11 +212,11 @@ def fmovie_backward(model, saved, g):
                   'hd_groupnorm_stats')
             check(lib.hd_im2col_t(fptr(src), B, T, Cc, 3, 1, fptr(gain), fptr(offset), 1, fptr(xt), kp, kp, st), 'hd_im2col_t')
             dW = torch.empty((3, 1, Cc, Cc), dtype=F32, device=dev)
-            _wgrad(xt, 3 * Cc, kp, [(gin, BT, Cc)], Cc, dW, st)
+            _wgrad(xt, 3 * Cc, kp, [(gin, BT, Cc)], Cc, dW, st, model.one_pass)
             db = torch.empty(Cc, dtype=F32, device=dev)
             _col_sum(gin, BT, Cc, Cc, db, st)
             # d relu(gn(src)) = conv(gin, W'); then the GroupNorm + ReLU backward (+ the block's residual gradient for gn1)
-            _tf32_gemm(gin, B, Cc, Cc, model.fm_bwd[i][k - 1], dact, Cc, T=T, KH=3, pad=1, stream=st)
+            _tf32_gemm(gin, B, Cc, Cc, model.fm_bwd[i][k - 1], dact, Cc, T=T, KH=3, pad=1, stream=st, one_pass=model.one_pass)
             check(lib.hd_groupnorm_relu_backward(fptr(src), fptr(gam), fptr(bet), fptr(dact), fptr(addend) if addend is not None else None,
                                                  fptr(gout), fptr(pg), fptr(pb), B, T, Cc, GN_GROUPS, GN_EPS, 1, st),
                   'hd_groupnorm_relu_backward')
@@ -265,7 +272,7 @@ def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st):
             G[2].copy_(torch.as_strided(g, (N, d), (g_ld, 1)))
         # dpre2 = (g . W3^T) * (h2 > 0);  dpre1 = (dpre2 . W2^T) * (h1 > 0);  dprev = g + dpre1 . W1theta^T
         check(lib.hd_fc_small_dgrad(fptr(gs), gld, fptr(head['W3t']), 1024, d, fptr(h2[s]), fptr(DP2[s]), N, st), 'hd_fc_small_dgrad')
-        _tf32_gemm(DP2[s], N, 1024, 1024, head['fc2_bwd'], DP1[s], 1024, stream=st)
+        _tf32_gemm(DP2[s], N, 1024, 1024, head['fc2_bwd'], DP1[s], 1024, stream=st, one_pass=model.one_pass)
         check(lib.hd_relu_backward(fptr(h1[s]), fptr(DP1[s]), fptr(DP1[s]), N * 1024, st), 'hd_relu_backward')
         dst = G[s - 1] if s > 0 else dstart
         check(lib.hd_ief_fc3(fptr(DP1[s]), fptr(head['W1tT']), fptr(model._zeros), fptr(gs), gld, fptr(dst), d, N, 1024, d, st),
@@ -281,12 +288,13 @@ def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st):
     _col_sum(DP2, 3 * N, 1024, 1024, b2, st)
     _col_sum(G, 3 * N, d, d, b3, st)
     feat = head['feat']
-    _wgrad(_xt([(phi, N, feat)], feat, kp1, st), feat, kp1, [(dP, N, 1024)], 1024, W1, st)
-    _wgrad(_xt([(t, N, ld) for t, ld in ins], d, kp3, st), d, kp3, [(DP1.view(3 * N, 1024), 3 * N, 1024)], 1024, W1[feat:], st)
-    _wgrad(_xt([(h1.view(3 * N, 1024), 3 * N, 1024)], 1024, kp3, st), 1024, kp3, [(DP2.view(3 * N, 1024), 3 * N, 1024)], 1024, W2, st)
-    _wgrad(_xt([(h2.view(3 * N, 1024), 3 * N, 1024)], 1024, kp3, st), 1024, kp3, [(G.view(3 * N, d), 3 * N, d)], d, W3, st)
+    op = model.one_pass
+    _wgrad(_xt([(phi, N, feat)], feat, kp1, st), feat, kp1, [(dP, N, 1024)], 1024, W1, st, op)
+    _wgrad(_xt([(t, N, ld) for t, ld in ins], d, kp3, st), d, kp3, [(DP1.view(3 * N, 1024), 3 * N, 1024)], 1024, W1[feat:], st, op)
+    _wgrad(_xt([(h1.view(3 * N, 1024), 3 * N, 1024)], 1024, kp3, st), 1024, kp3, [(DP2.view(3 * N, 1024), 3 * N, 1024)], 1024, W2, st, op)
+    _wgrad(_xt([(h2.view(3 * N, 1024), 3 * N, 1024)], 1024, kp3, st), 1024, kp3, [(G.view(3 * N, d), 3 * N, d)], d, W3, st, op)
     out = torch.empty((N, feat), dtype=F32, device=dev) if dphi is None else dphi
-    _tf32_gemm(dP, N, 1024, 1024, head['fc1_bwd'], out, feat, res=dphi, stream=st)
+    _tf32_gemm(dP, N, 1024, 1024, head['fc1_bwd'], out, feat, res=dphi, stream=st, one_pass=op)
     return dstart, [W1, b1, W2, b2, W3, b3], out
 
 
@@ -314,17 +322,17 @@ def hal_backward(model, x, h1, h2, g):
     dh2, dh1, dx = (torch.empty((N, 2048), dtype=F32, device=dev) for _ in range(3))
     for inp, gin, name in ((h2, g, 'fc3'), (h1, dh2, 'fc2'), (x, dh1, 'fc1')):
         W, b = torch.empty((2048, 2048), dtype=F32, device=dev), torch.empty(2048, dtype=F32, device=dev)
-        _wgrad(_xt([(inp, N, 2048)], 2048, kp, st), 2048, kp, [(gin, N, 2048)], 2048, W, st)
+        _wgrad(_xt([(inp, N, 2048)], 2048, kp, st), 2048, kp, [(gin, N, 2048)], 2048, W, st, model.one_pass)
         _col_sum(gin, N, 2048, 2048, b, st)
         grads = [W, b] + grads
         if name == 'fc3':
-            _tf32_gemm(g, N, 2048, 2048, L['fc3_bwd'], dh2, 2048, stream=st)
+            _tf32_gemm(g, N, 2048, 2048, L['fc3_bwd'], dh2, 2048, stream=st, one_pass=model.one_pass)
             check(lib.hd_relu_backward(fptr(h2), fptr(dh2), fptr(dh2), N * 2048, st), 'hd_relu_backward')
         elif name == 'fc2':
-            _tf32_gemm(dh2, N, 2048, 2048, L['fc2_bwd'], dh1, 2048, stream=st)
+            _tf32_gemm(dh2, N, 2048, 2048, L['fc2_bwd'], dh1, 2048, stream=st, one_pass=model.one_pass)
             check(lib.hd_relu_backward(fptr(h1), fptr(dh1), fptr(dh1), N * 2048, st), 'hd_relu_backward')
         else:
-            _tf32_gemm(dh1, N, 2048, 2048, L['fc1_bwd'], dx, 2048, res=g, stream=st)
+            _tf32_gemm(dh1, N, 2048, 2048, L['fc1_bwd'], dx, 2048, res=g, stream=st, one_pass=model.one_pass)
     return dx, grads
 
 
@@ -487,7 +495,10 @@ class TemporalModel(nn.Module):
     + split for T*64 <= 1280 with HD_FAST_HEADS on, GroupNorm statistics + conv prologue otherwise), so it is bit-identical to the engine
     at every T.  The IEF heads always run IEFPlan's fast-head kernels, whose saved h1 / h2 the backward reads; the HD_FAST_HEADS=0 A/B
     switch of the inference plans (generic IEF descriptors) does not apply here, and with it set the engine's IEF outputs differ from
-    this model's in the last bits."""
+    this model's in the last bits.
+
+    The backward's GEMMs follow `config.grad_precision` when the config has one (objective.TrainConfig): 'fp32' (3xTF32, the default)
+    or 'tf32' (1xTF32, nets.GRAD_PRECISIONS)."""
 
     def __init__(self, weights, config=None, device=None):
         super().__init__()
@@ -495,6 +506,7 @@ class TemporalModel(nn.Module):
         from .engine import load_weights
         self.config = config or HMMRConfig()
         require_training_impl(self.config.impl, 'TemporalModel')
+        self.one_pass = grad_one_pass(getattr(self.config, 'grad_precision', 'fp32'), 'TemporalModel')
         if not torch.cuda.is_available():
             raise _lib.HDError('TemporalModel needs a CUDA device: the hot path has no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)

@@ -7,7 +7,7 @@ reference builds the trunk with weight_decay=e_wd (trainer_sequence_fc.py:571), 
 regularisation losses to e_loss, so the trunk trains without weight decay, and so does this module.
 
 The forward is nets.ResNetTrainPlan with keep=True (its phis are bit-identical to the frozen trunk's); the backward is the plan's
-`backward` (csrc/resnet_grad.cu + hd_conv_gemm 3xTF32).  A parameter changed in place (optimizer.step()) repacks its forward pack (for
+`backward` (csrc/resnet_grad.cu + hd_conv_gemm 3xTF32, or 1xTF32 with grad_precision='tf32').  A parameter changed in place (optimizer.step()) repacks its forward pack (for
 conv1, the padded fp16 plane layout as well) and its data-gradient pack on the device before their next use.
 
     net = TrainableResNet(weights)                     # anything engine.load_weights accepts, with the resnet_v2_50/* variables
@@ -24,7 +24,7 @@ from torch import nn
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from .nets import PackedResNet, ResNetBatchNorm, ResNetTrainPlan, RESNET_BLOCKS, sync_packing
+from .nets import PackedResNet, ResNetBatchNorm, ResNetTrainPlan, RESNET_BLOCKS, grad_one_pass, sync_packing
 from .trainable import BackwardDataPack, repack_stale
 
 F32 = torch.float32
@@ -81,11 +81,14 @@ class ResNetFunction(torch.autograd.Function):
 class TrainableResNet(nn.Module):
     """The trunk's trainable variables as fp32 parameters on one CUDA device, addressable by TF name (`net.param(name)`), and the
     training-mode forward over them.  The batch-norm gamma / beta parameters share storage with `bn.gamma` / `bn.beta`, which the plans
-    read in place; conv weights and biases are read in place by their packs and epilogues."""
+    read in place; conv weights and biases are read in place by their packs and epilogues.  grad_precision: 'fp32' (3xTF32 weight and
+    data gradients) or 'tf32' (1xTF32, nets.GRAD_PRECISIONS); the forward is the same in both."""
 
-    def __init__(self, weights, device=None, blocks=RESNET_BLOCKS):
+    def __init__(self, weights, device=None, blocks=RESNET_BLOCKS, grad_precision='fp32'):
         super().__init__()
         from .engine import load_weights
+        grad_one_pass(grad_precision, 'TrainableResNet')
+        self.grad_precision = grad_precision
         if not torch.cuda.is_available() and (device is None or torch.device(device).type == 'cuda'):
             raise _lib.HDError('TrainableResNet needs a CUDA device: the hot path has no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
@@ -146,7 +149,7 @@ class TrainableResNet(nn.Module):
         if key not in self._plans:
             self._plans.clear()
             with torch.cuda.device(self.device) if self.device.type == 'cuda' else contextlib.nullcontext():
-                self._plans[key] = ResNetTrainPlan(self.packed, self.bn, n, size, keep=True)
+                self._plans[key] = ResNetTrainPlan(self.packed, self.bn, n, size, keep=True, grad_precision=self.grad_precision)
         return self._plans[key]
 
     def gradient_of(self, name, grads):

@@ -167,7 +167,10 @@ int hd_bn_moving_update(const float *mean, const float *var, long long rows, int
 /* ---- backward of the training-mode trunk (csrc/resnet_grad.cu): what the ResNet needs to train with freeze_phi=False
  * (trainer_sequence_fc.py:681-685).  Deterministic: no atomics, every sum over a partition fixed by the shapes and merged in a fixed
  * order, so repeats are bit-identical and results do not depend on the device's SM count.  Every argument is checked before any launch
- * (HD_ERR_INVALID). ----
+ * (HD_ERR_INVALID).  The TF32 gradient mode of training (grad_precision='tf32' in Python) runs the weight gradients as
+ * hd_conv_wgrad_ex(impl HD_IMPL_TC_1XTF32) and the data gradients as hd_conv_gemm impl 2 over the backward-data pack's head (w_nk_lo,
+ * tmap_lo NULL): one TF32 MMA per product on round-to-nearest heads; the batch-norm, pool and zero-insertion entries are the same in
+ * both modes. ----
  * hd_conv_wgrad: the weight gradient of a conv with hd_conv_gemm's geometry (x [n_img, H, W, Cin] at pixel pitch x_ld; output
  *   [n_img, Ho, Wo, Cout]; input pixel of (oy, ox, ky, kx) = (oy*stride - pad_t + ky, ox*stride - pad_l + kx), zero outside):
  *     dw[(ky*KW + kx)*Cin + ci, co] = sum_{n,oy,ox} a[n, iy, ix, ci] * dy[(n*Ho + oy)*Wo + ox][co]     (dy row pitch dy_ld)
@@ -182,6 +185,16 @@ size_t hd_conv_wgrad_workspace_bytes(long long pixels, int K, int Cout, int bias
 int hd_conv_wgrad(const float *x, long long x_ld, int n_img, int H, int W, int Cin, int Ho, int Wo, int KH, int KW, int stride, int pad_t,
                   int pad_l, const float *pre_scale, const float *pre_shift, const float *dy, long long dy_ld, int Cout, float *dw, float *db,
                   void *workspace, size_t workspace_bytes, void *stream);
+/* hd_conv_wgrad_ex: hd_conv_wgrad with a precision mode; hd_conv_wgrad is its impl = HD_IMPL_TC_3XTF32 call.
+ *   impl HD_IMPL_TC_3XTF32 (1): the 3xTF32 split above, FP32-class.
+ *   impl HD_IMPL_TC_1XTF32 (2): the TF32 training-gradient mode: every operand value is rounded to nearest to a TF32 head
+ *     ((bits + 0x1000) & 0xFFFFE000, after the prologue in fp32) and each product is one TF32 MMA, with no remainder; the chunking,
+ *     the round-to-nearest stage adds and the fp64 chunk-order merge are those of impl 1, so the result is deterministic and does
+ *     not depend on the SM count, and db (summed from the fp32 dy values) is bit-identical to impl 1's.  Same workspace.
+ *   Any other impl: HD_ERR_INVALID, before any launch. */
+int hd_conv_wgrad_ex(const float *x, long long x_ld, int n_img, int H, int W, int Cin, int Ho, int Wo, int KH, int KW, int stride, int pad_t,
+                     int pad_l, const float *pre_scale, const float *pre_shift, const float *dy, long long dy_ld, int Cout, float *dw,
+                     float *db, void *workspace, size_t workspace_bytes, int impl, void *stream);
 /* hd_bn_relu_backward: training-mode batch norm + ReLU backward over the raw map x [rows, C] (dense) that hd_bn_batch_stats normalised
  * into scale / shift (and its biased variance var), gamma the layer's gamma:
  *   z = fma(x, scale, shift), g = dz * (z > 0)  (TF's ReluGrad is 0 at 0), xhat = (x - mean_b) * rstd, rstd = 1 / sqrt(var + eps)
@@ -462,7 +475,8 @@ enum { HD_PACK_FORWARD = 0, HD_PACK_BACKWARD_DATA = 1 };
  * Rows / columns past the matrix are zero.  rows % 64 == 0, k_pad % 32 (tf32) / % 64 (fp16) == 0, hi / lo 16-byte aligned. */
 int hd_pack_weight(const float *w, int KH, int Cin, int Cout, int mode, int elem_bytes, void *hi, void *lo, int rows, int k_pad, void *stream);
 /* Transpose with optional split: hi[r*out_ld + k] (and lo) = split(x[k*ld + r]) for r < cols, k < rows; 0 for r in [cols, out_rows) or
- * k in [rows, out_cols).  mode 0 = plain fp32 (lo NULL), 1 = TF32 head / remainder, 2 = fp16 head / 2^11-scaled remainder.  Used for
+ * k in [rows, out_cols).  mode 0 = plain fp32 (lo NULL), 1 = TF32 head / remainder (lo NULL: the head alone, the B
+ * operand of a 1xTF32 GEMM), 2 = fp16 head / 2^11-scaled remainder.  Used for
  * the dY^T operand of a weight-gradient GEMM (mode 1; pass column offsets in hi / lo to stack several products along K) and for the
  * transposed inputs of FC weight gradients (mode 0). */
 int hd_transpose_split(const float *x, long long rows, int cols, long long ld, int mode, void *hi, void *lo, long long out_ld, int out_rows,
