@@ -101,6 +101,14 @@ class LossGrad(C.Structure):
     _fields_ = [('src', C.c_void_p), ('grad', C.c_void_p), ('numel', C.c_longlong)]
 
 
+HD_ADAM_MAX_TENSORS = 256
+
+
+class AdamTensor(C.Structure):
+    """Mirror of hd_adam_tensor."""
+    _fields_ = [('param', C.c_void_p), ('grad', C.c_void_p), ('m', C.c_void_p), ('v', C.c_void_p), ('numel', C.c_longlong)]
+
+
 HD_AUG_SRC_U8, HD_AUG_ROTATE, HD_AUG_FLIP = 1, 2, 4
 
 
@@ -208,6 +216,7 @@ SIGNATURES = {
     'hd_loss_workspace_bytes': (_sz, [_vp, _i]),
     'hd_loss_forward': (_i, [_vp, _i, _vp, _vp, _sz, _vp]),
     'hd_loss_backward': (_i, [_vp, _i, _vp, _i, _vp, _vp, _sz, _vp]),
+    'hd_adam_tf': (_i, [C.POINTER(AdamTensor), _i, _f, _f, _f, _f, _vp, _vp]),
     'hd_render_workspace_bytes': (_sz, [_i, _i, _i]),
     'hd_tube_augment': (_i, [C.POINTER(TubeAugArgs), _vp]),
     'hd_render_mesh': (_i, [_vp, _ll, _i, _i, _vp, _i, _vp, _i, C.POINTER(RenderParams), _vp, _i, _vp, _vp, _vp, _sz, _vp]),

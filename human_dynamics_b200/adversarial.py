@@ -47,6 +47,29 @@ def tf_names():
     return ['D_pose/%s/%s' % (n, k) for n, _ in DPOSE_LAYERS for k in ('weights', 'biases')]
 
 
+def stack_heads(w):
+    """{PARAM_NAMES name: float32 ndarray} from TF-named D_pose arrays (tf_names()): the 23 heads pose_out_j<j> stacked."""
+    a = {n: np.asarray(w[n], np.float32) for n in tf_names()}
+    a['D_pose/pose_out_j/weights'] = np.stack([a['D_pose/pose_out_j%d/weights' % j].reshape(CH) for j in range(J)])
+    a['D_pose/pose_out_j/biases'] = np.concatenate([a['D_pose/pose_out_j%d/biases' % j].reshape(1) for j in range(J)])
+    return a
+
+
+def split_heads(a):
+    """The reverse of stack_heads: {PARAM_NAMES name: array} -> {TF name: array in the reference's shape}."""
+    from .synthetic import DPOSE_LAYERS
+    out = {}
+    for name, shape in DPOSE_LAYERS:
+        if name.startswith('pose_out_j'):
+            j = int(name[len('pose_out_j'):])
+            out['D_pose/%s/weights' % name] = a['D_pose/pose_out_j/weights'][j].reshape(shape).copy()
+            out['D_pose/%s/biases' % name] = a['D_pose/pose_out_j/biases'][j:j + 1].copy()
+        else:
+            out['D_pose/%s/weights' % name] = a['D_pose/%s/weights' % name].reshape(shape)
+            out['D_pose/%s/biases' % name] = a['D_pose/%s/biases' % name]
+    return out
+
+
 def _load(weights):
     """engine.load_weights, except that a checkpoint's D_* variables are read (load_weights leaves them out, as Tester does)."""
     from . import tf_checkpoint
@@ -155,9 +178,7 @@ class PoseDiscriminator(nn.Module):
         missing = [n for n in tf_names() if n not in w]
         if missing:
             raise _lib.HDError('PoseDiscriminator: the weights lack %d D_pose variables (first: %s)' % (len(missing), missing[0]))
-        a = {n: np.asarray(w[n], np.float32) for n in tf_names()}
-        a['D_pose/pose_out_j/weights'] = np.stack([a['D_pose/pose_out_j%d/weights' % j].reshape(CH) for j in range(J)])
-        a['D_pose/pose_out_j/biases'] = np.concatenate([a['D_pose/pose_out_j%d/biases' % j].reshape(1) for j in range(J)])
+        a = stack_heads(w)
         self._params = nn.ParameterDict()
         for n in PARAM_NAMES:
             self._params[n] = nn.Parameter(torch.from_numpy(np.ascontiguousarray(a[n])).to(self.device))
@@ -214,15 +235,4 @@ class PoseDiscriminator(nn.Module):
 
     def tf_variables(self):
         """The D_pose/* variables under the reference's names and shapes: {name: float32 ndarray}."""
-        from .synthetic import DPOSE_LAYERS
-        a = {n: self.param(n).detach().cpu().numpy() for n in PARAM_NAMES}
-        out = {}
-        for name, shape in DPOSE_LAYERS:
-            if name.startswith('pose_out_j'):
-                j = int(name[len('pose_out_j'):])
-                out['D_pose/%s/weights' % name] = a['D_pose/pose_out_j/weights'][j].reshape(shape).copy()
-                out['D_pose/%s/biases' % name] = a['D_pose/pose_out_j/biases'][j:j + 1].copy()
-            else:
-                out['D_pose/%s/weights' % name] = a['D_pose/%s/weights' % name].reshape(shape)
-                out['D_pose/%s/biases' % name] = a['D_pose/%s/biases' % name]
-        return out
+        return split_heads({n: self.param(n).detach().cpu().numpy() for n in PARAM_NAMES})

@@ -11,6 +11,9 @@ sum of its terms, with the weights of trainer_sequence_fc.py:280-310.
         out = trainer.step(batch, mocap)              # device scalars, no synchronise
     trainer.save_checkpoint('/path/model.ckpt-1000')  # Tester and PoseDiscriminator load it
 
+    trainer = HMMRTrainer(cfg, weights, smpl_model, optimizer=TFAdam)         # TF's Adam: the checkpoint holds the optimizer state
+    trainer = HMMRTrainer.resume(cfg, '/path/model.ckpt-1000', smpl_model)    # ... which resume restores (tf.train.Supervisor's restore)
+
 With precomputed_phi=False (the reference's online-augmentation path) a batch carries `images` (B, T, S, S, 3) float32 in [-1, 1], e.g.
 augment.TubeAugmentor(...)['images'], instead of `phis`: the frozen ResNet runs over all B*T crops in training mode (batch statistics,
 nets.ResNetTrainPlan) without autograd, and each `step` applies the trunk's update ops once (one moving-average step of its 49
@@ -20,8 +23,9 @@ save_checkpoint writes their trained values.  Like the reference (whose gather_l
 trunk trains without weight decay.
 
 Differences from the reference trainer: IEF dropout is the identity (the backward of trainable.TemporalModel follows the inference
-graph); torch's Adam adds eps to sqrt(v_hat) where TF's adds it to sqrt(v) before the bias correction; the static `use_hmr_only` branch
-is not built, and freeze_phi=False needs image input (precomputed phis have no trunk to train).  A frame with no visible keypoint in an optimal-camera term
+graph); the default optimizer, torch's Adam, adds eps to sqrt(v_hat) where TF's adds it to sqrt(v) before the bias correction, and
+`optimizer=optim.TFAdam` removes that difference (TF's arithmetic, with its slots, beta powers and global_step in the checkpoint, so
+that `HMMRTrainer.resume(config, prefix, smpl_model)` continues a run where it stopped); the static `use_hmr_only` branch is not built, and freeze_phi=False needs image input (precomputed phis have no trunk to train).  A frame with no visible keypoint in an optimal-camera term
 contributes 0 (the reference's procrustes2d_vis divides 0 / 0 there and the loss is NaN).  The moving statistics start from whatever
 `weights` holds, so a resumed run continues them; a fresh reference run restores only the trainable variables from its hmr_noS5
 checkpoint (trainer_sequence_fc.py:346-392), so its moving statistics start at 0 / 1 -- pass those values in `weights` to reproduce it.
@@ -337,7 +341,9 @@ class HMMRTrainer(object):
     d_opt): f_movie (and fc2_res with do_hallucinate) over precomputed phis, the IEF heads from the tiled mean_param, one SMPL call over
     every prediction set, the objective, D_pose on reals + fakes, and both updates from the same pre-step parameters.
 
-    `optimizer`: optional factory (params, lr) -> torch optimizer, default torch.optim.Adam.
+    `optimizer`: optional factory (params, lr) -> torch optimizer, default torch.optim.Adam; optim.TFAdam is TF's Adam, whose slots and
+    beta powers save_checkpoint writes.  `global_step` counts the applied updates like the reference's (both minimize calls pass it:
+    +2 per step that trains D, +1 with d_lw_pose = 0); it starts at the checkpoint's when `weights` is a checkpoint prefix, else at 0.
     With config.precomputed_phi=False, `weights` must also hold the resnet_v2_50/* variables (see the module docstring)."""
 
     def __init__(self, config, weights, smpl_model, disc_weights=None, optimizer=None, device=None):
@@ -368,6 +374,56 @@ class HMMRTrainer(object):
         self.e_opt = make(self.e_params, config.e_lr)
         self.d_opt = make(self.d_params, config.d_lr)
         self._objectives = {}
+        self.global_step = _checkpoint_step(weights)
+
+    @classmethod
+    def resume(cls, config, prefix, smpl_model, device=None):
+        """Continue a run from its checkpoint (tf.train.Supervisor's restore from logdir, trainer_sequence_fc.py:410-418): E, D and
+        the moving statistics from `prefix` as in the constructor, optim.TFAdam for both optimizers with every slot, both pairs of beta
+        powers (D's only when d_lw_pose > 0) and global_step restored.  A missing entry raises HDError naming it.  To fine-tune from a
+        checkpoint without optimizer state, construct with weights=prefix instead: the slots start at zero."""
+        from .optim import TFAdam
+        from .tf_checkpoint import is_checkpoint, load_checkpoint
+        prefix = prefix[:-len('.index')] if isinstance(prefix, str) and prefix.endswith('.index') else prefix
+        if not is_checkpoint(prefix):
+            raise _lib.HDError('HMMRTrainer.resume: %r is not a TensorFlow checkpoint prefix (no .index file)' % (prefix,))
+        tr = cls(config, prefix, smpl_model, disc_weights=prefix, optimizer=TFAdam, device=device)
+        want = tr.optimizer_state_names()
+        state = load_checkpoint(prefix, names=set(want))
+        missing = [n for n in want if n not in state]
+        if missing:
+            raise _lib.HDError('HMMRTrainer.resume: %s lacks %d optimizer entries, first: %s' % (prefix, len(missing), missing[0]))
+        trained = set(tr._e_names())
+        tr.e_opt.load_tf_slots(state, [n if n in trained else None for n in tr._e_param_names()])
+        d_trained = config.d_lw_pose > 0
+        if d_trained:
+            from .adversarial import PARAM_NAMES, stack_heads, tf_names
+            d = {}
+            for s in ('/Adam', '/Adam_1'):
+                d.update({k + s: a for k, a in stack_heads({n: state[n + s] for n in tf_names()}).items() if k in PARAM_NAMES})
+            d.update({k: state[k] for k in ('beta1_power_1', 'beta2_power_1')})
+            tr.d_opt.load_tf_slots(d, PARAM_NAMES, suffix='_1')
+        tr.global_step = int(state['global_step'])
+        return tr
+
+    def _e_param_names(self):
+        """The TF variable of each of e_params, in order."""
+        return list(self.model.names) + (list(self.trunk.net.names) if self.trunk is not None and self.trunk.net is not None else [])
+
+    def _e_names(self):
+        """The E variables the reference's optimizer holds (get_unfrozen_E_vars): fc2_res exists in its graph only with
+        do_hallucinate, so without it those parameters never get a gradient or slots here either."""
+        from .trainable import HAL_NAMES
+        return [n for n in self._e_param_names() if self.config.do_hallucinate or n not in HAL_NAMES]
+
+    def optimizer_state_names(self):
+        """The optimizer entries a TFAdam trainer's checkpoint holds, as TF names them (E's optimizer is created first in
+        setup_optimizers, so its beta powers take the plain names and D's the _1 suffix; D's only when D trains)."""
+        from .adversarial import tf_names
+        names = [n + s for n in self._e_names() for s in ('/Adam', '/Adam_1')] + ['beta1_power', 'beta2_power']
+        if self.config.d_lw_pose > 0:
+            names += [n + s for n in tf_names() for s in ('/Adam', '/Adam_1')] + ['beta1_power_1', 'beta2_power_1']
+        return names + ['global_step']
 
     def objective(self, B, T, K):
         key = (B, T, K)
@@ -446,22 +502,38 @@ class HMMRTrainer(object):
             p.grad = g
         self.e_opt.step()
         self.e_opt.zero_grad(set_to_none=True)
+        self.global_step += 1
         if use_d:
             for p, g in zip(self.d_params, gd):
                 p.grad = g
             self.d_opt.step()
             self.d_opt.zero_grad(set_to_none=True)
+            self.global_step += 1
         out = {k: v.detach() for k, v in named.items()}
         out['e_loss'], out['d_loss'] = e_loss.detach(), d_loss.detach()
         return out
 
     def tf_variables(self):
         """E and D variables; with image input the trunk's moving statistics are the current ones, and with freeze_phi=False its
-        trained weights, biases, gamma and beta as well."""
-        v = self.model.tf_variables()
+        trained weights, biases, gamma and beta as well.  With optim.TFAdam optimizers, also their state (optimizer_state_names()):
+        the slots in each variable's shape, the beta powers and global_step (int64).  Optimizer entries that came in with `weights`
+        are never passed through."""
+        from .optim import TFAdam
+        v = {k: a for k, a in self.model.tf_variables().items() if not _optimizer_entry(k)}
         if self.trunk is not None:
             v.update(self.trunk.bn.moving() if self.trunk.net is None else self.trunk.net.tf_variables())
         v.update(self.disc.tf_variables())
+        if isinstance(self.e_opt, TFAdam):
+            s = self.e_opt.tf_slots(self._e_param_names())
+            v.update({k: a.reshape(np.shape(v[k.rsplit('/', 1)[0]])) if k.endswith(('/Adam', '/Adam_1')) else a for k, a in s.items()})
+            v['global_step'] = np.asarray(self.global_step, np.int64)
+        if isinstance(self.d_opt, TFAdam) and self.config.d_lw_pose > 0:
+            from .adversarial import PARAM_NAMES, split_heads
+            s = self.d_opt.tf_slots(PARAM_NAMES, suffix='_1')
+            for sfx in ('/Adam', '/Adam_1'):
+                if all(n + sfx in s for n in PARAM_NAMES):
+                    v.update({k + sfx: a for k, a in split_heads({n: s[n + sfx] for n in PARAM_NAMES}).items()})
+            v.update({k: s[k] for k in ('beta1_power_1', 'beta2_power_1')})
         return v
 
     def save_checkpoint(self, prefix):
@@ -469,6 +541,23 @@ class HMMRTrainer(object):
         from .tf_checkpoint import save_checkpoint
         save_checkpoint(prefix, self.tf_variables())
         return prefix
+
+
+def _optimizer_entry(name):
+    """A TF optimizer entry rather than a model variable: an Adam slot, a beta power or the step counter."""
+    return name.rsplit('/', 1)[-1] in ('Adam', 'Adam_1') or name in ('global_step', 'beta1_power', 'beta2_power', 'beta1_power_1',
+                                                                       'beta2_power_1')
+
+
+def _checkpoint_step(weights):
+    """global_step of a checkpoint prefix (load_checkpoint's default skip drops it), 0 for anything else or a checkpoint without one."""
+    from .tf_checkpoint import is_checkpoint, load_checkpoint
+    if not isinstance(weights, str):
+        return 0
+    prefix = weights[:-len('.index')] if weights.endswith('.index') else weights
+    if not is_checkpoint(prefix):
+        return 0
+    return int(load_checkpoint(prefix, names=['global_step']).get('global_step', 0))
 
 
 class _TrainTrunk(object):

@@ -573,6 +573,28 @@ int hd_loss_forward(const hd_loss_term *terms, int n, float *values, void *ws, s
 int hd_loss_backward(const hd_loss_term *terms, int n, const hd_loss_grad *grads, int n_grads, const float *dvalues, const void *ws,
                      size_t ws_bytes, void *stream);
 
+/* ---- TensorFlow's Adam (tf.train.AdamOptimizer of the reference trainer, trainer_sequence_fc.py:326 / 752-768; csrc/adam.cu) ----
+ * hd_adam_tf applies TF 1.8's ApplyAdam (use_nesterov=False) to every tensor of t[0..n), element by element, in fp32 with one
+ * rounding per operation (IEEE division and square root, no contraction):
+ *   alpha = lr * sqrt(1 - beta2_power) / (1 - beta1_power)
+ *   m += (1 - beta1) * (g - m);   v += (1 - beta2) * (g*g - v);   param -= (alpha * m) / (epsilon + sqrt(v))
+ * then TF's _finish, once after every tensor: beta1_power *= beta1, beta2_power *= beta2 (fp32).  The powers live on the device
+ * (powers[0] = beta1_power, powers[1] = beta2_power; TF creates them as beta1 and beta2).  The table is passed by value in the
+ * kernel parameters, HD_ADAM_MAX_TENSORS at a time: ceil(n / HD_ADAM_MAX_TENSORS) update launches (none for a group with no
+ * element) and one single-thread launch for the powers.  No host synchronisation, no host-to-device copy.  A tensor whose four
+ * pointers are 16-byte aligned moves in 16-byte loads and stores; any other runs element by element.  Tensors must not overlap.
+ * HD_ERR_INVALID (before any launch): t NULL with n > 0, n < 0, a NULL pointer in an entry, numel < 0, powers NULL, or a non-finite
+ * lr, beta1, beta2 or epsilon. */
+enum { HD_ADAM_MAX_TENSORS = 256 };
+typedef struct {
+  float *param;
+  const float *grad;
+  float *m;                       /* TF's slot <var>/Adam */
+  float *v;                       /* TF's slot <var>/Adam_1 */
+  long long numel;
+} hd_adam_tensor;
+int hd_adam_tf(const hd_adam_tensor *t, int n, float lr, float beta1, float beta2, float epsilon, float *powers, void *stream);
+
 /* ---- Mesh rendering (the visualiser of src/util/render/nmr_renderer.py:43-240: NMR with camera_mode='look_at',
  * perspective=False, anti_aliasing and fill_back on), one colour per mesh.  The model is R1-R8 of oracle/render_ref.py:
  *   x = s*(X + tx), y = -s*(Y + ty), z = Z - eye_z  (R1); a 2S x 2S sample grid whose sample (r, c) sits at image
