@@ -26,8 +26,8 @@ from torch.autograd.function import once_differentiable
 
 from . import _lib
 from ._lib import lib, check, fptr, current_stream
-from .nets import PackedConv, grad_one_pass, sync_packing
-from .trainable import BackwardDataPack, _col_sum, _round, _tf32_gemm, _vp, _wgrad, _xt, repack_stale
+from .nets import BackwardDataPack, PackedConv, dgrad_op, grad_one_pass
+from .trainable import TrainableModule, _col_sum, _round, _vp, _wgrad, _xt
 
 F32 = torch.float32
 J, CH, FLAT, HID = 23, 32, 736, 1024
@@ -109,9 +109,9 @@ def dpose_backward(d, x, saved, g, want_dx, want_dw):
     dflat = torch.empty((N, FLAT), dtype=F32, device=dev)
     # df2 = g[:, 23] w_out^T * (f2 > 0);  df1 = (df2 . Wfc2^T) * (f1 > 0);  dflat = df1 . Wfc1^T
     check(lib.hd_fc_small_dgrad(_vp(g, J * 4), J + 1, fptr(P[10]), HID, 1, fptr(f2), fptr(df2), N, st), 'hd_fc_small_dgrad')
-    _tf32_gemm(df2, N, HID, HID, d.fc2_bwd, df1, HID, stream=st, one_pass=d.one_pass)
+    dgrad_op(d.fc2_bwd, df2, N, 1, 1, 1, 1, df1, one_pass=d.one_pass).run(st)
     check(lib.hd_relu_backward(fptr(f1), fptr(df1), fptr(df1), N * HID, st), 'hd_relu_backward')
-    _tf32_gemm(df1, N, HID, HID, d.fc1_bwd, dflat, FLAT, stream=st, one_pass=d.one_pass)
+    dgrad_op(d.fc1_bwd, df1, N, 1, 1, 1, 1, dflat, one_pass=d.one_pass).run(st)
     dx = torch.empty((N, J, 9), dtype=F32, device=dev) if want_dx else None
     ws_bytes = int(lib.hd_dpose_workspace_bytes(N)) if want_dw else 0
     ws = torch.empty(ws_bytes // 4, dtype=F32, device=dev) if want_dw else None
@@ -151,14 +151,14 @@ class DPoseFunction(torch.autograd.Function):
         need = ctx.needs_input_grad
         want_dw = any(need[2:])
         if want_dw or need[1]:
-            repack_stale(disc._bwd_packs, disc._bwd_seen, disc.param)
+            disc.sync_bwd_packs()
         x, *saved = ctx.saved_tensors
         dx, grads = dpose_backward(disc, x, saved, g.contiguous(), need[1], want_dw)
         grads = grads or [None] * len(PARAM_NAMES)
         return (None, dx) + tuple(gr if n else None for gr, n in zip(grads, need[2:]))
 
 
-class PoseDiscriminator(nn.Module):
+class PoseDiscriminator(TrainableModule):
     """D_pose as fp32 parameters on one CUDA device.  `weights`: anything engine.load_weights accepts that holds the D_pose/* variables
     (other variables are ignored); without it, slim's default initialisation from `seed` (synthetic.make_dpose_weights).
 
@@ -179,7 +179,6 @@ class PoseDiscriminator(nn.Module):
         if missing:
             raise _lib.HDError('PoseDiscriminator: the weights lack %d D_pose variables (first: %s)' % (len(missing), missing[0]))
         a = stack_heads(w)
-        self._params = nn.ParameterDict()
         for n in PARAM_NAMES:
             self._params[n] = nn.Parameter(torch.from_numpy(np.ascontiguousarray(a[n])).to(self.device))
         self._p = [self._params[n] for n in PARAM_NAMES]
@@ -189,18 +188,9 @@ class PoseDiscriminator(nn.Module):
             self.fc2 = PackedConv(P[8], self.device, post_shift=P[9], post_relu=True, tc='auto')     # Cin 1024: fp16-split pack
             self.fc1_bwd = BackwardDataPack(P[6], 1, FLAT, HID)
             self.fc2_bwd = BackwardDataPack(P[8], 1, HID, HID)
-            sync_packing(self.device)
-        self._fwd_packs = [(PARAM_NAMES[6], self.fc1), (PARAM_NAMES[8], self.fc2)]
-        self._bwd_packs = [(PARAM_NAMES[6], self.fc1_bwd), (PARAM_NAMES[8], self.fc2_bwd)]
-        self._seen = {n: self.param(n)._version for n, _ in self._fwd_packs}
-        self._bwd_seen = {}
-
-    def param(self, name):
-        return self._params[name]
-
-    def sync_packs(self):
-        """Repack the fc weights whose parameter changed since they were last packed (called by each forward).  Returns the count."""
-        return repack_stale(self._fwd_packs, self._seen, self.param)
+        self._fwd_packs += [(PARAM_NAMES[6], self.fc1), (PARAM_NAMES[8], self.fc2)]
+        self._bwd_packs += [(PARAM_NAMES[6], self.fc1_bwd), (PARAM_NAMES[8], self.fc2_bwd)]
+        self._packs_written(self.device)
 
     def _input(self, rotmats):
         x = rotmats
@@ -217,7 +207,7 @@ class PoseDiscriminator(nn.Module):
         """rotmats (N, 23, 9) or (N, 23, 1, 9) -> logits (N, 24): the 23 per-joint scores, then the whole-pose score."""
         x = self._input(rotmats)
         self.sync_packs()
-        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self._p)):
+        if self._grad_on(PARAM_NAMES, x):
             return DPoseFunction.apply(self, x, *self._p)
         with torch.no_grad():
             return dpose_forward(self, x.detach())[0]

@@ -246,6 +246,54 @@ class PackedConv(object):
         return op
 
 
+class BackwardDataPack(object):
+    """PackedConv's backward twin: the transposed, tap-flipped weight of a conv whose conv is dX, written on the device from the fp32
+    weight [KH, Cin, Cout] (KH: the conv's taps; FC: 1) by hd_pack_weight(HD_PACK_BACKWARD_DATA): TF32 head / remainder
+    [roundup64(Cin), KH*Cout] for impl tc3, the B operand of dgrad_op."""
+
+    def __init__(self, weight, KH, Cin, Cout):
+        self.src, self.src_shape = weight, (KH, Cin, Cout)
+        self.Cout, self.K = Cin, KH * Cout
+        if self.K % 32 != 0:
+            raise _lib.HDError('BackwardDataPack: K = %d does not fit the TF32 packing' % self.K)
+        self.w_nk_hi = torch.empty(((Cin + 63) // 64 * 64, self.K), dtype=torch.float32, device=weight.device)
+        self.w_nk_lo = torch.empty_like(self.w_nk_hi)
+        self.tmap_hi, self.tmap_lo = weight_tmap(self.w_nk_hi), weight_tmap(self.w_nk_lo)
+
+    def repack(self, stream):
+        KH, Cin, Cout = self.src_shape
+        check(lib.hd_pack_weight(fptr(self.src), KH, Cin, Cout, _lib.HD_PACK_BACKWARD_DATA, 4, _vp(self.w_nk_hi), _vp(self.w_nk_lo),
+                                 self.w_nk_hi.shape[0], self.K, stream), 'hd_pack_weight')
+
+
+def dgrad_op(pack, inp, n, H, W, KH, KW, out, res=None, one_pass=False):
+    """A backward GEMM as an hd_conv_gemm op in its 3xTF32 mode (one_pass: 1xTF32 on the pack's head alone): out[n, H, W, pack.Cout]
+    (+ res) = the stride-1 SAME KH x KW conv of inp [n, H, W, Cin] with the B operand `pack`, Cin = pack.K / (KH*KW).
+
+    pack: a BackwardDataPack (the data gradient of a conv, or over the zero-inserted gradient of a strided conv2d_same 3x3; f_movie's
+    3x1 conv over n clips of H = T frames; an FC layer, H = W = KH = KW = 1), or any operand with its fields w_nk_hi / w_nk_lo /
+    tmap_hi / tmap_lo / Cout / K (a weight gradient's stacked upstream gradient).  The op holds `pack` and the tensors until it is
+    dropped."""
+    Cin, Cout = pack.K // (KH * KW), pack.Cout
+    d = ConvDesc()
+    d.in_, d.in_ld = inp.data_ptr(), Cin
+    d.n_img, d.H, d.W, d.Cin = n, H, W, Cin
+    d.Ho, d.Wo, d.KH, d.KW, d.stride, d.pad_t, d.pad_l = H, W, KH, KW, 1, KH // 2, KW // 2
+    d.w_kn = pack.w_nk_hi.data_ptr()
+    d.w_nk_hi = pack.w_nk_hi.data_ptr()
+    d.Cout, d.K_pad = Cout, pack.K
+    if res is not None:
+        d.res, d.res_ld, d.res_H, d.res_W, d.res_stride = res.data_ptr(), Cout, H, W, 1
+    d.out, d.out_ld = out.data_ptr(), Cout
+    d.tmap_hi = C.cast(pack.tmap_hi, C.c_void_p)
+    if one_pass:
+        d.impl = _lib.HD_IMPL_TC_1XTF32
+    else:
+        d.impl = _lib.HD_IMPL_TC_3XTF32
+        d.w_nk_lo, d.tmap_lo = pack.w_nk_lo.data_ptr(), C.cast(pack.tmap_lo, C.c_void_p)
+    return ConvOp(d, (pack, inp, out, res), (H, W))
+
+
 class SubsampleOp(object):
     """x[:, ::s, ::s, :] into a dense buffer (slim's max_pool2d(1x1, stride) shortcut): one op in a plan's op list."""
     __slots__ = ('src', 'dst', 'geom', 'd')
@@ -891,13 +939,13 @@ class ResNetTrainPlan(object):
                 ws_w = max(ws_w, lib.hd_conv_wgrad_workspace_bytes(n * pix, K, Cout, bias))
             u = {'gy': gy, 'gx': gx, 'H': H, 'Ho': Ho}
             op = self.one_pass
-            u['conv3'] = _dgrad_op(unit['conv3'], gy, n, Ho, Ho, 1, D1, one_pass=op)
-            u['conv2'] = _dgrad_op(unit['conv2'], D2 if s == 1 else Z, n, H, H, 3, D1, one_pass=op)
+            u['conv3'] = dgrad_op(unit['conv3'].bwd, gy, n, Ho, Ho, 1, 1, D1, one_pass=op)
+            u['conv2'] = dgrad_op(unit['conv2'].bwd, D2 if s == 1 else Z, n, H, H, 3, 3, D1, one_pass=op)
             if 'shortcut' in unit:
-                u['shortcut'] = _dgrad_op(unit['shortcut'], gy, n, H, H, 1, P, one_pass=op)
-                u['conv1'] = _dgrad_op(unit['conv1'], D2, n, H, H, 1, P, res=P, one_pass=op)
+                u['shortcut'] = dgrad_op(unit['shortcut'].bwd, gy, n, H, H, 1, 1, P, one_pass=op)
+                u['conv1'] = dgrad_op(unit['conv1'].bwd, D2, n, H, H, 1, 1, P, res=P, one_pass=op)
             else:
-                u['conv1'] = _dgrad_op(unit['conv1'], D2, n, H, H, 1, P, one_pass=op)
+                u['conv1'] = dgrad_op(unit['conv1'].bwd, D2, n, H, H, 1, 1, P, one_pass=op)
             ops.append(u)
             H = Ho
         self._bwd = dict(G=G, D1=D1, D2=D2, Z=Z, P=P, units=ops, ws_w=torch.empty(max(16, int(ws_w)), dtype=torch.uint8, device=p.device),
@@ -977,30 +1025,6 @@ class ResNetTrainPlan(object):
         self._wgrad(images, (n, self.size, self.size, 3, self.H1, self.H1, 7, 7, 2, 3, 3), None, P, 64, dW, db, st, self.one_pass)
         grads['resnet_v2_50/conv1/weights'], grads['resnet_v2_50/conv1/biases'] = dW, db
         return grads
-
-
-def _dgrad_op(conv, inp, n, H, W, KH, out, res=None, one_pass=False):
-    """The data gradient of a stride-1 KH x KH SAME conv (or, over the zero-inserted gradient, of a strided conv2d_same 3x3) as an
-    hd_conv_gemm op in its 3xTF32 mode (one_pass: 1xTF32 on the pack's head alone): out[n, H, W, Cin] (+ res) = conv(inp [n, H, W, Cout],
-    tap-flipped W^T = conv.bwd)."""
-    bwd = conv.bwd
-    d = ConvDesc()
-    d.in_, d.in_ld = inp.data_ptr(), conv.Cout
-    d.n_img, d.H, d.W, d.Cin = n, H, W, conv.Cout
-    d.Ho, d.Wo, d.KH, d.KW, d.stride, d.pad_t, d.pad_l = H, W, KH, KH, 1, KH // 2, KH // 2
-    d.w_kn = bwd.w_nk_hi.data_ptr()
-    d.w_nk_hi = bwd.w_nk_hi.data_ptr()
-    d.Cout, d.K_pad = conv.Cin, KH * KH * conv.Cout
-    if res is not None:
-        d.res, d.res_ld, d.res_H, d.res_W, d.res_stride = res.data_ptr(), conv.Cin, H, W, 1
-    d.out, d.out_ld = out.data_ptr(), conv.Cin
-    d.tmap_hi = C.cast(bwd.tmap_hi, C.c_void_p)
-    if one_pass:
-        d.impl = _lib.HD_IMPL_TC_1XTF32
-    else:
-        d.impl = _lib.HD_IMPL_TC_3XTF32
-        d.w_nk_lo, d.tmap_lo = bwd.w_nk_lo.data_ptr(), C.cast(bwd.tmap_lo, C.c_void_p)
-    return ConvOp(d, (conv, bwd, inp, out, res), (H, W))
 
 
 # ------------------------------------------------------------------------------------------------

@@ -42,7 +42,7 @@ from torch.autograd.function import once_differentiable
 from . import _lib
 from ._lib import lib, check, current_stream
 from .config import HMMRConfig
-from .nets import RESNET_BLOCKS, grad_one_pass, require_training_impl
+from .nets import grad_one_pass, require_training_impl
 
 F32 = torch.float32
 
@@ -567,15 +567,8 @@ class _TrainTrunk(object):
 
     def __init__(self, w, device, trainable=False, grad_precision='fp32'):
         from .nets import PackedResNet, ResNetBatchNorm
-        p = 'resnet_v2_50'
-        need = [p + '/conv1/weights', p + '/conv1/biases']
-        for b, (_, units, _) in enumerate(RESNET_BLOCKS, start=1):
-            for u in range(1, units + 1):
-                q = '%s/block%d/unit_%d/bottleneck_v2' % (p, b, u)
-                need += [q + '/conv%d/weights' % k for k in (1, 2, 3)] + [q + '/conv3/biases']
-                if u == 1:
-                    need += [q + '/shortcut/weights', q + '/shortcut/biases']
-        missing = [k for k in need if k not in w]
+        from .trunk import conv_names
+        missing = [k for k in conv_names() if k not in w]
         if missing:
             raise _lib.HDError('precomputed_phi=False runs the ResNet: weights lack %d resnet_v2_50 variables, e.g. %s'
                                % (len(missing), missing[0]))

@@ -88,7 +88,8 @@ class TFAdam(torch.optim.Optimizer):
         with torch.cuda.device(plan[3]):
             check(lib.hd_adam_tf(table.ctypes.data_as(C.POINTER(_lib.AdamTensor)), len(table), g['lr'], g['beta1'], g['beta2'],
                                  g['epsilon'], C.c_void_p(self._powers.data_ptr()), current_stream()), 'hd_adam_tf')
-        # a raw-pointer write does not move the version counter that repack_stale and the stale-graph check in trunk.py read
+        # a raw-pointer write does not move the version counter that trainable.TrainableModule's repacking and the stale-graph check in
+        # trunk.py read
         torch.autograd.graph.increment_version(items)
         return loss
 

@@ -20,6 +20,7 @@ are ordinary torch code:
 from __future__ import annotations
 
 import ctypes as C
+import types
 
 import numpy as np
 import torch
@@ -27,8 +28,9 @@ from torch import nn
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from ._lib import lib, check, fptr, current_stream, ConvDesc
-from .nets import FAST_HEADS, GN_EPS, GN_GROUPS, PackedConv, grad_one_pass, require_training_impl, sync_packing, weight_tmap
+from ._lib import lib, check, fptr, current_stream
+from .nets import (FAST_HEADS, GN_EPS, GN_GROUPS, BackwardDataPack, PackedConv, dgrad_op, grad_one_pass, require_training_impl,
+                   sync_packing, weight_tmap)
 
 F32 = torch.float32
 
@@ -39,25 +41,6 @@ def _vp(t, off=0):
 
 def _round(x, m):
     return (x + m - 1) // m * m
-
-
-class BackwardDataPack(object):
-    """The transposed, tap-flipped weight of a KH x 1 conv (FC: KH = 1) whose conv is dX, written on the device from the fp32 weight
-    [KH, Cin, Cout] by hd_pack_weight(HD_PACK_BACKWARD_DATA): TF32 head / remainder [roundup64(Cin), KH*Cout] for impl tc3."""
-
-    def __init__(self, weight, KH, Cin, Cout):
-        self.src, self.src_shape = weight, (KH, Cin, Cout)
-        self.Cout, self.K = Cin, KH * Cout
-        if self.K % 32 != 0:
-            raise _lib.HDError('BackwardDataPack: K = %d does not fit the TF32 packing' % self.K)
-        self.w_nk_hi = torch.empty((_round(Cin, 64), self.K), dtype=F32, device=weight.device)
-        self.w_nk_lo = torch.empty_like(self.w_nk_hi)
-        self.tmap_hi, self.tmap_lo = weight_tmap(self.w_nk_hi), weight_tmap(self.w_nk_lo)
-
-    def repack(self, stream):
-        KH, Cin, Cout = self.src_shape
-        check(lib.hd_pack_weight(fptr(self.src), KH, Cin, Cout, _lib.HD_PACK_BACKWARD_DATA, 4, _vp(self.w_nk_hi), _vp(self.w_nk_lo),
-                                 self.w_nk_hi.shape[0], self.K, stream), 'hd_pack_weight')
 
 
 class TransposedCopy(object):
@@ -72,56 +55,16 @@ class TransposedCopy(object):
                                      dst.shape[1], stream), 'hd_transpose_split')
 
 
-def repack_stale(packs, seen, param):
-    """Repack on the current stream every (name, pack) of `packs` whose parameter param(name) was changed in place (optimizer.step(),
-    copy_) since `seen` recorded its version counter, and record the new versions.  Returns the number of stale parameters."""
-    st = current_stream()
-    stale = {n for n, _ in packs if seen.get(n) != param(n)._version}
-    for n, pk in packs:
-        if n in stale:
-            pk.repack(st)
-    for n in stale:
-        seen[n] = param(n)._version
-    return len(stale)
-
-
-def _tf32_gemm(a, M, K, a_ld, b, out, out_ld, res=None, T=1, KH=1, pad=0, stream=None, one_pass=False):
-    """out[M', Cout] = (implicit conv of) a . B on the 3xTF32 tensor-core kernel (one_pass: 1xTF32, B's head alone).  b: a
-    BackwardDataPack or an operand tuple (hi, lo, tmap_hi, tmap_lo, Cout) from _bt_operand.  T / KH / pad > 1: a KH x 1 conv over T of
-    M = B clips."""
-    d = ConvDesc()
-    d.in_, d.in_ld = a.data_ptr(), a_ld
-    d.n_img, d.H, d.W, d.Cin = M, T, 1, K
-    d.Ho, d.Wo, d.KH, d.KW, d.stride, d.pad_t, d.pad_l = T, 1, KH, 1, 1, pad, 0
-    if isinstance(b, BackwardDataPack):
-        hi, lo, th, tl, Cout = b.w_nk_hi, b.w_nk_lo, b.tmap_hi, b.tmap_lo, b.Cout
-    else:
-        hi, lo, th, tl, Cout = b
-    d.w_kn = hi.data_ptr()
-    d.w_nk_hi = hi.data_ptr()
-    d.Cout, d.K_pad = Cout, KH * K
-    if res is not None:
-        d.res, d.res_ld, d.res_H, d.res_W, d.res_stride = res.data_ptr(), out_ld, T, 1, 1
-    d.out, d.out_ld = out.data_ptr(), out_ld
-    d.tmap_hi = C.cast(th, C.c_void_p)
-    if one_pass:
-        d.impl = _lib.HD_IMPL_TC_1XTF32
-    else:
-        d.impl = _lib.HD_IMPL_TC_3XTF32
-        d.w_nk_lo, d.tmap_lo = lo.data_ptr(), C.cast(tl, C.c_void_p)
-    check(lib.hd_conv_gemm(C.byref(d), current_stream() if stream is None else stream),
-          'hd_conv_gemm (backward, %s)' % ('1xTF32' if one_pass else '3xTF32'))
-
-
 def _bt_operand(pieces, cols, k_pad, st, one_pass=False):
-    """B operand of a weight-gradient GEMM: the row blocks `pieces` = [(x, rows, ld)] of an upstream gradient stacked along K,
-    transposed and TF32-split into [roundup64(cols), k_pad] (zero past the real rows / columns).  one_pass: the round-to-nearest TF32
-    head alone (lo and its map are None)."""
+    """B operand of a weight-gradient GEMM, with a BackwardDataPack's fields for dgrad_op: the row blocks `pieces` = [(x, rows, ld)]
+    of an upstream gradient stacked along K, transposed and TF32-split into w_nk_hi / w_nk_lo [roundup64(cols), k_pad] (zero past the
+    real rows / columns).  one_pass: the round-to-nearest TF32 head alone (w_nk_lo and tmap_lo are None)."""
     rows = _round(cols, 64)
     hi = torch.empty((rows, k_pad), dtype=F32, device=pieces[0][0].device)
     lo = None if one_pass else torch.empty_like(hi)
     _stack_t(pieces, cols, k_pad, 1, hi, lo, rows, st)
-    return (hi, lo, weight_tmap(hi), None if one_pass else weight_tmap(lo), cols), (hi, lo)
+    return types.SimpleNamespace(w_nk_hi=hi, w_nk_lo=lo, tmap_hi=weight_tmap(hi), tmap_lo=None if one_pass else weight_tmap(lo),
+                                 Cout=cols, K=k_pad)
 
 
 def _stack_t(pieces, cols, k_pad, mode, hi, lo, out_rows, st):
@@ -146,8 +89,7 @@ def _col_sum(x, rows, cols, ld, out, st):
 
 def _wgrad(xt, M, k_pad, g_pieces, cols, out, st, one_pass=False):
     """out[M, cols] = xt . (stacked g) : the weight gradient, 3xTF32 (one_pass: 1xTF32)."""
-    op, _keep = _bt_operand(g_pieces, cols, k_pad, st, one_pass)
-    _tf32_gemm(xt, M, k_pad, k_pad, op, out, cols, stream=st, one_pass=one_pass)
+    dgrad_op(_bt_operand(g_pieces, cols, k_pad, st, one_pass), xt, M, 1, 1, 1, 1, out, one_pass=one_pass).run(st)
 
 
 # ------------------------------------------------------------------------------------------------------------------------------------
@@ -216,7 +158,7 @@ def fmovie_backward(model, saved, g):
             db = torch.empty(Cc, dtype=F32, device=dev)
             _col_sum(gin, BT, Cc, Cc, db, st)
             # d relu(gn(src)) = conv(gin, W'); then the GroupNorm + ReLU backward (+ the block's residual gradient for gn1)
-            _tf32_gemm(gin, B, Cc, Cc, model.fm_bwd[i][k - 1], dact, Cc, T=T, KH=3, pad=1, stream=st, one_pass=model.one_pass)
+            dgrad_op(model.fm_bwd[i][k - 1], gin, B, T, 1, 3, 1, dact, one_pass=model.one_pass).run(st)
             check(lib.hd_groupnorm_relu_backward(fptr(src), fptr(gam), fptr(bet), fptr(dact), fptr(addend) if addend is not None else None,
                                                  fptr(gout), fptr(pg), fptr(pb), B, T, Cc, GN_GROUPS, GN_EPS, 1, st),
                   'hd_groupnorm_relu_backward')
@@ -272,7 +214,7 @@ def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st):
             G[2].copy_(torch.as_strided(g, (N, d), (g_ld, 1)))
         # dpre2 = (g . W3^T) * (h2 > 0);  dpre1 = (dpre2 . W2^T) * (h1 > 0);  dprev = g + dpre1 . W1theta^T
         check(lib.hd_fc_small_dgrad(fptr(gs), gld, fptr(head['W3t']), 1024, d, fptr(h2[s]), fptr(DP2[s]), N, st), 'hd_fc_small_dgrad')
-        _tf32_gemm(DP2[s], N, 1024, 1024, head['fc2_bwd'], DP1[s], 1024, stream=st, one_pass=model.one_pass)
+        dgrad_op(head['fc2_bwd'], DP2[s], N, 1, 1, 1, 1, DP1[s], one_pass=model.one_pass).run(st)
         check(lib.hd_relu_backward(fptr(h1[s]), fptr(DP1[s]), fptr(DP1[s]), N * 1024, st), 'hd_relu_backward')
         dst = G[s - 1] if s > 0 else dstart
         check(lib.hd_ief_fc3(fptr(DP1[s]), fptr(head['W1tT']), fptr(model._zeros), fptr(gs), gld, fptr(dst), d, N, 1024, d, st),
@@ -294,8 +236,31 @@ def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st):
     _wgrad(_xt([(h1.view(3 * N, 1024), 3 * N, 1024)], 1024, kp3, st), 1024, kp3, [(DP2.view(3 * N, 1024), 3 * N, 1024)], 1024, W2, st, op)
     _wgrad(_xt([(h2.view(3 * N, 1024), 3 * N, 1024)], 1024, kp3, st), 1024, kp3, [(G.view(3 * N, d), 3 * N, d)], d, W3, st, op)
     out = torch.empty((N, feat), dtype=F32, device=dev) if dphi is None else dphi
-    _tf32_gemm(dP, N, 1024, 1024, head['fc1_bwd'], out, feat, res=dphi, stream=st, one_pass=op)
+    dgrad_op(head['fc1_bwd'], dP, N, 1, 1, 1, 1, out, res=dphi, one_pass=op).run(st)
     return dstart, [W1, b1, W2, b2, W3, b3], out
+
+
+def regress_forward(model, keys, tiled, phi, start):
+    """call_hmr_ief over phi (N,2048) from start (N,85), or the tiled (1,85) when `tiled`: the main head, then the delta heads `keys`
+    from its pose.  Returns ((theta, deltas...), saved) with saved = [the main head's start (N,85), then per head h1, h2 and the
+    outputs of stages 0 and 1]."""
+    N = phi.shape[0]
+    st = current_stream()
+    dev = phi.device
+    phi_split = (torch.empty((N, 2048), dtype=torch.float16, device=dev), torch.empty((N, 2048), dtype=torch.float16, device=dev))
+    check(lib.hd_split_f16(fptr(phi), _vp(phi_split[0]), _vp(phi_split[1]), phi.numel(), st), 'hd_split_f16')
+    s0 = start.expand(N, 85).contiguous() if tiled else start
+    theta = torch.empty((N, 85), dtype=F32, device=dev)
+    saved = [s0] + list(ief_head_forward(model, model.ief['main'], phi_split, N, s0, 85, theta, 85, st))
+    outs = [theta]
+    for k in keys:
+        o = torch.empty((N, 85), dtype=F32, device=dev)
+        check(lib.hd_ief_delta_init(fptr(theta), fptr(o), 85, N, st), 'hd_ief_delta_init')
+        pose = torch.as_strided(theta, (N, 72), (85, 1), theta.storage_offset() + 3)
+        saved += ief_head_forward(model, model.ief[k], phi_split, N, pose, 85, torch.as_strided(o, (N, 72), (85, 1), o.storage_offset() + 3),
+                                  85, st)
+        outs.append(o)
+    return tuple(outs), saved
 
 
 # ------------------------------------------------------------------------------------------------------------------------------------
@@ -326,13 +291,13 @@ def hal_backward(model, x, h1, h2, g):
         _col_sum(gin, N, 2048, 2048, b, st)
         grads = [W, b] + grads
         if name == 'fc3':
-            _tf32_gemm(g, N, 2048, 2048, L['fc3_bwd'], dh2, 2048, stream=st, one_pass=model.one_pass)
+            dgrad_op(L['fc3_bwd'], g, N, 1, 1, 1, 1, dh2, one_pass=model.one_pass).run(st)
             check(lib.hd_relu_backward(fptr(h2), fptr(dh2), fptr(dh2), N * 2048, st), 'hd_relu_backward')
         elif name == 'fc2':
-            _tf32_gemm(dh2, N, 2048, 2048, L['fc2_bwd'], dh1, 2048, stream=st, one_pass=model.one_pass)
+            dgrad_op(L['fc2_bwd'], dh2, N, 1, 1, 1, 1, dh1, one_pass=model.one_pass).run(st)
             check(lib.hd_relu_backward(fptr(h1), fptr(dh1), fptr(dh1), N * 2048, st), 'hd_relu_backward')
         else:
-            _tf32_gemm(dh1, N, 2048, 2048, L['fc1_bwd'], dx, 2048, res=g, stream=st, one_pass=model.one_pass)
+            dgrad_op(L['fc1_bwd'], dh1, N, 1, 1, 1, 1, dx, res=g, one_pass=model.one_pass).run(st)
     return dx, grads
 
 
@@ -352,7 +317,7 @@ class FMovieFunction(torch.autograd.Function):
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        ctx.model._ensure_bwd()
+        ctx.model.sync_bwd_packs()
         t = ctx.saved_tensors
         dx, grads = fmovie_backward(ctx.model, [(t[2 * i], t[2 * i + 1]) for i in range(len(t) // 2)], g)
         return (None, dx) + tuple(t for blk in grads for t in blk)
@@ -365,36 +330,21 @@ class RegressFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, keys, tiled, phi, start, *params):
-        N = phi.shape[0]
-        st = current_stream()
-        dev = phi.device
-        phi_split = (torch.empty((N, 2048), dtype=torch.float16, device=dev), torch.empty((N, 2048), dtype=torch.float16, device=dev))
-        check(lib.hd_split_f16(fptr(phi), _vp(phi_split[0]), _vp(phi_split[1]), phi.numel(), st), 'hd_split_f16')
-        s0 = start.expand(N, 85).contiguous() if tiled else start
-        theta = torch.empty((N, 85), dtype=F32, device=dev)
-        saved = list(ief_head_forward(model, model.ief['main'], phi_split, N, s0, 85, theta, 85, st))
-        outs = [theta]
-        for k in keys:
-            o = torch.empty((N, 85), dtype=F32, device=dev)
-            check(lib.hd_ief_delta_init(fptr(theta), fptr(o), 85, N, st), 'hd_ief_delta_init')
-            pose = torch.as_strided(theta, (N, 72), (85, 1), theta.storage_offset() + 3)
-            saved += ief_head_forward(model, model.ief[k], phi_split, N, pose, 85, torch.as_strided(o, (N, 72), (85, 1), o.storage_offset() + 3),
-                                      85, st)
-            outs.append(o)
+        outs, saved = regress_forward(model, keys, tiled, phi, start)
         # Everything the backward reads goes through save_for_backward (theta, an output, included): no tensor or view of one is held on
         # ctx, so an unused graph is freed with its outputs and retain_graph works.  The delta heads' start is theta's pose, rebuilt there.
         ctx.model, ctx.keys, ctx.tiled = model, keys, tiled
-        ctx.save_for_backward(phi, s0, theta, *saved)
+        ctx.save_for_backward(phi, outs[0], *saved)
         ctx.set_materialize_grads(False)
-        return tuple(outs)
+        return outs
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dtheta, *ddeltas):
         model, keys = ctx.model, ctx.keys
-        model._ensure_bwd()
+        model.sync_bwd_packs()
         t = ctx.saved_tensors
-        phi, s0, theta = t[:3]
+        phi, theta, s0 = t[:3]
         N = phi.shape[0]
         pose = torch.as_strided(theta, (N, 72), (85, 1), theta.storage_offset() + 3)
         heads = [t[3 + 4 * j:7 + 4 * j] for j in range(1 + len(keys))]
@@ -440,7 +390,7 @@ class HalFunction(torch.autograd.Function):
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        ctx.model._ensure_bwd()
+        ctx.model.sync_bwd_packs()
         x, h1, h2 = ctx.saved_tensors
         dx, grads = hal_backward(ctx.model, x, h1, h2, g.contiguous())
         return (None, dx) + tuple(grads)
@@ -483,7 +433,50 @@ def trainable_names(w, num_conv_layers=3, delta_t_values=(-5, 5)):
     return names
 
 
-class TemporalModel(nn.Module):
+class TrainableModule(nn.Module):
+    """fp32 parameters addressable by TF variable name (`param(name)`), and the device packs that read them in place, as (name, pack)
+    pairs: `_fwd_packs` are written by their constructors, `_bwd_packs` by the first backward.  A pack is rewritten on the current
+    stream when its parameter was changed in place (optimizer.step(), copy_), detected by the parameter's version counter."""
+
+    def __init__(self):
+        super().__init__()
+        self._params = nn.ParameterDict()
+        self._fwd_packs, self._bwd_packs = [], []
+        self._seen, self._bwd_seen = {}, {}
+
+    def param(self, name):
+        return self._params[name]
+
+    def _packs_written(self, device):
+        """Wait for the packing the constructors of `_fwd_packs` queued on `device`, and record their parameters' versions: from here on
+        only what changes is repacked."""
+        sync_packing(device)
+        self._seen = {n: self.param(n)._version for n, _ in self._fwd_packs}
+
+    def _repack(self, packs, seen):
+        st = current_stream()
+        stale = {n for n, _ in packs if seen.get(n) != self.param(n)._version}
+        for n, pk in packs:
+            if n in stale:
+                pk.repack(st)
+        for n in stale:
+            seen[n] = self.param(n)._version
+        return len(stale)
+
+    def sync_packs(self):
+        """Repack every forward weight whose parameter changed since it was last packed (called by each forward).  Returns the count."""
+        return self._repack(self._fwd_packs, self._seen)
+
+    def sync_bwd_packs(self):
+        """The same for the backward packs (called by each backward; the first one writes them all).  Returns the count."""
+        return self._repack(self._bwd_packs, self._bwd_seen)
+
+    def _grad_on(self, names, *inputs):
+        """Whether a forward goes on the autograd graph: grad mode is on and an input or a parameter of `names` requires grad."""
+        return torch.is_grad_enabled() and (any(x.requires_grad for x in inputs) or any(self.param(n).requires_grad for n in names))
+
+
+class TemporalModel(TrainableModule):
     """The trainable part of HMMR (f_movie, the IEF heads, mean_param, fc2_res) as fp32 parameters on one CUDA device.
 
     Parameters are addressable by their TF variable names (`model.param('single_view_ief/3D_module/fc2/weights')`); `parameters()`
@@ -515,7 +508,6 @@ class TemporalModel(nn.Module):
         self.num_conv_layers = int(self.config.num_conv_layers)
         self.delta_keys = sorted(int(d) for d in self.config.delta_t_values if int(d) != 0)
         self.names = trainable_names(w, self.num_conv_layers, self.delta_keys)
-        self._params = nn.ParameterDict()
         for n in self.names:
             a = np.asarray(w[n], np.float32)
             if n == 'mean_param':
@@ -523,15 +515,11 @@ class TemporalModel(nn.Module):
             self._params[n] = nn.Parameter(torch.from_numpy(np.ascontiguousarray(a)).to(self.device))
         with torch.cuda.device(self.device):
             self._build()
-        self._bwd_seen = {}
 
     # ---------------------------------------------------------------- packing
-    def param(self, name):
-        return self._params[name]
-
     def _build(self):
         P = self.param
-        self.fm_blocks, self.fm_bwd, self._fwd_packs, self._bwd_packs = [], [], [], []
+        self.fm_blocks, self.fm_bwd = [], []
         self.has_fmovie = 'AZ_FC_block2_conv1block_0/weights' in self.names
         Cc = 2048
         if self.has_fmovie:
@@ -574,19 +562,7 @@ class TemporalModel(nn.Module):
                 self.hal['fc%d_bwd' % i] = BackwardDataPack(P(wn).data, 1, 2048, 2048)
                 self._fwd_packs.append((wn, self.hal['fc%d' % i]))
                 self._bwd_packs.append((wn, self.hal['fc%d_bwd' % i]))
-        # the forward packs were written by their constructors: complete them, and repack only what changes from here on
-        sync_packing(self.device)
-        self._seen = {n: self.param(n)._version for n, _ in self._fwd_packs}
-
-    def _repack(self, packs, seen):
-        return repack_stale(packs, seen, self.param)
-
-    def sync_packs(self):
-        """Repack every forward weight whose parameter changed since it was last packed (called by each forward).  Returns the count."""
-        return self._repack(self._fwd_packs, self._seen)
-
-    def _ensure_bwd(self):
-        return self._repack(self._bwd_packs, self._bwd_seen)
+        self._packs_written(self.device)
 
     # ---------------------------------------------------------------- forward API
     def _check_input(self, x, name, last=2048):
@@ -597,9 +573,6 @@ class TemporalModel(nn.Module):
         if x.device != self.device:
             raise _lib.HDError('%s: tensor is on %s, the model on %s' % (name, x.device, self.device))
 
-    def _grad_on(self, x, names):
-        return torch.is_grad_enabled() and (x.requires_grad or any(self.param(n).requires_grad for n in names))
-
     def temporal_encode(self, phi):
         """az_fc2_groupnorm ("f_movie"): (B,T,2048) -> (B,T,2048)."""
         self._check_input(phi, 'temporal_encode')
@@ -608,7 +581,7 @@ class TemporalModel(nn.Module):
         self.sync_packs()
         phi = phi.contiguous()
         names = [n for i in range(self.num_conv_layers) for n in fmovie_names(i)]
-        if self._grad_on(phi, names):
+        if self._grad_on(names, phi):
             return FMovieFunction.apply(self, phi, *[self.param(n) for n in names])
         with torch.no_grad():
             return fmovie_forward(self, phi.detach(), False)[0]
@@ -620,7 +593,7 @@ class TemporalModel(nn.Module):
             raise _lib.HDError('no fc2_res weights were loaded')
         self.sync_packs()
         x = phi.contiguous().reshape(-1, 2048)
-        if self._grad_on(x, HAL_NAMES):
+        if self._grad_on(HAL_NAMES, x):
             return HalFunction.apply(self, x, *[self.param(n) for n in HAL_NAMES]).view(phi.shape)
         with torch.no_grad():
             return hal_forward(self, x.detach())[0].view(phi.shape)
@@ -641,12 +614,11 @@ class TemporalModel(nn.Module):
             self._check_input(start, 'regress(omega_start)', 85)
             start = start.contiguous()
         names = [n for dt in (0,) + keys for n in ief_names(dt)]
-        params = [self.param(n) for n in names]
-        if self._grad_on(feats, names + ['mean_param']) or start.requires_grad and torch.is_grad_enabled():
-            outs = RegressFunction.apply(self, keys, tiled, feats, start, *params)
+        if self._grad_on(names + ['mean_param'], feats, start):
+            outs = RegressFunction.apply(self, keys, tiled, feats, start, *[self.param(n) for n in names])
         else:
             with torch.no_grad():
-                outs = RegressFunction.forward(_NoCtx(), self, keys, tiled, feats.detach(), start.detach(), *params)
+                outs = regress_forward(self, keys, tiled, feats.detach(), start.detach())[0]
         return outs[0], {k: outs[1 + i] for i, k in enumerate(keys)}
 
     def predict_from_features(self, phi, smpl, single_frame=False):
@@ -701,14 +673,11 @@ class TemporalModel(nn.Module):
                         out['fm%d.gn%d' % (i, k)] = (a.t() > 0).reshape(B, T, 1, Cc).cpu()
             if feats is not None:
                 keys = tuple(self.delta_keys) if delta_keys is None else tuple(sorted(int(k) for k in delta_keys if int(k) != 0))
-                ctx = _NoCtx()
                 tiled = omega_start is None
                 start = self.param('mean_param') if tiled else omega_start.contiguous()
-                RegressFunction.forward(ctx, self, keys, tiled, feats.contiguous(), start.detach(),
-                                        *[self.param(n) for dt in (0,) + keys for n in ief_names(dt)])
-                t = ctx.saved_tensors
+                _, saved = regress_forward(self, keys, tiled, feats.contiguous(), start.detach())
                 for j, name in enumerate(['main'] + ['d%d' % k for k in keys]):
-                    h1, h2 = t[3 + 4 * j], t[4 + 4 * j]
+                    h1, h2 = saved[1 + 4 * j], saved[2 + 4 * j]
                     for s in range(3):
                         out['%s.s%d.fc1' % (name, s)] = (h1[s] > 0).cpu()
                         out['%s.s%d.fc2' % (name, s)] = (h2[s] > 0).cpu()
@@ -731,13 +700,3 @@ class TemporalModel(nn.Module):
         from .tf_checkpoint import save_checkpoint
         save_checkpoint(prefix, self.tf_variables())
         return prefix
-
-
-class _NoCtx(object):
-    """Stand-in ctx for running an autograd Function's forward without recording a graph."""
-
-    def save_for_backward(self, *a):
-        self.saved_tensors = a
-
-    def set_materialize_grads(self, v):
-        pass

@@ -24,8 +24,8 @@ from torch import nn
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from .nets import PackedResNet, ResNetBatchNorm, ResNetTrainPlan, RESNET_BLOCKS, grad_one_pass, sync_packing
-from .trainable import BackwardDataPack, repack_stale
+from .nets import BackwardDataPack, PackedResNet, ResNetBatchNorm, ResNetTrainPlan, RESNET_BLOCKS, grad_one_pass
+from .trainable import TrainableModule
 
 F32 = torch.float32
 
@@ -78,7 +78,7 @@ class ResNetFunction(torch.autograd.Function):
         return (None, None, None) + tuple(net.gradient_of(n, g) for n in net.names)
 
 
-class TrainableResNet(nn.Module):
+class TrainableResNet(TrainableModule):
     """The trunk's trainable variables as fp32 parameters on one CUDA device, addressable by TF name (`net.param(name)`), and the
     training-mode forward over them.  The batch-norm gamma / beta parameters share storage with `bn.gamma` / `bn.beta`, which the plans
     read in place; conv weights and biases are read in place by their packs and epilogues.  grad_precision: 'fp32' (3xTF32 weight and
@@ -99,7 +99,6 @@ class TrainableResNet(nn.Module):
         if missing:
             raise _lib.HDError('TrainableResNet: weights lack %d resnet_v2_50 variables, e.g. %s' % (len(missing), missing[0]))
         self._source = w
-        self._params = nn.ParameterDict()
         for n in cn:
             self._params[n] = nn.Parameter(torch.tensor(np.asarray(w[n], np.float32), device=self.device))      # a copy
         with torch.cuda.device(self.device) if self.device.type == 'cuda' else contextlib.nullcontext():
@@ -116,10 +115,9 @@ class TrainableResNet(nn.Module):
 
     def _build_packs(self):
         p, pk = self.packed, 'resnet_v2_50'
-        self._fwd_packs = [(pk + '/conv1/weights', p.conv1)]
+        self._fwd_packs.append((pk + '/conv1/weights', p.conv1))
         if p.conv1_planes is not None:
             self._fwd_packs.append((pk + '/conv1/weights', p.conv1_planes))
-        self._bwd_packs = []
         qs = [n[:-len('/conv1/weights')] for n in conv_names(self.blocks) if n.endswith('bottleneck_v2/conv1/weights')]
         for q, unit in zip(qs, p.units):
             for c in ('shortcut', 'conv1', 'conv2', 'conv3'):
@@ -129,19 +127,7 @@ class TrainableResNet(nn.Module):
                 conv.bwd = BackwardDataPack(self._params[name].data, conv.KH * conv.KW, conv.Cin, conv.Cout)
                 self._fwd_packs.append((name, conv))
                 self._bwd_packs.append((name, conv.bwd))
-        sync_packing(self.device)
-        self._seen = {n: self._params[n]._version for n, _ in self._fwd_packs}
-        self._bwd_seen = {}
-
-    def param(self, name):
-        return self._params[name]
-
-    def sync_packs(self):
-        """Repack every forward weight whose parameter changed since it was last packed.  Returns the count."""
-        return repack_stale(self._fwd_packs, self._seen, self.param)
-
-    def sync_bwd_packs(self):
-        return repack_stale(self._bwd_packs, self._bwd_seen, self.param)
+        self._packs_written(self.device)
 
     def plan(self, n, size):
         """The keep=True training plan for n frames of size x size (one batch shape at a time: it holds ~32 MB per frame at 224)."""
@@ -170,9 +156,8 @@ class TrainableResNet(nn.Module):
         self.sync_packs()
         plan = self.plan(n, S)
         images = images.detach().contiguous()
-        params = [self._params[k] for k in self.names]
-        if torch.is_grad_enabled() and any(q.requires_grad for q in params):
-            return ResNetFunction.apply(self, plan, images, *params), plan
+        if self._grad_on(self.names):
+            return ResNetFunction.apply(self, plan, images, *[self._params[k] for k in self.names]), plan
         phis = torch.empty((n, self.packed.out_dim), dtype=F32, device=self.device)
         with torch.no_grad():
             plan.run(images, phis)

@@ -173,10 +173,10 @@ def test_maxpool_backward_against_float64(H, W):
 
 
 @pytest.mark.parametrize('H,Cin,Cout,s', [(14, 64, 64, 2), (15, 128, 64, 2), (9, 64, 128, 1), (28, 256, 256, 1)])
-def test_conv3x3_data_gradient_against_float64(H, Cin, Cout, s):
+def test_dgrad_op_conv3x3_against_float64(H, Cin, Cout, s):
     """dX of a conv2d_same 3x3 through the 2-D backward-data pack (tap flip of the flattened (ky, kx)), stride 2 via zero insertion."""
     from human_dynamics_b200._lib import lib, check
-    from human_dynamics_b200.nets import PackedConv, _dgrad_op
+    from human_dynamics_b200.nets import PackedConv, dgrad_op
     from human_dynamics_b200.trainable import BackwardDataPack
     from oracle.nets_ref import conv2d_same
     rng = np.random.RandomState(H + Cin + s)
@@ -195,7 +195,7 @@ def test_conv3x3_data_gradient_against_float64(H, Cin, Cout, s):
     if s > 1:
         check(lib.hd_zero_insert(_vp(dyt), _vp(z), n, Ho, Ho, Cout, s, H, H, _st()), 'hd_zero_insert')
         src = z
-    _dgrad_op(conv, src, n, H, H, 3, out).run(_st())
+    dgrad_op(conv.bwd, src, n, H, H, 3, 3, out).run(_st())
     xt = torch.zeros((n, H, H, Cin), dtype=torch.float64, requires_grad=True)
     y = conv2d_same(xt, torch.from_numpy(w.astype(np.float64)), s)
     want, = torch.autograd.grad(y, xt, torch.from_numpy(dy.astype(np.float64)))

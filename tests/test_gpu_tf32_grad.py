@@ -148,9 +148,9 @@ def test_wgrad_ex_bad_impl_launches_nothing():
 # ------------------------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize('H,Cin,Cout,K,s', [(14, 64, 64, 3, 2), (15, 128, 64, 3, 2), (9, 64, 128, 3, 1), (28, 256, 256, 3, 1),
                                             (14, 256, 1024, 1, 1)])
-def test_data_gradient_1xtf32(H, Cin, Cout, K, s):
+def test_dgrad_op_1xtf32(H, Cin, Cout, K, s):
     from human_dynamics_b200._lib import lib, check
-    from human_dynamics_b200.nets import PackedConv, _dgrad_op
+    from human_dynamics_b200.nets import PackedConv, dgrad_op
     from human_dynamics_b200.trainable import BackwardDataPack
     from oracle.nets_ref import conv2d_same
     rng = np.random.RandomState(H + Cin + s + K)
@@ -168,7 +168,7 @@ def test_data_gradient_1xtf32(H, Cin, Cout, K, s):
         src = torch.empty((n, H, H, Cout), device='cuda')
         check(lib.hd_zero_insert(_vp(dyt), _vp(src), n, Ho, Ho, Cout, s, H, H, _st()), 'hd_zero_insert')
     out = torch.empty((n, H, H, Cin), device='cuda')
-    op = _dgrad_op(conv, src, n, H, H, K, out, one_pass=True)
+    op = dgrad_op(conv.bwd, src, n, H, H, K, K, out, one_pass=True)
     assert op.d.impl == 2 and not op.d.w_nk_lo and not op.d.tmap_lo
     op.run(_st())
 

@@ -81,7 +81,7 @@ def main():
     def repack():
         touch()
         model.sync_packs()
-        model._ensure_bwd()
+        model.sync_bwd_packs()
 
     res = {'tool': 'bench_temporal_grad', **card(), 'B': B, 'T': T, 'frames': N, 'params': n_params, 'bound': bound(B, T, n_params),
            'losses': {}}
