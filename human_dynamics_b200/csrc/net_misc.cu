@@ -323,13 +323,13 @@ __global__ void __launch_bounds__(256) ief_fc3_kernel(const float *__restrict__ 
 #pragma unroll
   for (int r = 0; r < 8; ++r) acc[r][0] = acc[r][1] = acc[r][2] = 0.f;
   const int kper = K / 8;
-  const bool c1 = lane + 32 < D, c2 = lane + 64 < D;
+  const bool c0 = lane < D, c1 = lane + 32 < D, c2 = lane + 64 < D;     // D < 32: no column of W past D is read
   for (int k0 = warp * kper; k0 < (warp + 1) * kper; k0 += 8) {       // (kper % 8 == 0 is required by the host entry)
     float w0[8], w1[8], w2[8];
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
       const float *wr = W + (size_t)(k0 + u) * D;
-      w0[u] = __ldg(wr + lane); w1[u] = c1 ? __ldg(wr + lane + 32) : 0.f; w2[u] = c2 ? __ldg(wr + lane + 64) : 0.f;
+      w0[u] = c0 ? __ldg(wr + lane) : 0.f; w1[u] = c1 ? __ldg(wr + lane + 32) : 0.f; w2[u] = c2 ? __ldg(wr + lane + 64) : 0.f;
     }
 #pragma unroll
     for (int u = 0; u < 8; ++u) {

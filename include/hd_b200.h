@@ -52,6 +52,9 @@ void hd_launch_count_reset(void);
  *   if res: v += res[(n*res_H + oy*res_stride)*res_W + ox*res_stride][co]
  *   if post_relu: v = max(v,0)
  *   out[(n*Ho+oy)*Wo+ox][co] = v          (out may be NULL when out_hi/out_lo are given, see below)
+ * In place (impl 1 and 2): `out` may be `res` when the residual is row-aligned with the output (res_stride 1, res_H == Ho,
+ * res_W == Wo, res_ld == out_ld).  Each element is read by the thread that writes it, before it writes it, so the result is
+ * bit-identical to the same call with a separate residual buffer (the backward's dX += dY . W^T accumulations rely on it).
  * ------------------------------------------------------------------------------------------ */
 /* impl 3 (3xFP16) is FP32-class: A_hi*B_hi + (A_lo*B_hi + A_hi*B_lo) per product.  impl 4 (1xFP16) is its half-precision
  * inference mode: A_hi*B_hi alone, one MMA per product, on the same formats -- w_nk_hi / tmap_hi (and tmap_hi_n64) are the heads of
