@@ -134,7 +134,6 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  const int xmode = p.dbg ? (int)p.dbg[15] : 0;      // timing experiments (hd_conv_gemm_profile only; results invalid)
 
   if (warp >= W_PROD) {
     // =============================== A producers (PROD_THREADS) ===============================
@@ -158,7 +157,6 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
       if (t != 0) return;
       const int n0 = (((int)blockIdx.x + ti * (int)gridDim.x) % tiles_n) * BN;
       const uint32_t b_hi = smem_base + s * C::STAGE_BYTES + C::B_OFFSET;
-      if (xmode & 2) { mbar_arrive(full_bar(s)); return; }
       // BN = 128: two 64-row boxes.  Weight rows are padded to 64, so the second box is either wholly inside the weights or
       // wholly past Cout; then it is not loaded, and the stale columns it would have filled only reach outputs c >= Cout,
       // which the epilogue never stores.
@@ -380,8 +378,8 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int iy = pf_rs.iy[i] + ky, ix = pf_rs.ix[i] + kx;
-        const bool ok = pf_rs.n[i] >= 0 && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
-        if (ok && !(xmode & 4)) {
+        const bool ok = pf_rs.n[i] >= 0 && (unsigned)iy < (unsigned)p.H && (unsigned)ix < (unsigned)p.W;
+        if (ok) {
           const float4 *src = reinterpret_cast<const float4 *>(p.in + ((size_t)((size_t)pf_rs.n[i] * p.H + iy) * p.W + ix) * p.in_ld + ci);
 #pragma unroll
           for (int v = 0; v < V; ++v) dst[i * V + v] = __ldg(src + v);
@@ -443,7 +441,6 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           for (int e = 0; e < 4; ++e) split_f16x2(xs[2 * e], xs[2 * e + 1], h[e], l[e]);
         }
         const uint32_t off = (uint32_t)(rb + 32 * i) * 128u + sw_off;
-        if (xmode & 1) continue;
         *reinterpret_cast<uint4 *>(a_hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
         if (SPLIT) *reinterpret_cast<uint4 *>(a_lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
       }

@@ -7,7 +7,6 @@ Weights come in as a dict of numpy arrays keyed by TF variable names (SURVEY.md 
 from __future__ import annotations
 
 import ctypes as C
-import os
 
 import numpy as np
 import torch
@@ -240,8 +239,6 @@ class PackedConv(object):
         else:
             d.impl = _lib.HD_IMPL_SIMT
         op = ConvOp(d, (self, inp, out, pre, res, inp_split, out_split, post2, post), (Ho, Wo))
-        if not TMA_EPILOGUE:
-            d.flags |= _lib.HD_CONV_NO_TMA_EPILOGUE
         op.encode_act_maps()
         return op
 
@@ -312,11 +309,6 @@ class SubsampleOp(object):
         check(lib.hd_subsample(fptr(self.src), fptr(self.dst), n, H, W, Cc, s, stream), 'hd_subsample')
 
 
-SUBSAMPLE_RES = os.environ.get('HD_SUBSAMPLE_RES', '1') != '0'    # A/B switch: strided identity shortcuts via hd_subsample + plain residual
-SUBSAMPLE_EPI = os.environ.get('HD_SUBSAMPLE_EPI', '1') != '0'    # A/B switch: the unit in front of a strided identity unit writes x[:, ::s, ::s] itself
-TMA_EPILOGUE = os.environ.get('HD_TMA_EPILOGUE', '1') != '0'     # 0: set HD_CONV_NO_TMA_EPILOGUE (results identical; refuses out_subsample)
-
-
 class ConvOp(object):
     __slots__ = ('d', 'keep', 'out_hw', 'ref', 'dyn', 'maps')
 
@@ -361,11 +353,6 @@ class ConvOp(object):
         rc = lib.hd_conv_gemm(self.ref, stream)
         if rc:
             check(rc, 'hd_conv_gemm')
-
-
-DROP_DEAD_FP32 = os.environ.get('HD_DROP_DEAD_FP32', '1') != '0'   # A/B switch: skip fp32 block outputs nobody reads
-FAST_HEADS = os.environ.get('HD_FAST_HEADS', '1') != '0'          # A/B switch: f_movie / IEF through the pre-split + small-GEMM kernels
-CONV1_PLANES = os.environ.get('HD_CONV1_PLANES', '1') != '0'      # A/B switch: conv1 from padded fp16 planes vs fp32 row-segment gather
 
 
 class PackedConv1Planes(object):
@@ -423,7 +410,7 @@ class PackedConv1Planes(object):
         d.w_nk_hi, d.tmap_hi = self.w_nk_hi.data_ptr(), C.cast(self.tmap_hi, C.c_void_p)
         if not heads:
             d.w_nk_lo, d.tmap_lo = self.w_nk_lo.data_ptr(), C.cast(self.tmap_lo, C.c_void_p)
-        d.flags = _lib.HD_CONV_INPUT_PLANES | (0 if TMA_EPILOGUE else _lib.HD_CONV_NO_TMA_EPILOGUE)
+        d.flags = _lib.HD_CONV_INPUT_PLANES
         op = ConvOp(d, (self, planes, out), (size // 2, size // 2))
         op.encode_act_maps()
         return op
@@ -469,6 +456,35 @@ class PackedResNet(object):
         self.post = (_dev(s, device), _dev(b, device))
         self.out_dim = d_in
         sync_packing(device)
+
+
+def bind_root_conv1(packed: PackedResNet, n, size, impl, out):
+    """The root conv1 of a trunk plan writing `out` (the plan's root_buf) -> (planes, op): in the fp16 impls at an even size, the
+    padded fp16 planes and their PackedConv1Planes op; else, when conv1 has a tensor-core packing and impl is not 'simt', (None, the
+    row-segment gather op, the only tensor-core conv1 at odd sizes; its `in_` is set per run); else (None, None): hd_conv1_7x7s2."""
+    if packed.conv1_planes is not None and impl in F16_IMPLS and size % 2 == 0:
+        planes = packed.conv1_planes.alloc_planes(n, size, impl)
+        return planes, packed.conv1_planes.bind(planes, n, size, out, impl)
+    if packed.conv1.tc and impl != 'simt':
+        return None, packed.conv1.bind(out, n, size, size, out, in_ld=3, impl=impl)
+    return None, None
+
+
+def run_root_conv1(plan, images, st):
+    """Run the root conv1 that bind_root_conv1 gave `plan` (its planes, conv1_op, root_buf) over images (n,size,size,3) contiguous
+    float32; images None: the planes were filled by the caller (uint8 frames through hd_process_image)."""
+    n, size = plan.n, plan.size
+    if plan.planes is not None:
+        if images is not None:
+            check(lib.hd_pack_conv1_planes(fptr(images), _vp(plan.planes[0]), _vp(plan.planes[1]), n, size, size,
+                                           plan.planes[0].shape[2], st), 'hd_pack_conv1_planes')
+        plan.conv1_op.run(st)
+    elif plan.conv1_op is not None:
+        plan.conv1_op.d.in_ = images.data_ptr()
+        plan.conv1_op.run(st)
+    else:
+        check(lib.hd_conv1_7x7s2(fptr(images), fptr(plan.p.conv1_w), fptr(plan.p.conv1_b), fptr(plan.root_buf), n, size, size, st),
+              'hd_conv1_7x7s2')
 
 
 class ResNetPlan(object):
@@ -518,13 +534,8 @@ class ResNetPlan(object):
         self.bufB = torch.empty(n * mx_io, **f32)
         self.bufS = torch.empty(n * mx_io, **f32)
         self.ops = []
-        self.conv1_op = None
-        self.planes = None
-        if root and packed.conv1_planes is not None and impl in F16_IMPLS and CONV1_PLANES and size % 2 == 0:
-            self.planes = packed.conv1_planes.alloc_planes(n, size, impl)
-            self.conv1_op = packed.conv1_planes.bind(self.planes, n, size, self.bufS, impl)
-        elif root and packed.conv1.tc and impl != 'simt':
-            self.conv1_op = packed.conv1.bind(self.bufS, n, size, size, self.bufS, in_ld=3, impl=impl)   # `in_` is set per run
+        self.root_buf = self.bufS             # conv1 output, read by pool1
+        self.planes, self.conv1_op = bind_root_conv1(packed, n, size, impl, self.root_buf) if root else (None, None)
         self.in_refs = []                     # (op, field) descriptor fields that read the stage input
         self.pool_split = None
         self.pool_f32_dead = False
@@ -538,7 +549,7 @@ class ResNetPlan(object):
             self.in_split = xs
             if root:
                 self.pool_split = (units[0]['pre'][0], units[0]['pre'][1], xs)
-                self.pool_f32_dead = DROP_DEAD_FP32 and 'shortcut' in units[0]
+                self.pool_f32_dead = 'shortcut' in units[0]
             self.out_split = None
             sub_ready = False                 # bufS already holds x[:, ::s, ::s] of this unit's input (written by the previous conv3)
             for ui, unit in enumerate(units):
@@ -549,7 +560,7 @@ class ResNetPlan(object):
                     if ui == 0:
                         self.in_refs += self._split_refs(self.ops[-1])
                     res, res_geom = self.bufS, (unit['depth'], Ho, Ho, 1)
-                elif s > 1 and SUBSAMPLE_RES:
+                elif s > 1:
                     # strided identity shortcut: a dense subsampled copy so conv3's residual is row-aligned (TMA slab loads) -- written by
                     # the previous unit's conv3 epilogue when that unit is in this plan, else by one hd_subsample pass
                     if not sub_ready:
@@ -558,7 +569,7 @@ class ResNetPlan(object):
                             self.in_refs.append((self.ops[-1], 'res', 2))
                     res, res_geom = self.bufS, (unit['depth'], Ho, Ho, 1)
                 else:
-                    res, res_geom = x, (unit['depth'], H, H, s)
+                    res, res_geom = x, (unit['depth'], H, H, 1)
                 self.ops.append(unit['conv1'].bind(None, n, H, H, None, inp_split=xs, out_split=r1, impl=impl))
                 if ui == 0:
                     self.in_refs += self._split_refs(self.ops[-1])
@@ -569,18 +580,17 @@ class ResNetPlan(object):
                 # the fp32 block output only feeds an IDENTITY shortcut: when the next unit changes depth (first unit of a block) its
                 # shortcut is a conv of the pre-activation, and the fp32 copy would be written for nobody
                 nxt_conv_shortcut = ('shortcut' in units[ui + 1]) if not last else bool(next_has_shortcut)
-                y_out = None if (osplit is not None and nxt_conv_shortcut and DROP_DEAD_FP32) else y
+                y_out = None if nxt_conv_shortcut else y
                 # the next unit is a strided identity unit: the only reader of this unit's fp32 output is that shortcut, x[:, ::s, ::s]
                 # -- write just those pixels, densely, into bufS (free here: this unit's own residual is not in bufS)
                 s_next = units[ui + 1]['stride'] if not last else 1
-                sub_ready = bool(SUBSAMPLE_EPI and SUBSAMPLE_RES and not last and s_next > 1 and 'shortcut' not in units[ui + 1] and
-                                 'shortcut' not in unit and s == 1 and y_out is not None and osplit is not None)
+                sub_ready = not last and s_next > 1 and not nxt_conv_shortcut and 'shortcut' not in unit and s == 1
                 if sub_ready:
                     y_out = self.bufS
                 self.ops.append(unit['conv3'].bind(None, n, Ho, Ho, y_out, inp_split=r2, res=res, res_geom=res_geom, impl=impl,
                                                    out_split=osplit, post2=(nxt[0], nxt[1], 1) if nxt is not None else None,
                                                    out_subsample=s_next if sub_ready else 0))
-                if ui == 0 and 'shortcut' not in unit and not (s > 1 and SUBSAMPLE_RES):
+                if ui == 0 and 'shortcut' not in unit and s == 1:
                     self.in_refs.append((self.ops[-1], 'res', 2))
                 if last:
                     self.out_split = osplit
@@ -653,19 +663,9 @@ class ResNetPlan(object):
         st = current_stream() if stream is None else stream
         n, p = self.n, self.p
         if self.root:
-            if self.planes is not None:
-                if images is not None:        # None: the planes were filled by the caller (uint8 frames through hd_process_image_planes)
-                    check(lib.hd_pack_conv1_planes(fptr(images), _vp(self.planes[0]), _vp(self.planes[1]),
-                                                   n, self.size, self.size, self.planes[0].shape[2], st), 'hd_pack_conv1_planes')
-                self.conv1_op.run(st)
-            elif self.conv1_op is not None:
-                self.conv1_op.d.in_ = images.data_ptr()
-                self.conv1_op.run(st)
-            else:
-                check(lib.hd_conv1_7x7s2(fptr(images), fptr(p.conv1_w), fptr(p.conv1_b), fptr(self.bufS), n, self.size, self.size, st),
-                      'hd_conv1_7x7s2')
+            run_root_conv1(self, images, st)
             ps = self.pool_split
-            check(lib.hd_maxpool3x3s2_same(fptr(self.bufS), None if self.pool_f32_dead else fptr(self.bufA), n, self.H1, self.H1, 64,
+            check(lib.hd_maxpool3x3s2_same(fptr(self.root_buf), None if self.pool_f32_dead else fptr(self.bufA), n, self.H1, self.H1, 64,
                                            fptr(ps[0]) if ps else None, fptr(ps[1]) if ps else None,
                                            _vp(ps[2][0]) if ps else None, _vp(ps[2][1]) if ps else None, st), 'hd_maxpool3x3s2_same')
         for op in self.ops:
@@ -797,17 +797,10 @@ class ResNetTrainPlan(object):
         else:
             self.bufA, self.bufB, self.bufS = (torch.empty(n * mx_io, **f32) for _ in range(3))
             self.bufR1, self.bufR2 = torch.empty(n * mx_r, **f32), torch.empty(n * mx_r, **f32)
-        root_out = self.root_out if self.keep else self.bufS
+        self.root_buf = self.root_out if self.keep else self.bufS
         L = bn.offsets[-1]
         self.scale, self.shift, self.mean, self.var = (torch.empty(L, **f32) for _ in range(4))
-        self.planes = None
-        self.conv1_op = None
-        if packed.conv1_planes is not None and impl in ('auto', 'tc3h') and CONV1_PLANES and size % 2 == 0:
-            self.planes = packed.conv1_planes.alloc_planes(n, size)
-            self.conv1_op = packed.conv1_planes.bind(self.planes, n, size, root_out)
-        elif packed.conv1.tc and impl != 'simt':
-            self.conv1_op = packed.conv1.bind(root_out, n, size, size, root_out, in_ld=3, impl=impl)
-        self.root_buf = root_out
+        self.planes, self.conv1_op = bind_root_conv1(packed, n, size, impl, self.root_buf)
         self.ops, self.stats = [], []
         shapes = []                           # (map, rows, C) of every normalised map, in scope order
         h = H2
@@ -859,17 +852,7 @@ class ResNetTrainPlan(object):
         (n,2048) float32 view: the phis with batch statistics.  The moving statistics are not touched."""
         st = current_stream() if stream is None else stream
         n, p = self.n, self.p
-        if self.planes is not None:
-            if images is not None:
-                check(lib.hd_pack_conv1_planes(fptr(images), C.c_void_p(self.planes[0].data_ptr()), C.c_void_p(self.planes[1].data_ptr()),
-                                               n, self.size, self.size, self.planes[0].shape[2], st), 'hd_pack_conv1_planes')
-            self.conv1_op.run(st)
-        elif self.conv1_op is not None:
-            self.conv1_op.d.in_ = images.data_ptr()
-            self.conv1_op.run(st)
-        else:
-            check(lib.hd_conv1_7x7s2(fptr(images), fptr(p.conv1_w), fptr(p.conv1_b), fptr(self.root_buf), n, self.size, self.size, st),
-                  'hd_conv1_7x7s2')
+        run_root_conv1(self, images, st)
         check(lib.hd_maxpool3x3s2_same(fptr(self.root_buf), fptr(self.pool_out), n, self.H1, self.H1, 64, None, None, None, None, st),
               'hd_maxpool3x3s2_same')
         self.generation += 1
@@ -1078,7 +1061,7 @@ class FMoviePlan(object):
 
     def _bind(self, x):
         if self.impl in F16_IMPLS and self.p.blocks and all(b[k].tc == 'f16' for b in self.p.blocks for k in ('conv1', 'conv2')) \
-                and self.T * (self.p.C // GN_GROUPS) <= 1280 and FAST_HEADS:
+                and self.T * (self.p.C // GN_GROUPS) <= 1280:
             return self._bind_fast(x)
         steps = []
         cur = x
@@ -1167,7 +1150,7 @@ class IEFPlan(object):
         self.impl = impl
         self._bound_for = None
         heads = [packed.main] + [packed.deltas[k] for k in self.delta_keys]
-        self.fast = FAST_HEADS and impl in F16_IMPLS and all(h.fc1_phi.tc == 'f16' and h.fc2.tc == 'f16' for h in heads)
+        self.fast = impl in F16_IMPLS and all(h.fc1_phi.tc == 'f16' and h.fc2.tc == 'f16' for h in heads)
         if self.fast:
             self.phi_split = f16_pair((N, heads[0].feat), dev, impl)
             self.h1_split = f16_pair((N, 1024), dev, impl)

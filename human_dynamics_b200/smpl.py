@@ -6,7 +6,6 @@ reference-named class lives in src/tf_smpl/batch_smpl.py and delegates here.
 from __future__ import annotations
 
 import ctypes as C
-import os
 import pickle
 
 import numpy as np
@@ -163,8 +162,8 @@ class SMPLConstants(object):
             w_hi = wd.astype(np.float16)
             self.w_hi = torch.from_numpy(w_hi).to(dev)
             self.w_lo = torch.from_numpy((wd - w_hi.astype(np.float32)).astype(np.float16)).to(dev)
-        self.lbs_tc = bool(tc) and os.environ.get('HD_LBS_TC', '1') != '0' and (V * 3 * 4) % 8 == 0
-        self.lbs_tc_min_batch = int(os.environ.get('HD_LBS_TC_MIN', '2112'))         # 132 SMs x 16 poses
+        self.lbs_tc = bool(tc) and (V * 3 * 4) % 8 == 0
+        self.lbs_tc_min_batch = 2112                       # 132 SMs x 16 poses
         # host copies for the backward's extra arrays, packed and uploaded on the first backward call (grad_state)
         self._grad_src = (weights, kreg, dirs)
         self._grad = None

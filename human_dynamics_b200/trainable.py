@@ -29,7 +29,7 @@ from torch.autograd.function import once_differentiable
 
 from . import _lib
 from ._lib import lib, check, fptr, current_stream
-from .nets import (FAST_HEADS, GN_EPS, GN_GROUPS, BackwardDataPack, PackedConv, dgrad_op, grad_one_pass, require_training_impl,
+from .nets import (GN_EPS, GN_GROUPS, BackwardDataPack, PackedConv, dgrad_op, grad_one_pass, require_training_impl,
                    sync_packing, weight_tmap)
 
 F32 = torch.float32
@@ -101,7 +101,7 @@ def fmovie_forward(model, x, save):
     B, T, Cc = x.shape
     st = current_stream()
     dev = x.device
-    fast = FAST_HEADS and T * (Cc // GN_GROUPS) <= 1280
+    fast = T * (Cc // GN_GROUPS) <= 1280
     if fast:
         act = (torch.empty((B * T, Cc), dtype=torch.float16, device=dev), torch.empty((B * T, Cc), dtype=torch.float16, device=dev))
     else:
@@ -485,10 +485,8 @@ class TemporalModel(TrainableModule):
     kernels and build no graph.
 
     The forward follows HMMREngine's default configuration (impl 'auto'): f_movie takes the same branch as FMoviePlan (fused GroupNorm
-    + split for T*64 <= 1280 with HD_FAST_HEADS on, GroupNorm statistics + conv prologue otherwise), so it is bit-identical to the engine
-    at every T.  The IEF heads always run IEFPlan's fast-head kernels, whose saved h1 / h2 the backward reads; the HD_FAST_HEADS=0 A/B
-    switch of the inference plans (generic IEF descriptors) does not apply here, and with it set the engine's IEF outputs differ from
-    this model's in the last bits.
+    + split for T*64 <= 1280, GroupNorm statistics + conv prologue otherwise), so it is bit-identical to the engine at every T.  The IEF
+    heads run IEFPlan's fast-head kernels, whose saved h1 / h2 the backward reads.
 
     The backward's GEMMs follow `config.grad_precision` when the config has one (objective.TrainConfig): 'fp32' (3xTF32, the default)
     or 'tf32' (1xTF32, nets.GRAD_PRECISIONS)."""

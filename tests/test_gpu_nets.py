@@ -131,13 +131,11 @@ def test_conv_gemm_tcgen05_3xf16(case):
     (6, 14, 256, 160, 1, 1, False, True),    # Cout = 160: the third N tile has 32 valid columns of 64
 ])
 @pytest.mark.parametrize('tma', [True, False])
-def test_conv_gemm_presplit_activations(shape, tma, monkeypatch):
+def test_conv_gemm_presplit_activations_tma_flag(shape, tma):
     """A operand as a pre-activated fp16 head/remainder pair (cp.async producer) and the epilogue's second output
     relu(v*s2+b2) as such a pair, against an fp64 reference of the same arithmetic."""
     from human_dynamics_b200 import _lib
     from human_dynamics_b200.nets import PackedConv
-    from human_dynamics_b200 import nets
-    monkeypatch.setattr(nets, 'TMA_EPILOGUE', tma)       # with / without HD_CONV_NO_TMA_EPILOGUE: results must not depend on it
     n, H, Cin, Cout, k, stride, with_res, fp32_out = shape
     rng = np.random.RandomState(sum(shape))
     dev = torch.device('cuda')
@@ -155,6 +153,8 @@ def test_conv_gemm_presplit_activations(shape, tma, monkeypatch):
     rt = torch.from_numpy(r).to(dev) if with_res else None
     op = pc.bind(None, n, H, H, out, inp_split=(hi, lo), out_split=(oh, ol), res=rt,
                  post2=(torch.from_numpy(s2).to(dev), torch.from_numpy(b2).to(dev), 1), impl='tc3h')
+    if not tma:                                          # with / without HD_CONV_NO_TMA_EPILOGUE: results must not depend on it
+        op.d.flags |= _lib.HD_CONV_NO_TMA_EPILOGUE
     assert op.d.impl == _lib.HD_IMPL_TC_3XF16
     assert bool(op.d.tmap_out_hi) and bool(op.d.flags & _lib.HD_CONV_NO_TMA_EPILOGUE) == (not tma)
     op.run(torch.cuda.current_stream().cuda_stream)
@@ -212,30 +212,50 @@ def test_resnet_matches_oracle(weights, impl, n, size):
     assert rel_err(phi.cpu().numpy(), ref) < REL
 
 
+def _run_whole_and_stages(packed, img, size, cut, next_has_shortcut):
+    """phi of the whole split plan, and of two stage plans cut in front of unit `cut` and chained the way engine._trunk chains them
+    (stage A writes the fp32 map and the pre-activated pair that stage B reads): (whole plan, stage A, stage B, phi, stage phi)."""
+    from human_dynamics_b200.nets import ResNetPlan, f16_pair
+    n, dev = img.shape[0], img.device
+    whole = ResNetPlan(packed, n, size, 'auto')
+    pa = ResNetPlan(packed, n, size, 'auto', units=(0, cut), root=True, tail=False, next_pre=packed.units[cut]['pre'],
+                    next_has_shortcut=next_has_shortcut)
+    pb = ResNetPlan(packed, n, size, 'auto', units=(cut, len(packed.units)), root=False)
+    assert whole.split and pa.split and pb.split
+    mid = torch.full((n, pa.out_hw, pa.out_hw, pa.out_depth), float('nan'), device=dev)
+    mid_split = f16_pair(mid.shape, dev, 'auto')
+    pa.set_output(mid, mid_split)
+    pb.set_input(mid, mid_split)
+    phi, phi_s = (torch.empty((n, 2048), dtype=torch.float32, device=dev) for _ in range(2))
+    whole.run(img, phi)
+    pa.run(img, None)
+    pb.run(None, phi_s)
+    torch.cuda.synchronize()
+    return whole, pa, pb, phi, phi_s
+
+
+def _out_subsample_ops(plan):
+    return sum(1 for op in plan.ops if getattr(op, 'd', None) is not None and op.d.out_subsample > 1)
+
+
 @pytest.mark.parametrize('size', [224, 72])
-def test_resnet_epilogue_subsample_equals_subsample_pass(weights, monkeypatch, size):
+def test_resnet_epilogue_subsample_equals_stage_subsample_pass(weights, size):
     """The unit in front of a strided identity unit writes x[:, ::s, ::s] from its conv3 epilogue (hd_conv_desc.out_subsample) instead of
-    the full fp32 map + an hd_subsample pass: same bits, three passes fewer (size 72 walks odd maps: 9 -> 5 -> 3)."""
-    from human_dynamics_b200 import synthetic, nets, _lib
-    from human_dynamics_b200.nets import PackedResNet, ResNetPlan, SubsampleOp
+    the full fp32 map + an hd_subsample pass: same bits, three passes fewer (size 72 walks odd maps: 9 -> 5 -> 3).  A stage plan that
+    starts at block 1's strided identity unit has no unit in front of it and runs the hd_subsample pass."""
+    from human_dynamics_b200 import synthetic, _lib
+    from human_dynamics_b200.nets import PackedResNet, SubsampleOp
     from oracle import nets_ref
     dev = torch.device('cuda')
     img_h = synthetic.make_images(3, seed=8, size=size)
     img = torch.from_numpy(img_h).to(dev)
     packed = PackedResNet(weights, dev, tc='auto')
-    outs = []
-    for epi in (True, False):
-        monkeypatch.setattr(nets, 'SUBSAMPLE_EPI', epi)
-        plan = ResNetPlan(packed, 3, size, 'auto')
-        assert plan.split
-        assert sum(isinstance(op, SubsampleOp) for op in plan.ops) == (0 if epi else 3)
-        assert sum(1 for op in plan.ops if getattr(op, 'd', None) is not None and op.d.out_subsample > 1) == (3 if epi else 0)
-        phi = torch.empty((3, 2048), dtype=torch.float32, device=dev)
-        plan.run(img, phi)
-        torch.cuda.synchronize()
-        outs.append(phi)
-    assert torch.equal(outs[0], outs[1])
-    assert rel_err(outs[0].cpu().numpy(), nets_ref.encoder_resnet(img_h, weights).numpy()) < REL
+    plan, pa, pb, phi, phi_s = _run_whole_and_stages(packed, img, size, 2, False)
+    assert not any(isinstance(op, SubsampleOp) for op in plan.ops) and _out_subsample_ops(plan) == 3
+    assert isinstance(pb.ops[0], SubsampleOp) and sum(isinstance(op, SubsampleOp) for op in pa.ops + pb.ops) == 1
+    assert _out_subsample_ops(pa) + _out_subsample_ops(pb) == 2
+    assert torch.equal(phi, phi_s)
+    assert rel_err(phi.cpu().numpy(), nets_ref.encoder_resnet(img_h, weights).numpy()) < REL
     # descriptors outside the activation-map contract refuse the flag instead of silently writing the full map
     op = next(op for op in plan.ops if getattr(op, 'd', None) is not None and op.d.out and op.d.res)
     op.d.out_subsample = 2
@@ -244,24 +264,25 @@ def test_resnet_epilogue_subsample_equals_subsample_pass(weights, monkeypatch, s
     op.d.out_subsample = 0
 
 
-def test_resnet_dead_fp32_outputs_are_dead(weights, monkeypatch):
-    """Skipping the fp32 copies nobody reads (pool1 output, block outputs in front of a conv shortcut) must not change a bit."""
-    from human_dynamics_b200 import synthetic, nets
-    from human_dynamics_b200.nets import PackedResNet, ResNetPlan
+def test_resnet_dead_fp32_outputs_are_dead_across_stages(weights):
+    """Skipping the fp32 copies nobody reads (pool1 output, block outputs in front of a conv shortcut) must not change a bit: the whole
+    plan against stage plans cut in front of block 2's conv shortcut, whose stage A skips its fp32 output or writes it."""
+    from human_dynamics_b200 import synthetic
+    from human_dynamics_b200.nets import PackedResNet
     dev = torch.device('cuda')
     img = torch.from_numpy(synthetic.make_images(3, seed=5, size=224)).to(dev)
     packed = PackedResNet(weights, dev, tc='auto')
+    assert 'shortcut' in packed.units[3]
+
+    def dead(plan):
+        return sum(1 for op in plan.ops if getattr(op, 'd', None) is not None and not op.d.out and op.d.res)
     outs = []
-    for drop in (True, False):
-        monkeypatch.setattr(nets, 'DROP_DEAD_FP32', drop)
-        plan = ResNetPlan(packed, 3, 224, 'auto')
-        assert plan.split and plan.pool_f32_dead == drop
-        assert sum(1 for op in plan.ops if getattr(op, 'd', None) is not None and not op.d.out and op.d.res) == (3 if drop else 0)
-        phi = torch.empty((3, 2048), dtype=torch.float32, device=dev)
-        plan.run(img, phi)
-        torch.cuda.synchronize()
-        outs.append(phi.cpu().numpy())
-    assert np.array_equal(outs[0], outs[1])
+    for skip in (True, False):
+        plan, pa, pb, phi, phi_s = _run_whole_and_stages(packed, img, 224, 3, skip)
+        assert plan.pool_f32_dead and pa.pool_f32_dead
+        assert dead(plan) == 3 and dead(pa) + dead(pb) == (3 if skip else 2)
+        outs += [phi, phi_s]
+    assert all(torch.equal(outs[0], o) for o in outs[1:])
 
 
 @pytest.mark.parametrize('impl', ['simt', 'auto'])
@@ -412,13 +433,12 @@ def test_hal_mode_and_models_surface(weights, smpl_model):
 
 @pytest.mark.parametrize('n,size', [(2, 24), (3, 224), (5, 64)])
 @pytest.mark.parametrize('tma', [True, False])
-def test_conv1_from_padded_fp16_planes(n, size, tma, monkeypatch):
+def test_conv1_from_padded_fp16_planes_tma_flag(n, size, tma):
     """ResNet root conv1 (7x7/2, explicit pad 3+3, bias) through the plane-input tensor-core path: hd_pack_conv1_planes
     + hd_conv_gemm(HD_CONV_INPUT_PLANES) against an fp64 convolution."""
-    from human_dynamics_b200 import nets
+    from human_dynamics_b200 import nets, _lib
     from human_dynamics_b200._lib import lib, check, fptr
     import ctypes as C
-    monkeypatch.setattr(nets, 'TMA_EPILOGUE', tma)
     rng = np.random.RandomState(n * 1000 + size)
     dev = torch.device('cuda')
     x = rng.uniform(-1, 1, size=(n, size, size, 3)).astype(np.float32)
@@ -428,6 +448,8 @@ def test_conv1_from_padded_fp16_planes(n, size, tma, monkeypatch):
     planes = pc.alloc_planes(n, size)
     out = torch.zeros((n, size // 2, size // 2, 64), device=dev)
     op = pc.bind(planes, n, size, out)
+    if not tma:                                          # results must not depend on HD_CONV_NO_TMA_EPILOGUE
+        op.d.flags |= _lib.HD_CONV_NO_TMA_EPILOGUE
     assert bool(op.d.tmap_out) and bool(op.d.flags & 1) == (not tma)
     st = torch.cuda.current_stream().cuda_stream
     xt = torch.from_numpy(x).to(dev)

@@ -25,33 +25,61 @@ def _convs(plan):
     return [o for o in plan.ops if getattr(o, 'd', None) is not None]
 
 
-def test_resnet_plan_wiring(fake_device, monkeypatch):
+def test_resnet_plan_and_stage_wiring(fake_device):
     nets = fake_device
     from human_dynamics_b200 import synthetic
     packed = nets.PackedResNet(synthetic.make_resnet_weights(seed=1), 'cpu', tc='auto')
     assert len(packed.units) == 16
-    for epi in (True, False):
-        monkeypatch.setattr(nets, 'SUBSAMPLE_EPI', epi)
-        plan = nets.ResNetPlan(packed, 2, 64, 'auto')
-        assert plan.split and plan.pool_f32_dead
-        convs = _convs(plan)
-        assert len(convs) == 52                                            # 16 units x 3 + 4 shortcut convs (conv1 of the root is separate)
-        subs = [o for o in plan.ops if isinstance(o, nets.SubsampleOp)]
-        epis = [(o.d.Cout, o.d.Ho, o.d.out_subsample) for o in convs if o.d.out_subsample > 1]
-        # the units in front of the three strided identity units write x[:, ::2, ::2] themselves (maps 16 -> 8 -> 4 -> 2 at size 64)
-        assert (len(subs), epis) == ((0, [(256, 16, 2), (512, 8, 2), (1024, 4, 2)]) if epi else (3, []))
-        assert sum(1 for o in convs if not o.d.out and o.d.res) == 3       # fp32 outputs in front of a conv shortcut are never written
-        assert plan.num_launches == 3 + len(plan.ops) + 1
-        for o in convs:
-            d = o.d
-            assert d.in_hi and d.in_lo and not d.in_ and d.impl == 3       # every trunk conv reads a pre-split pair
-            if d.res:
-                assert (d.res_stride, d.res_H, d.res_W, d.res_ld) == (1, d.Ho, d.Wo, d.Cout)   # residual rows == output rows (TMA slabs)
-            if d.out_subsample > 1:
-                assert d.out and not d.tmap_out and d.tmap_out_hi and d.res                      # dense subsample: no fp32 TMA store
-        # the residual of a strided identity unit is the dense subsampled buffer in both variants
-        strided = [o for o in convs if o.d.KH == 1 and o.d.res and o.d.res == plan.bufS.data_ptr() and o.d.Cout in (256, 512, 1024)]
-        assert len(strided) >= 3
+    plan = nets.ResNetPlan(packed, 2, 64, 'auto')
+    assert plan.split and plan.pool_f32_dead
+    convs = _convs(plan)
+    assert len(convs) == 52                                            # 16 units x 3 + 4 shortcut convs (conv1 of the root is separate)
+    subs = [o for o in plan.ops if isinstance(o, nets.SubsampleOp)]
+    epis = [(o.d.Cout, o.d.Ho, o.d.out_subsample) for o in convs if o.d.out_subsample > 1]
+    # the units in front of the three strided identity units write x[:, ::2, ::2] themselves (maps 16 -> 8 -> 4 -> 2 at size 64)
+    assert (len(subs), epis) == (0, [(256, 16, 2), (512, 8, 2), (1024, 4, 2)])
+    assert sum(1 for o in convs if not o.d.out and o.d.res) == 3       # fp32 outputs in front of a conv shortcut are never written
+    assert plan.num_launches == 3 + len(plan.ops) + 1
+    for o in convs:
+        d = o.d
+        assert d.in_hi and d.in_lo and not d.in_ and d.impl == 3       # every trunk conv reads a pre-split pair
+        if d.res:
+            assert (d.res_stride, d.res_H, d.res_W, d.res_ld) == (1, d.Ho, d.Wo, d.Cout)   # residual rows == output rows (TMA slabs)
+        if d.out_subsample > 1:
+            assert d.out and not d.tmap_out and d.tmap_out_hi and d.res                      # dense subsample: no fp32 TMA store
+    # the residual of a strided identity unit is the dense subsampled buffer
+    strided = [o for o in convs if o.d.KH == 1 and o.d.res and o.d.res == plan.bufS.data_ptr() and o.d.Cout in (256, 512, 1024)]
+    assert len(strided) >= 3
+
+    # cut in front of block 1's strided identity unit: stage A writes its fp32 output, and stage B subsamples it in one hd_subsample
+    # pass that reads the stage input
+    nxt = packed.units[2]
+    pa = nets.ResNetPlan(packed, 2, 64, 'auto', units=(0, 2), root=True, tail=False, next_pre=nxt['pre'], next_has_shortcut=False)
+    pb = nets.ResNetPlan(packed, 2, 64, 'auto', units=(2, 16), root=False)
+    assert _convs(pa)[-1].d.out and not any(o.d.out_subsample > 1 for o in _convs(pa))
+    assert isinstance(pb.ops[0], nets.SubsampleOp) and (pb.ops[0], 'res', 2) in pb.in_refs
+    assert sum(isinstance(o, nets.SubsampleOp) for o in pb.ops) == 1
+    assert [o.d.out_subsample for o in _convs(pb) if o.d.out_subsample > 1] == [2, 2]
+    assert _convs(pb)[2].d.res == pb.bufS.data_ptr()                  # the strided unit's conv3 reads the dense copy
+
+
+def test_root_conv1_choice(fake_device):
+    """bind_root_conv1: the fp16 impls read padded fp16 planes at even sizes and gather the fp32 images at odd ones; 'simt' has no
+    conv1 op (hd_conv1_7x7s2)."""
+    nets = fake_device
+    from human_dynamics_b200 import _lib, synthetic
+    w = synthetic.make_resnet_weights(seed=1)
+    packed = nets.PackedResNet(w, 'cpu', tc='auto')
+    even = nets.ResNetPlan(packed, 2, 64, 'auto')
+    assert even.planes is not None and even.conv1_op.d.flags & _lib.HD_CONV_INPUT_PLANES
+    assert even.conv1_op.d.out == even.root_buf.data_ptr() and even.num_launches == 3 + len(even.ops) + 1
+    odd = nets.ResNetPlan(packed, 2, 63, 'auto')
+    d = odd.conv1_op.d
+    assert odd.planes is None and d.impl == _lib.HD_IMPL_TC_3XF16 and not d.flags & _lib.HD_CONV_INPUT_PLANES
+    assert (d.KH, d.KW, d.Cin, d.in_ld, d.H) == (7, 7, 3, 3, 63) and d.out == odd.root_buf.data_ptr()
+    assert odd.num_launches == 2 + len(odd.ops) + 1
+    simt = nets.ResNetPlan(nets.PackedResNet(w, 'cpu', tc=False), 2, 64, 'simt')
+    assert simt.planes is None and simt.conv1_op is None and simt.num_launches == 2 + len(simt.ops) + 1
 
 
 def test_stage_plans_keep_the_pairs_inside_a_stage(fake_device):

@@ -31,18 +31,8 @@ for n, H, Cin, Cout, k, s, res, pre in cases:
     else:
         op = pc.bind(x, n, H, H, out, pre=pr, res=r, impl=os.environ.get('HD_IMPL', 'tc3h'))
     st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    modes = [int(a) for a in sys.argv[1:]] or [0]
-    for mode in modes:
-        dbg = torch.zeros(16, dtype=torch.int64, device=dev)
-        dbg[15] = mode
-        for _ in range(3):
-            check(lib.hd_conv_gemm_profile(op.ref, st, C.c_void_p(dbg.data_ptr())))
-        torch.cuda.synchronize()
-        if mode:
-            d = dbg.cpu().numpy()
-            print('   [xmode %d: 1=no A STS, 2=no B TMA, 4=no A loads]  ' % mode + '  '.join('%s=%d' % (nm, v) for nm, v in zip(NAMES, d)))
     dbg = torch.zeros(16, dtype=torch.int64, device=dev)
-    for _ in range(2):
+    for _ in range(3):
         check(lib.hd_conv_gemm_profile(op.ref, st, C.c_void_p(dbg.data_ptr())))
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
