@@ -138,6 +138,28 @@ class EvalFramesArgs(C.Structure):
     ]
 
 
+HD_JPEG_BAD_CODE, HD_JPEG_OVERRUN, HD_JPEG_MARKER, HD_JPEG_BAD_HEADER = 1, 2, 4, 8
+
+
+class JpegHuffman(C.Structure):
+    """Mirror of hd_jpeg_huffman."""
+    _fields_ = [('bits', C.c_uint8 * 16), ('vals', C.c_uint8 * 256)]
+
+
+class JpegHeader(C.Structure):
+    """Mirror of hd_jpeg_header."""
+    _fields_ = [
+        ('width', C.c_int), ('height', C.c_int), ('h_samp', C.c_int), ('v_samp', C.c_int), ('restart_interval', C.c_int),
+        ('qt', C.c_int * 3), ('dc', C.c_int * 3), ('ac', C.c_int * 3), ('data_offset', C.c_longlong), ('data_bytes', C.c_longlong),
+    ]
+
+
+class JpegTables(C.Structure):
+    """Mirror of hd_jpeg_tables."""
+    _fields_ = [('quant', (C.c_uint16 * 64) * 4), ('dc', JpegHuffman * 4), ('ac', JpegHuffman * 4),
+                ('quant_defined', C.c_int), ('dc_defined', C.c_int), ('ac_defined', C.c_int)]
+
+
 # name -> (restype, argtypes); must list every symbol include/hd_b200.h declares.
 _vp, _i, _ll, _f, _sz = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_size_t
 SIGNATURES = {
@@ -223,6 +245,9 @@ SIGNATURES = {
     'hd_eval_frames': (_i, [C.POINTER(EvalFramesArgs), _vp]),
     'hd_eval_mesh_tpose': (_i, [C.POINTER(SmplConsts), _vp, _i, _vp, _i, _i, _vp, _vp]),
     'hd_eval_verts_error': (_i, [_vp, _ll, _vp, _ll, _i, _i, _vp, _vp]),
+    'hd_jpeg_parse': (_i, [_vp, _sz, C.POINTER(JpegHeader), C.POINTER(JpegTables)]),
+    'hd_jpeg_workspace_bytes': (_sz, [_i, _i, _i, _i, _i]),
+    'hd_jpeg_decode': (_i, [_vp, _ll, _vp, _i, _i, _i, _i, _i, _vp, _i, _vp, _i, _vp, _vp, _vp, _sz, _vp]),
 }
 
 

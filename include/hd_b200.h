@@ -669,6 +669,56 @@ int hd_eval_mesh_tpose(const hd_smpl_consts *c, const float *beta_gt, int beta_g
                        double *out, void *stream);
 int hd_eval_verts_error(const float *a, long long a_ld, const float *b, long long b_ld, int N, int V, double *out, void *stream);
 
+/* ---- JPEG decoding: libjpeg's default decompression (what tf.image.decode_jpeg and cv2.imdecode run) of baseline streams ----
+ * Supported: SOF0 / SOF1, Huffman coding, 8-bit samples, 3 components read as YCbCr, one interleaved scan, luma sampling 1x1, 2x1 or
+ * 2x2 with chroma 1x1 (4:4:4, 4:2:2, 4:2:0), with or without restart intervals.  The output is bit for bit libjpeg's: the islow
+ * integer IDCT with its range-limit table, fancy (triangle) chroma upsampling, the integer YCbCr -> RGB tables (oracle/jpeg_ref.py).
+ *
+ * hd_jpeg_parse (host code, no device touched): the markers of one JPEG `data[0, len)` into *hdr and the tables it defines into *tables
+ * (both host, both required).  qt / dc / ac are the stream's table slots 0..3; data_offset / data_bytes delimit the
+ * entropy-coded data, from the end of the SOS segment to the first marker other than RSTn, which must be EOI.  Never reads outside
+ * data[0, len); fill bytes (FF) before EOI are not counted.  HD_ERR_UNSUPPORTED: progressive, lossless or arithmetic coding, precision
+ * other than 8, other than 3 components, other sampling, a second scan, RGB colour (Adobe transform 0 or component ids 'R','G','B'),
+ * more than 2^31 - 1 pixels or bytes of entropy-coded data.  HD_ERR_INVALID: malformed or truncated
+ * markers, a bad Huffman table (codes that do not fit, DC symbols > 15), a scan using an undefined table, entropy-coded data without
+ * a terminating marker.
+ *
+ * hd_jpeg_decode: N images of one size H x W and one luma sampling (h_samp, v_samp) into out uint8 RGB [N, H, W, 3].  Four launches
+ * whatever N: restart-marker scan and Huffman lookup tables; Huffman decoding, one thread per entropy-coded segment (a whole image, or
+ * one restart interval), writing dequantised int16 coefficients; the IDCT, one 8x8 block per 8 threads; upsampling and colour
+ * conversion, one output pixel per thread.  data: device bytes holding every image's entropy-coded data at hdrs[i].data_offset (the
+ * JPEGs themselves, concatenated, do); data_size: its length.  hdrs: device [N]; their qt index quant [n_quant][64] (uint16, natural
+ * order) and dc / ac index huff [n_huff] (both device).  status: device int [N], written for every image: 0, or an OR of
+ * HD_JPEG_BAD_CODE (no code matches), HD_JPEG_OVERRUN (more bits consumed than the segment holds), HD_JPEG_MARKER (a marker inside a
+ * segment, restart markers missing, extra or out of sequence), HD_JPEG_BAD_HEADER (size, sampling, table index or data range does not
+ * fit the call, or data_bytes > 2^31 - 1; nothing of that image's data is read).  Fill bytes before a restart marker are skipped.  A flagged image's pixels are unspecified but written; every other image
+ * decodes exactly.  Workspace: hd_jpeg_workspace_bytes(N, H, W, h_samp, v_samp) bytes, 256-byte aligned.  HD_ERR_INVALID (before any
+ * launch): a null pointer, N < 1, H or W outside [1, 65535], H * W > 2^31 - 1, N so large that a launch's grid would exceed 2^31 - 1
+ * blocks (hd_jpeg_workspace_bytes returns 0 for the same arguments), unsupported sampling, n_quant < 1, n_huff outside [1, 6N], or a
+ * short workspace. */
+enum { HD_JPEG_BAD_CODE = 1, HD_JPEG_OVERRUN = 2, HD_JPEG_MARKER = 4, HD_JPEG_BAD_HEADER = 8 };
+typedef struct {
+  uint8_t bits[16];               /* number of codes of each length 1..16 */
+  uint8_t vals[256];              /* symbols in code order */
+} hd_jpeg_huffman;
+typedef struct {
+  int width, height;
+  int h_samp, v_samp;             /* luma sampling factors; chroma are 1x1 */
+  int restart_interval;           /* MCUs per restart interval, 0 = none */
+  int qt[3], dc[3], ac[3];        /* tables of Y, Cb, Cr: stream slots after hd_jpeg_parse, array indices for hd_jpeg_decode */
+  long long data_offset, data_bytes;
+} hd_jpeg_header;
+typedef struct {
+  uint16_t quant[4][64];          /* natural order */
+  hd_jpeg_huffman dc[4], ac[4];
+  int quant_defined, dc_defined, ac_defined;   /* bit s set: slot s was defined */
+} hd_jpeg_tables;
+int hd_jpeg_parse(const uint8_t *data, size_t len, hd_jpeg_header *hdr, hd_jpeg_tables *tables);
+size_t hd_jpeg_workspace_bytes(int N, int H, int W, int h_samp, int v_samp);
+int hd_jpeg_decode(const uint8_t *data, long long data_size, const hd_jpeg_header *hdrs, int N, int H, int W, int h_samp, int v_samp,
+                   const uint16_t *quant, int n_quant, const hd_jpeg_huffman *huff, int n_huff, uint8_t *out, int *status,
+                   void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

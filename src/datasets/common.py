@@ -4,8 +4,8 @@ plus the `tf.python_io.tf_record_iterator` it is fed from.
 A tfrecord file is a sequence of records: uint64 length (little endian), uint32 masked CRC32C of those 8 bytes, the payload, uint32
 masked CRC32C of the payload.  Both checksums are verified; a short or corrupt record raises IOError.  The payload is a serialized
 `tf.train.Example` (a Features map of name -> BytesList / FloatList / Int64List), decoded here from the protobuf wire format in pure
-Python (packed and unpacked repeated fields both accepted).  JPEG frames are decoded with OpenCV, as RGB.  Writing records is not part
-of this module.
+Python (packed and unpacked repeated fields both accepted).  JPEG frames are decoded as RGB, one at a time with OpenCV (decode_jpeg), or a
+tube at once on the GPU (decode_jpegs).  Writing records is not part of this module.
 
 The checksums are computed in Python (slicing-by-8 tables): about 15 MB/s on one host core, so a test record of a few hundred 224^2
 JPEGs (a few MB) costs a fraction of a second to verify; tools/bench_eval.py times reading a record of that size.
@@ -178,6 +178,19 @@ def decode_jpeg(data):
     if img is None or img.ndim != 3 or img.shape[2] != 3:
         raise ValueError('not a 3-channel JPEG')
     return img[:, :, ::-1].copy()
+
+
+def decode_jpegs(datas):
+    """The JPEG strings of one tube -> its frames, RGB: a uint8 CUDA tensor (N, H, W, 3) from the GPU decoder
+    (human_dynamics_b200.jpeg, bit for bit what decode_jpeg gives) when it takes every frame, else an N x H x W x 3 uint8 array from
+    decode_jpeg.  decode_jpeg stays the path for streams the GPU decoder does not take (progressive, grayscale, other samplings,
+    mixed sizes) and for corrupt data, where libjpeg returns an image with a warning.  Any other failure (no CUDA device, a failed
+    launch) raises HDError: there is no host fallback for those."""
+    from human_dynamics_b200 import jpeg
+    try:
+        return jpeg.decode(datas)
+    except (jpeg.UnsupportedJPEG, jpeg.CorruptJPEG):
+        return np.asarray([decode_jpeg(d) for d in datas])
 
 
 def read_from_example(serialized_ex, decode_images=True):

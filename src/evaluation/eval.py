@@ -93,6 +93,13 @@ def _mesh_model(smpl):
 
 
 def _img_size(images):
+    """The frame height of a tube: read from the first JPEG's SOF marker (hd_jpeg_parse, no decoding), or from a decoded frame."""
+    if len(images) and isinstance(images[0], (bytes, bytearray)):
+        from human_dynamics_b200 import jpeg
+        try:
+            return jpeg.parse(images[0])[0].height
+        except jpeg.UnsupportedJPEG:
+            pass
     return decode_frames(images[:1]).shape[1]
 
 

@@ -53,16 +53,28 @@ def split_preds(preds):
 
 
 def decode_frames(images):
-    """Frames as an N x H x W x 3 array; JPEG strings (read_from_example(..., decode_images=False)) are decoded here."""
+    """Frames as an N x H x W x 3 array; JPEG strings (read_from_example(..., decode_images=False)) are decoded here, on the GPU into a
+    uint8 CUDA tensor when the GPU decoder takes every frame (src.datasets.common.decode_jpegs)."""
     if len(images) and isinstance(images[0], (bytes, bytearray)):
-        from src.datasets.common import decode_jpeg
-        images = [decode_jpeg(im) for im in images]
+        from src.datasets.common import decode_jpegs
+        return decode_jpegs(images)
     return np.asarray(images)
+
+
+def to_unit_range(frames):
+    """Decoded uint8 CUDA frames -> float32 CUDA frames, mapped from [0, 255] to [-1, 1] when the max is > 1.1: the same float32 values
+    as the host path's float64 (x / 255) * 2 - 1, from a 256-entry table computed with that numpy arithmetic."""
+    import torch
+    if int(frames.max()) <= 1.1:
+        return frames.float()
+    lut = torch.from_numpy(((np.arange(256, dtype=np.float64) / 255) * 2 - 1).astype(np.float32)).to(frames.device)
+    return lut.index_select(0, frames.reshape(-1).int()).view(frames.shape)
 
 
 def get_predictions(model, images, load_path, tf_path, p_id, pred_dir=PRED_DIR, incl_verts=False):
     """The cached predictions of a tube if they exist, else model.predict_all_images on its frames (cached for next time).  `images`
-    may be decoded frames or JPEG strings; JPEGs are decoded only on a cache miss."""
+    may be decoded frames or JPEG strings; JPEGs are decoded only on a cache miss, on the GPU when the GPU decoder takes them, and the
+    frames then stay on the device."""
     t0 = time()
     pred_path, _ = get_pred_path_name(load_path, tf_path, p_id, pred_dir=pred_dir, incl_verts=False)
     vert_path, _ = get_pred_path_name(load_path, tf_path, p_id, pred_dir=pred_dir, incl_verts=True)
@@ -76,7 +88,9 @@ def get_predictions(model, images, load_path, tf_path, p_id, pred_dir=PRED_DIR, 
     else:
         print('Computing the predictions.')
         images = decode_frames(images)
-        if np.max(images) > 1.1:                 # frames in [0, 255] -> [-1, 1], as the reference's sanity check does
+        if not isinstance(images, np.ndarray):   # decoded on the device
+            images = to_unit_range(images)
+        elif np.max(images) > 1.1:               # frames in [0, 255] -> [-1, 1], as the reference's sanity check does
             images = (np.array(images) / 255) * 2 - 1
         preds = model.predict_all_images(images)
         preds.update({'tf_path': tf_path, 'p_id': p_id})

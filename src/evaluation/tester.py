@@ -156,7 +156,8 @@ class Tester(object):
             yield {k: (v.numpy().copy() if copy else v.numpy()) for k, v in prev[0].items()}
 
     def predict_all_images(self, all_images, cache_features=True):
-        """Sliding-window prediction over a whole sequence (tester.py:260-312).  all_images: N x H x W x 3.
+        """Sliding-window prediction over a whole sequence (tester.py:260-312).  all_images: N x H x W x 3, a numpy array or a float32
+        CUDA tensor (read in place on the device, no host round trip with the default cache_features).
 
         Windows are formed exactly as the reference does (margin zero-images in front, zero-image fill at the back, stride
         g = T - 2*margin, keep [margin:-margin]) because GroupNorm couples all T frames of a window.  With
@@ -174,15 +175,26 @@ class Tester(object):
             raise ValueError('sequence_length %d leaves no frame with full field of view %d' % (T, self.fov))
         count = int(np.ceil(N / (g * B)))
         num_fill = count * B * g + T - N
-        all_images = np.asarray(all_images, dtype=np.float32)
+        on_device = isinstance(all_images, torch.Tensor) and all_images.is_cuda
+        if on_device:
+            if all_images.dtype != torch.float32:
+                raise ValueError('all_images on the device must be float32, got %s' % all_images.dtype)
+            all_images = all_images.contiguous()
+        else:
+            all_images = np.asarray(all_images, dtype=np.float32)
         if tuple(all_images.shape[1:]) != (H, W, 3):
             raise ValueError('all_images must be N x %d x %d x 3' % (H, W))
+        if on_device and not cache_features:
+            all_images = all_images.cpu().numpy()
         results = {}
         if cache_features:
             dev = self.engine.device
             phi_parts = []
             for i in range(0, N, 640):                       # bounded device residency of raw frames
-                x = torch.from_numpy(all_images[i:i + 640]).to(dev, non_blocking=True)
+                if on_device:
+                    x = all_images[i:i + 640].to(dev)
+                else:
+                    x = torch.from_numpy(all_images[i:i + 640]).to(dev, non_blocking=True)
                 phi_parts.append(self.engine.encode_images(x).clone())
             phi_zero = self.engine.encode_images(torch.zeros((1, H, W, 3), dtype=torch.float32, device=dev)).clone()
             phi_padded = torch.cat([phi_zero.expand(margin, -1)] + phi_parts + [phi_zero.expand(num_fill, -1)], dim=0)
