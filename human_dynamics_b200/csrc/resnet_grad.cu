@@ -522,16 +522,23 @@ extern "C" size_t hd_conv_wgrad_workspace_bytes(long long pixels, int K, int Cou
 
 namespace {
 
+constexpr int kMaxDevices = 64;
+
 template <bool SPLIT>
 int launch_wgrad(const WgradArgs &a, dim3 grid, cudaStream_t st) {
-  static bool smem_set = false;               // (benign race: every caller sets the same value)
-  if (!smem_set) {
+  // function attributes are per device: a process may drive several GPUs through this library
+  // (benign race: every caller sets the same value)
+  static bool configured[kMaxDevices] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= kMaxDevices) { hd::set_last_error_text("hd_conv_wgrad: device ordinal out of range"); return HD_ERR_UNSUPPORTED; }
+  if (!configured[dev]) {
     const cudaError_t e = cudaFuncSetAttribute(wgrad_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgradCfg<SPLIT>::kSmem);
     if (e != cudaSuccess) {
       hd::set_last_error("hd_conv_wgrad: cudaFuncSetAttribute", e);
       return HD_ERR_CUDA;
     }
-    smem_set = true;
+    configured[dev] = true;
   }
   wgrad_kernel<SPLIT><<<grid, kWgradThreads, WgradCfg<SPLIT>::kSmem, st>>>(a);
   return hd::check_launch("wgrad_kernel");

@@ -362,15 +362,21 @@ __global__ void orth_proj_kernel(const float *__restrict__ X, const float *__res
   out[i * 2 + 1] = s * (X[i * 3 + 1] + ty);
 }
 
+constexpr int kMaxDevices = 64;
+
 template <int PT, int NNZ>
 int launch_skin(const hd_smpl_consts *c, const float *beta, int beta_ld, const float *Rs, const float *A12, float *verts, int N,
                 int out_mul, int out_off, cudaStream_t st) {
   const size_t smem = (size_t)(kNumDirs * PT + PT * 288) * sizeof(float);
-  static bool configured = false;
-  if (!configured) {
+  // function attributes are per device: a process may drive several GPUs through this library
+  static bool configured[kMaxDevices] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= kMaxDevices) { hd::set_last_error_text("smpl_skin: device ordinal out of range"); return HD_ERR_UNSUPPORTED; }
+  if (!configured[dev]) {
     cudaError_t e = cudaFuncSetAttribute(smpl_skin_kernel<PT, NNZ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { hd::set_last_error("smpl_skin attr", e); return HD_ERR_CUDA; }
-    configured = true;
+    configured[dev] = true;
   }
   dim3 grid(hd::ceil_div(N, PT), hd::ceil_div(c->num_verts, 128));
   smpl_skin_kernel<PT, NNZ><<<grid, 128, smem, st>>>(c->v_template, c->dirs, c->lbs_idx, c->lbs_w, c->lbs_nnz, beta, beta_ld, Rs,

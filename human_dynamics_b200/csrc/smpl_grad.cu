@@ -393,15 +393,21 @@ __global__ void __launch_bounds__(128) orth_proj_backward_kernel(const float *__
 
 size_t lbs_backward_smem(int K) { return (size_t)(2 * kLbsPT * 288 + kLbsPT * 12 * kTile + kLbsPT * K * 3) * sizeof(float); }
 
+constexpr int kMaxDevices = 64;
+
 template <int NNZ>
 int launch_lbs_backward(const hd_smpl_consts *c, const hd_smpl_grad_consts *g, const float *v_posed, long long vp_ld, const float *A12,
                         const float *dverts, const float *djoints, float *dv_posed, float *dA12, int N, cudaStream_t st) {
   const size_t smem = lbs_backward_smem(kMaxKps);
-  static bool configured = false;
-  if (!configured) {
+  // function attributes are per device: a process may drive several GPUs through this library
+  static bool configured[kMaxDevices] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= kMaxDevices) { hd::set_last_error_text("smpl_lbs_backward: device ordinal out of range"); return HD_ERR_UNSUPPORTED; }
+  if (!configured[dev]) {
     cudaError_t e = cudaFuncSetAttribute(smpl_lbs_backward_kernel<NNZ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { hd::set_last_error("smpl_lbs_backward attr", e); return HD_ERR_CUDA; }
-    configured = true;
+    configured[dev] = true;
   }
   smpl_lbs_backward_kernel<NNZ><<<hd::ceil_div(N, kLbsPT), kLbsThreads, lbs_backward_smem(c->num_kps), st>>>(
       v_posed, vp_ld, A12, dverts, djoints, c->lbs_idx, c->lbs_w, c->lbs_nnz, g->kpv_ptr, g->kpv_kidx, g->kpv_w, c->num_kps, g->lbt_ptr,

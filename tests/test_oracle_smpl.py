@@ -132,3 +132,58 @@ def test_rot2aa_inverts_rodrigues():
     R = smpl_ref.batch_rodrigues(th, np.float64)
     assert np.allclose(smpl_ref.batch_rot2aa(R, np.float64), th, atol=1e-6)
     assert np.allclose(smpl_ref.batch_rot2aa(np.eye(3)[None], np.float64), 0.0)
+
+
+# ---- oracle/smpl_stages_ref.py: the stage-by-stage float64 restatement the GPU stage tests (test_gpu_smpl_stages.py) rely on ----
+
+def _rel64(a, b):
+    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
+    return float(np.abs(a - b).max() / max(np.abs(b).max(), 1e-300))
+
+
+@pytest.mark.parametrize('tree', ['smpl', 'chain', 'random1', 'random2'])
+def test_stage_ref_matches_smpl_ref(smpl_model, tree):
+    """Chained stages == SMPLRef(float64) (J through the precomposed J_template / J_shapedirs, FK level by level, dense skinning
+    in pose chunks) on SMPL's tree, the depth-23 chain and random trees, to float64 rounding."""
+    import torch
+    from oracle import smpl_stages_ref as sr
+    model = sr.with_tree(smpl_model, sr.test_trees()[tree])
+    beta, theta = synthetic.make_smpl_inputs(5, seed=3)
+    cam = np.random.RandomState(4).uniform(0.5, 1.5, size=(5, 3))
+    ref = smpl_ref.SMPLRef(model, dtype=np.float64)
+    verts, joints, Rs = ref(beta, theta, get_skin=True)
+    got = sr.smpl_forward(sr.model_constants(model), torch.from_numpy(beta), torch.from_numpy(theta), cam=cam)
+    want = {'verts': verts, 'joints': joints, 'Rs': Rs, 'Jtr': ref.J_transformed,
+            'kps': smpl_ref.batch_orth_proj_idrot(joints, cam, np.float64)}
+    for k, w in want.items():
+        assert _rel64(got[k].numpy(), w) < 1e-12, k
+    # the skinning in chunks of poses is the same as in one piece
+    assert _rel64(sr.skin(got['v_posed'], got['A'], model['weights'], chunk=2).numpy(), verts) < 1e-12
+
+
+@pytest.mark.parametrize('rotate_base', [False, True])
+@pytest.mark.parametrize('tree', ['smpl', 'chain', 'star', 'random1', 'random2'])
+def test_stage_fk_matches_global_rigid(tree, rotate_base):
+    import torch
+    from oracle import smpl_stages_ref as sr
+    parents = sr.test_trees()[tree]
+    rng = np.random.RandomState(5)
+    Rs = smpl_ref.batch_rodrigues(rng.normal(0, 0.5, size=(4 * 24, 3)), np.float64).reshape(4, 24, 3, 3)
+    Js = rng.normal(0, 0.3, size=(4, 24, 3))
+    nj, A = smpl_ref.batch_global_rigid_transformation(Rs, Js, parents, rotate_base=rotate_base, dtype=np.float64)
+    jtr, A34 = sr.forward_kinematics(torch.from_numpy(Rs), torch.from_numpy(Js), parents, rotate_base=rotate_base)
+    assert _rel64(jtr.numpy(), nj) < 1e-12 and _rel64(A34.numpy(), A[:, :, :3]) < 1e-12
+    if not rotate_base:                                          # and the independent 4x4 chains
+        nj2, A2 = _fk_loops(Rs, Js, parents)
+        assert _rel64(jtr.numpy(), nj2) < 1e-12 and _rel64(A34.numpy(), A2[:, :, :3]) < 1e-12
+    assert max(sr.tree_depths(parents)) == {'smpl': 8, 'chain': 23, 'star': 1}.get(tree, max(sr.tree_depths(parents)))
+
+
+def test_stage_rodrigues_matches_smpl_ref():
+    import torch
+    from oracle import smpl_stages_ref as sr
+    rng = np.random.RandomState(6)
+    th = np.concatenate([rng.normal(0, 1.0, size=(64, 3)), np.eye(3) * np.pi, np.eye(3) * 1e-7, [[0, 0, 0], [10, -3, 2]]])
+    assert _rel64(sr.rodrigues(torch.from_numpy(th)).numpy(), smpl_ref.batch_rodrigues(th, np.float64)) < 1e-14
+    # theta = 0: r = 0 and the angle is sqrt(3) 1e-8, so R = cos(angle) I, 1 to float64 rounding (and exactly I in float32)
+    assert (sr.rodrigues(torch.zeros(2, 3)) - torch.eye(3, dtype=torch.float64)).abs().max() < 1e-15
