@@ -14,7 +14,7 @@ import torch
 
 from . import _lib
 from .config import HMMRConfig
-from .nets import FMoviePlan, IEFPlan, PackedConv, PackedFMovie, PackedIEF, PackedResNet, ResNetPlan, f16_pair, sync_packing
+from .nets import FMoviePlan, IEFPlan, PackedFMovie, PackedHal, PackedIEF, PackedResNet, ResNetPlan, f16_pair
 from .smpl import SMPLConstants
 from ._lib import current_stream
 
@@ -99,16 +99,6 @@ def _rows(pair, i, n):
     if pair is None:
         return None
     return tuple(t[i:i + n] if t is not None else None for t in pair)
-
-
-class PackedHal(object):
-    """fc2_res hallucinator (models.py:270-296)."""
-
-    def __init__(self, w, device, tc=False, name='fc2_res'):
-        self.fc1 = PackedConv(w[name + '/fc1/weights'], device, post_shift=w[name + '/fc1/biases'], post_relu=True, tc=tc)
-        self.fc2 = PackedConv(w[name + '/fc2/weights'], device, post_shift=w[name + '/fc2/biases'], post_relu=True, tc=tc)
-        self.fc3 = PackedConv(w[name + '/fc3/weights'], device, post_shift=w[name + '/fc3/biases'], tc=tc)
-        sync_packing(device)
 
 
 class HMMREngine(object):
@@ -277,11 +267,7 @@ class HMMREngine(object):
             f32 = dict(dtype=torch.float32, device=feats.device)
             self._hal_plans[N] = [torch.empty((N, 2048), **f32) for _ in range(3)]
         h1, h2, out = self._hal_plans[N]
-        st = current_stream()
-        self.hal.fc1.bind(feats, N, 1, 1, h1, impl=self.impl).run(st)
-        self.hal.fc2.bind(h1, N, 1, 1, h2, impl=self.impl).run(st)
-        self.hal.fc3.bind(h2, N, 1, 1, out, res=feats, res_geom=(2048, 1, 1, 1), impl=self.impl).run(st)
-        return out.view(feats.shape)
+        return self.hal.run(feats.view(N, -1), h1, h2, out, self.impl).view(feats.shape)
 
     def theta_mean(self, N):
         if N not in self._theta0:

@@ -22,8 +22,8 @@ and batch-norm gamma / beta (trunk.TrainableResNet) join E's optimizer, e_loss's
 save_checkpoint writes their trained values.  Like the reference (whose gather_losses never adds slim's regularisation losses), the
 trunk trains without weight decay.
 
-Differences from the reference trainer: IEF dropout is the identity (the backward of trainable.TemporalModel follows the inference
-graph); the default optimizer, torch's Adam, adds eps to sqrt(v_hat) where TF's adds it to sqrt(v) before the bias correction, and
+Differences from the reference trainer: IEF dropout is the identity (trainable.TemporalModel runs the inference plans forward and
+follows the inference graph back); the default optimizer, torch's Adam, adds eps to sqrt(v_hat) where TF's adds it to sqrt(v) before the bias correction, and
 `optimizer=optim.TFAdam` removes that difference (TF's arithmetic, with its slots, beta powers and global_step in the checkpoint, so
 that `HMMRTrainer.resume(config, prefix, smpl_model)` continues a run where it stopped); the static `use_hmr_only` branch is not built, and freeze_phi=False needs image input (precomputed phis have no trunk to train).  A frame with no visible keypoint in an optimal-camera term
 contributes 0 (the reference's procrustes2d_vis divides 0 / 0 there and the loss is NaN).  The moving statistics start from whatever

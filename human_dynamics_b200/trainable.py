@@ -2,8 +2,9 @@
 hallucinator as torch parameters, differentiable on the GPU.
 
 This is what the reference trains in its default configuration (freeze_phi=True, precomputed_phi=True: src/config.py): everything
-after the ResNet.  Each forward runs the kernels and the packing of the inference plans (nets.FMoviePlan / IEFPlan fast heads,
-engine.PackedHal), so its outputs are bit-identical to HMMREngine's; the weights are packed on the device (hd_pack_weight) and repacked
+after the ResNet.  The model packs its parameters in place with the inference engine's packs (nets.PackedFMovie, PackedIEF, PackedHal)
+and each forward runs the inference plans over them (nets.FMoviePlan and IEFPlan with keep=True, which hold what the backward reads, and
+PackedHal.run), so its outputs are bit-identical to HMMREngine's; the weights are packed on the device (hd_pack_weight) and repacked
 before a forward whenever a parameter was changed in place (optimizer.step()).  The backward (csrc/net_grad.cu + hd_conv_gemm in its
 3xTF32 mode, or 1xTF32 with TrainConfig.grad_precision='tf32') is first-order, deterministic and follows the inference graph: dropout is the identity (is_training=False).
 
@@ -29,8 +30,8 @@ from torch.autograd.function import once_differentiable
 
 from . import _lib
 from ._lib import lib, check, fptr, current_stream
-from .nets import (GN_EPS, GN_GROUPS, BackwardDataPack, PackedConv, dgrad_op, grad_one_pass, require_training_impl,
-                   sync_packing, weight_tmap)
+from .nets import (GN_EPS, GN_GROUPS, BackwardDataPack, FMoviePlan, IEFPlan, PackedFMovie, PackedHal, PackedIEF, dgrad_op, grad_one_pass,
+                   require_training_impl, sync_packing, weight_tmap)
 
 F32 = torch.float32
 
@@ -95,39 +96,6 @@ def _wgrad(xt, M, k_pad, g_pieces, cols, out, st, one_pass=False):
 # ------------------------------------------------------------------------------------------------------------------------------------
 # f_movie
 # ------------------------------------------------------------------------------------------------------------------------------------
-def fmovie_forward(model, x, save):
-    """az_fc2_groupnorm over x (B,T,C) with the kernels of nets.FMoviePlan; returns (out, saved) with saved = [(block input, conv1
-    output)] per block when `save`."""
-    B, T, Cc = x.shape
-    st = current_stream()
-    dev = x.device
-    fast = T * (Cc // GN_GROUPS) <= 1280
-    if fast:
-        act = (torch.empty((B * T, Cc), dtype=torch.float16, device=dev), torch.empty((B * T, Cc), dtype=torch.float16, device=dev))
-    else:
-        gain, offset = torch.empty((B, Cc), dtype=F32, device=dev), torch.empty((B, Cc), dtype=F32, device=dev)
-    saved, cur = [], x
-    for blk in model.fm_blocks:
-        mid = torch.empty((B, T, Cc), dtype=F32, device=dev)
-        out = torch.empty((B, T, Cc), dtype=F32, device=dev)
-        for k, src, dst in ((1, cur, mid), (2, mid, out)):
-            g, b = blk['gn%d' % k]
-            conv = blk['conv%d' % k]
-            res = dict(res=cur, res_geom=(Cc, T, 1, 1)) if k == 2 else {}
-            if fast:
-                check(lib.hd_groupnorm_relu_split(fptr(src), fptr(g), fptr(b), _vp(act[0]), _vp(act[1]), B, T, Cc, GN_GROUPS, GN_EPS, st),
-                      'hd_groupnorm_relu_split')
-                conv.bind(None, B, T, 1, dst, inp_split=act, impl='auto', **res).run(st)
-            else:
-                check(lib.hd_groupnorm_stats(fptr(src), fptr(g), fptr(b), fptr(gain), fptr(offset), B, T, Cc, GN_GROUPS, GN_EPS, st),
-                      'hd_groupnorm_stats')
-                conv.bind(src, B, T, 1, dst, pre=(gain, offset, Cc, 1), impl='auto', **res).run(st)
-        if save:
-            saved.append((cur, mid))
-        cur = out
-    return cur, saved
-
-
 def fmovie_backward(model, saved, g):
     """Gradients of f_movie: returns (dx, [per block: dgamma1, dbeta1, dW1, db1, dgamma2, dbeta2, dW2, db2])."""
     st = current_stream()
@@ -139,10 +107,11 @@ def fmovie_backward(model, saved, g):
     gain, offset = torch.empty((B, Cc), dtype=F32, device=dev), torch.empty((B, Cc), dtype=F32, device=dev)
     pg, pb = torch.empty((B, Cc), dtype=F32, device=dev), torch.empty((B, Cc), dtype=F32, device=dev)
     dact = torch.empty((B, T, Cc), dtype=F32, device=dev)
-    grads = [None] * len(model.fm_blocks)
+    blocks = model.fmovie.blocks
+    grads = [None] * len(blocks)
     g = g.contiguous()
-    for i in range(len(model.fm_blocks) - 1, -1, -1):
-        blk = model.fm_blocks[i]
+    for i in range(len(blocks) - 1, -1, -1):
+        blk = blocks[i]
         x, mid = saved[i]
         gr = {}
         dmid = torch.empty((B, T, Cc), dtype=F32, device=dev)
@@ -158,7 +127,7 @@ def fmovie_backward(model, saved, g):
             db = torch.empty(Cc, dtype=F32, device=dev)
             _col_sum(gin, BT, Cc, Cc, db, st)
             # d relu(gn(src)) = conv(gin, W'); then the GroupNorm + ReLU backward (+ the block's residual gradient for gn1)
-            dgrad_op(model.fm_bwd[i][k - 1], gin, B, T, 1, 3, 1, dact, one_pass=model.one_pass).run(st)
+            dgrad_op(blk['conv%d' % k].bwd, gin, B, T, 1, 3, 1, dact, one_pass=model.one_pass).run(st)
             check(lib.hd_groupnorm_relu_backward(fptr(src), fptr(gam), fptr(bet), fptr(dact), fptr(addend) if addend is not None else None,
                                                  fptr(gout), fptr(pg), fptr(pb), B, T, Cc, GN_GROUPS, GN_EPS, 1, st),
                   'hd_groupnorm_relu_backward')
@@ -174,34 +143,12 @@ def fmovie_backward(model, saved, g):
 # ------------------------------------------------------------------------------------------------------------------------------------
 # IEF heads
 # ------------------------------------------------------------------------------------------------------------------------------------
-def ief_head_forward(model, head, phi_split, N, start, start_ld, out, out_ld, st):
-    """hmr_ief for one head with the kernels of IEFPlan's fast path.  Returns what the backward needs besides the head's start:
-    (h1 [3,N,1024], h2 [3,N,1024], the outputs of stages 0 and 1 [N,d])."""
-    dev = start.device
-    d = head['d']
-    P = torch.empty((N, 1024), dtype=F32, device=dev)
-    h1 = torch.empty((3, N, 1024), dtype=F32, device=dev)
-    h2 = torch.empty((3, N, 1024), dtype=F32, device=dev)
-    h1s = (torch.empty((N, 1024), dtype=torch.float16, device=dev), torch.empty((N, 1024), dtype=torch.float16, device=dev))
-    head['fc1_phi'].bind(None, N, 1, 1, P, inp_split=phi_split, impl='auto').run(st)
-    mids = [torch.empty((N, d), dtype=F32, device=dev) for _ in range(2)]
-    ins = [(start, start_ld), (mids[0], d), (mids[1], d)]
-    for s in range(3):
-        prev, pld = ins[s]
-        check(lib.hd_ief_fc1_theta(fptr(P), fptr(prev), pld, fptr(head['W1t']), d, 1024, _vp(h1s[0]), _vp(h1s[1]), fptr(h1[s]), N, st),
-              'hd_ief_fc1_theta')
-        head['fc2'].bind(None, N, 1, 1, h2[s], inp_split=h1s, impl='auto').run(st)
-        dst, dld = (mids[s], d) if s < 2 else (out, out_ld)
-        check(lib.hd_ief_fc3(fptr(h2[s]), fptr(head['W3']), fptr(head['b3']), fptr(prev), pld, fptr(dst), dld, N, 1024, d, st), 'hd_ief_fc3')
-    return h1, h2, mids[0], mids[1]
-
-
 def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st):
     """Backward of one hmr_ief head.  saved = (h1, h2, start, start_ld, stage-0 output, stage-1 output); g: gradient of the head's
     output (rows of d at stride g_ld).  Accumulates dL/dphi into `dphi`
     (None: written).  Returns (dstart [N, d], [dW1, db1, dW2, db2, dW3, db3], dphi)."""
     dev = phi.device
-    d = head['d']
+    d, feat = head.d, head.feat
     h1, h2, start, start_ld, mid0, mid1 = saved
     ins = [(start, start_ld), (mid0, d), (mid1, d)]
     G = torch.empty((3, N, d), dtype=F32, device=dev)
@@ -213,15 +160,15 @@ def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st):
         if s == 2:
             G[2].copy_(torch.as_strided(g, (N, d), (g_ld, 1)))
         # dpre2 = (g . W3^T) * (h2 > 0);  dpre1 = (dpre2 . W2^T) * (h1 > 0);  dprev = g + dpre1 . W1theta^T
-        check(lib.hd_fc_small_dgrad(fptr(gs), gld, fptr(head['W3t']), 1024, d, fptr(h2[s]), fptr(DP2[s]), N, st), 'hd_fc_small_dgrad')
-        dgrad_op(head['fc2_bwd'], DP2[s], N, 1, 1, 1, 1, DP1[s], one_pass=model.one_pass).run(st)
+        check(lib.hd_fc_small_dgrad(fptr(gs), gld, fptr(head.fc3.bwd.dst), 1024, d, fptr(h2[s]), fptr(DP2[s]), N, st), 'hd_fc_small_dgrad')
+        dgrad_op(head.fc2.bwd, DP2[s], N, 1, 1, 1, 1, DP1[s], one_pass=model.one_pass).run(st)
         check(lib.hd_relu_backward(fptr(h1[s]), fptr(DP1[s]), fptr(DP1[s]), N * 1024, st), 'hd_relu_backward')
         dst = G[s - 1] if s > 0 else dstart
-        check(lib.hd_ief_fc3(fptr(DP1[s]), fptr(head['W1tT']), fptr(model._zeros), fptr(gs), gld, fptr(dst), d, N, 1024, d, st),
+        check(lib.hd_ief_fc3(fptr(DP1[s]), fptr(head.fc1_theta.bwd.dst), fptr(model._zeros), fptr(gs), gld, fptr(dst), d, N, 1024, d, st),
               'hd_ief_fc3')
     kp3, kp1 = _round(3 * N, 32), _round(N, 32)
-    W1, W2, W3 = (torch.empty(p.shape, dtype=F32, device=dev) for p in (head['p'][0], head['p'][2], head['p'][4]))
-    b1, b2, b3 = (torch.empty(p.shape, dtype=F32, device=dev) for p in (head['p'][1], head['p'][3], head['p'][5]))
+    W1, W2, W3 = (torch.empty(shape, dtype=F32, device=dev) for shape in ((feat + d, 1024), (1024, 1024), (1024, d)))
+    b1, b2, b3 = (torch.empty(n, dtype=F32, device=dev) for n in (1024, 1024, d))
     # dP = sum over the stages (fixed order), then the phi part of fc1
     dP = torch.empty((N, 1024), dtype=F32, device=dev)
     check(lib.hd_add_strided(fptr(DP1[0]), 1024, fptr(DP1[1]), 1024, fptr(dP), 1024, N, 1024, st), 'hd_add_strided')
@@ -229,54 +176,29 @@ def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st):
     _col_sum(dP, N, 1024, 1024, b1, st)
     _col_sum(DP2, 3 * N, 1024, 1024, b2, st)
     _col_sum(G, 3 * N, d, d, b3, st)
-    feat = head['feat']
     op = model.one_pass
     _wgrad(_xt([(phi, N, feat)], feat, kp1, st), feat, kp1, [(dP, N, 1024)], 1024, W1, st, op)
     _wgrad(_xt([(t, N, ld) for t, ld in ins], d, kp3, st), d, kp3, [(DP1.view(3 * N, 1024), 3 * N, 1024)], 1024, W1[feat:], st, op)
     _wgrad(_xt([(h1.view(3 * N, 1024), 3 * N, 1024)], 1024, kp3, st), 1024, kp3, [(DP2.view(3 * N, 1024), 3 * N, 1024)], 1024, W2, st, op)
     _wgrad(_xt([(h2.view(3 * N, 1024), 3 * N, 1024)], 1024, kp3, st), 1024, kp3, [(G.view(3 * N, d), 3 * N, d)], d, W3, st, op)
     out = torch.empty((N, feat), dtype=F32, device=dev) if dphi is None else dphi
-    dgrad_op(head['fc1_bwd'], dP, N, 1, 1, 1, 1, out, res=dphi, one_pass=op).run(st)
+    dgrad_op(head.fc1_phi.bwd, dP, N, 1, 1, 1, 1, out, res=dphi, one_pass=op).run(st)
     return dstart, [W1, b1, W2, b2, W3, b3], out
 
 
-def regress_forward(model, keys, tiled, phi, start):
-    """call_hmr_ief over phi (N,2048) from start (N,85), or the tiled (1,85) when `tiled`: the main head, then the delta heads `keys`
-    from its pose.  Returns ((theta, deltas...), saved) with saved = [the main head's start (N,85), then per head h1, h2 and the
-    outputs of stages 0 and 1]."""
+def regress_plan(model, keys, tiled, phi, start):
+    """call_hmr_ief over phi (N,2048) from start (N,85), or the tiled (1,85) when `tiled`, through a keep=True IEFPlan built for this
+    call: the main head, then the delta heads `keys` from its pose.  Returns ((theta, deltas...), the start rows (N,85), the plan)."""
     N = phi.shape[0]
-    st = current_stream()
-    dev = phi.device
-    phi_split = (torch.empty((N, 2048), dtype=torch.float16, device=dev), torch.empty((N, 2048), dtype=torch.float16, device=dev))
-    check(lib.hd_split_f16(fptr(phi), _vp(phi_split[0]), _vp(phi_split[1]), phi.numel(), st), 'hd_split_f16')
     s0 = start.expand(N, 85).contiguous() if tiled else start
-    theta = torch.empty((N, 85), dtype=F32, device=dev)
-    saved = [s0] + list(ief_head_forward(model, model.ief['main'], phi_split, N, s0, 85, theta, 85, st))
-    outs = [theta]
-    for k in keys:
-        o = torch.empty((N, 85), dtype=F32, device=dev)
-        check(lib.hd_ief_delta_init(fptr(theta), fptr(o), 85, N, st), 'hd_ief_delta_init')
-        pose = torch.as_strided(theta, (N, 72), (85, 1), theta.storage_offset() + 3)
-        saved += ief_head_forward(model, model.ief[k], phi_split, N, pose, 85, torch.as_strided(o, (N, 72), (85, 1), o.storage_offset() + 3),
-                                  85, st)
-        outs.append(o)
-    return tuple(outs), saved
+    plan = IEFPlan(model.ief, N, 3, list(keys), keep=True)
+    theta, deltas = plan.run(phi, s0)
+    return (theta,) + tuple(deltas[k] for k in keys), s0, plan
 
 
 # ------------------------------------------------------------------------------------------------------------------------------------
 # fc2_res
 # ------------------------------------------------------------------------------------------------------------------------------------
-def hal_forward(model, x):
-    N = x.shape[0]
-    st = current_stream()
-    h1, h2, out = (torch.empty((N, 2048), dtype=F32, device=x.device) for _ in range(3))
-    L = model.hal
-    L['fc1'].bind(x, N, 1, 1, h1, impl='auto').run(st)
-    L['fc2'].bind(h1, N, 1, 1, h2, impl='auto').run(st)
-    L['fc3'].bind(h2, N, 1, 1, out, res=x, res_geom=(2048, 1, 1, 1), impl='auto').run(st)
-    return out, (h1, h2)
-
-
 def hal_backward(model, x, h1, h2, g):
     N = x.shape[0]
     st = current_stream()
@@ -291,13 +213,13 @@ def hal_backward(model, x, h1, h2, g):
         _col_sum(gin, N, 2048, 2048, b, st)
         grads = [W, b] + grads
         if name == 'fc3':
-            dgrad_op(L['fc3_bwd'], g, N, 1, 1, 1, 1, dh2, one_pass=model.one_pass).run(st)
+            dgrad_op(L.fc3.bwd, g, N, 1, 1, 1, 1, dh2, one_pass=model.one_pass).run(st)
             check(lib.hd_relu_backward(fptr(h2), fptr(dh2), fptr(dh2), N * 2048, st), 'hd_relu_backward')
         elif name == 'fc2':
-            dgrad_op(L['fc2_bwd'], dh2, N, 1, 1, 1, 1, dh1, one_pass=model.one_pass).run(st)
+            dgrad_op(L.fc2.bwd, dh2, N, 1, 1, 1, 1, dh1, one_pass=model.one_pass).run(st)
             check(lib.hd_relu_backward(fptr(h1), fptr(dh1), fptr(dh1), N * 2048, st), 'hd_relu_backward')
         else:
-            dgrad_op(L['fc1_bwd'], dh1, N, 1, 1, 1, 1, dx, res=g, one_pass=model.one_pass).run(st)
+            dgrad_op(L.fc1.bwd, dh1, N, 1, 1, 1, 1, dx, res=g, one_pass=model.one_pass).run(st)
     return dx, grads
 
 
@@ -309,9 +231,10 @@ class FMovieFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, x, *params):
-        out, saved = fmovie_forward(model, x, True)
+        plan = FMoviePlan(model.fmovie, x.shape[0], x.shape[1], keep=True)
+        out = plan.run(x)
         ctx.model = model
-        ctx.save_for_backward(*[t for pair in saved for t in pair])
+        ctx.save_for_backward(*[t for pair in plan.saved for t in pair])
         return out
 
     @staticmethod
@@ -330,11 +253,11 @@ class RegressFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, keys, tiled, phi, start, *params):
-        outs, saved = regress_forward(model, keys, tiled, phi, start)
+        outs, s0, plan = regress_plan(model, keys, tiled, phi, start)
         # Everything the backward reads goes through save_for_backward (theta, an output, included): no tensor or view of one is held on
         # ctx, so an unused graph is freed with its outputs and retain_graph works.  The delta heads' start is theta's pose, rebuilt there.
         ctx.model, ctx.keys, ctx.tiled = model, keys, tiled
-        ctx.save_for_backward(phi, outs[0], *saved)
+        ctx.save_for_backward(phi, outs[0], s0, *[t for head in plan.saved for t in head])
         ctx.set_materialize_grads(False)
         return outs
 
@@ -360,12 +283,12 @@ class RegressFunction(torch.autograd.Function):
             if dd is None:
                 continue
             dd = dd.contiguous()
-            ds, hg, dphi = ief_head_backward(model, model.ief[k], phi, N, state[1 + i], torch.as_strided(dd, (N, 72), (85, 1), dd.storage_offset() + 3),
-                                             85, dphi, st)
+            ds, hg, dphi = ief_head_backward(model, model.ief.deltas[k], phi, N, state[1 + i],
+                                             torch.as_strided(dd, (N, 72), (85, 1), dd.storage_offset() + 3), 85, dphi, st)
             head_grads[k] = hg
             check(lib.hd_add_strided(fptr(gm[:, 3:]), 85, fptr(ds), 72, fptr(gm[:, 3:]), 85, N, 72, st), 'hd_add_strided')
             check(lib.hd_add_strided(fptr(gm[:, 75:]), 85, fptr(dd[:, 75:]), 85, fptr(gm[:, 75:]), 85, N, 10, st), 'hd_add_strided')
-        dstart, hg, dphi = ief_head_backward(model, model.ief['main'], phi, N, state[0], gm, 85, dphi, st)
+        dstart, hg, dphi = ief_head_backward(model, model.ief.main, phi, N, state[0], gm, 85, dphi, st)
         head_grads['main'] = hg
         if ctx.tiled:
             ds = torch.empty((1, 85), dtype=F32, device=dev)
@@ -382,7 +305,8 @@ class HalFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, x, *params):
-        out, (h1, h2) = hal_forward(model, x)
+        h1, h2, out = (torch.empty_like(x) for _ in range(3))
+        model.hal.run(x, h1, h2, out)
         ctx.model = model
         ctx.save_for_backward(x, h1, h2)
         return out
@@ -484,9 +408,9 @@ class TemporalModel(TrainableModule):
     forward (detected by its version counter).  Under torch.no_grad(), or when nothing requires grad, the methods run the inference
     kernels and build no graph.
 
-    The forward follows HMMREngine's default configuration (impl 'auto'): f_movie takes the same branch as FMoviePlan (fused GroupNorm
-    + split for T*64 <= 1280, GroupNorm statistics + conv prologue otherwise), so it is bit-identical to the engine at every T.  The IEF
-    heads run IEFPlan's fast-head kernels, whose saved h1 / h2 the backward reads.
+    The forward is HMMREngine's in its default configuration (impl 'auto'): the engine's packs (PackedFMovie, PackedIEF, PackedHal) over
+    the parameters, run by FMoviePlan and IEFPlan built per call with keep=True (they keep the activations the backward reads) and by
+    PackedHal.run, so it is bit-identical to the engine at every T.
 
     The backward's GEMMs follow `config.grad_precision` when the config has one (objective.TrainConfig): 'fp32' (3xTF32, the default)
     or 'tf32' (1xTF32, nets.GRAD_PRECISIONS)."""
@@ -516,50 +440,33 @@ class TemporalModel(TrainableModule):
 
     # ---------------------------------------------------------------- packing
     def _build(self):
-        P = self.param
-        self.fm_blocks, self.fm_bwd = [], []
-        self.has_fmovie = 'AZ_FC_block2_conv1block_0/weights' in self.names
-        Cc = 2048
-        if self.has_fmovie:
-            for i in range(self.num_conv_layers):
-                n = fmovie_names(i)
-                blk = {'gn1': (P(n[0]).data, P(n[1]).data), 'gn2': (P(n[4]).data, P(n[5]).data)}
-                bwd = []
-                for k, wn, bn in ((1, n[2], n[3]), (2, n[6], n[7])):
-                    Cc = P(wn).shape[2]
-                    blk['conv%d' % k] = PackedConv(P(wn).data, self.device, post_shift=P(bn).data, pad=(1, 0), tc='auto')
-                    bwd.append(BackwardDataPack(P(wn).data, 3, Cc, Cc))
-                    self._fwd_packs.append((wn, blk['conv%d' % k]))
-                    self._bwd_packs.append((wn, bwd[-1]))
-                self.fm_blocks.append(blk)
-                self.fm_bwd.append(bwd)
-        self.ief = {}
+        """The engine's packs over the parameters, read in place, each layer with its input-gradient operand `bwd` beside it."""
+        w = {n: self.param(n).data for n in self.names}
+        f32 = dict(dtype=F32, device=self.device)
+        self.fmovie = PackedFMovie(w, self.device, self.num_conv_layers, tc='auto') if 'AZ_FC_block2_conv1block_0/weights' in w else None
+        self.ief = PackedIEF(w, self.device, delta_t_values=self.delta_keys, tc='auto')
+        self.hal = PackedHal(w, self.device, tc='auto') if 'fc2_res/fc1/weights' in w else None
+
+        def layer(name, conv):                                 # a PackedConv whose input gradient is a BackwardDataPack
+            conv.bwd = BackwardDataPack(conv.w_kn, conv.KH, conv.Cin, conv.Cout)
+            self._fwd_packs.append((name, conv))
+            self._bwd_packs.append((name, conv.bwd))
+        for i, blk in enumerate(self.fmovie.blocks if self.fmovie is not None else []):
+            layer(fmovie_names(i)[2], blk['conv1'])
+            layer(fmovie_names(i)[6], blk['conv2'])
         for dt in [0] + self.delta_keys:
             n = ief_names(dt)
-            W1, b1, W2, b2, W3, b3 = (P(x).data for x in n)
-            d = W3.shape[1]
-            feat = W1.shape[0] - d
-            h = {'d': d, 'feat': feat, 'p': [P(x) for x in n], 'W1t': W1[feat:], 'W3': W3, 'b3': b3,
-                 'fc1_phi': PackedConv(W1[:feat], self.device, post_shift=b1, tc='auto'),
-                 'fc1_bwd': BackwardDataPack(W1, 1, feat, 1024),
-                 'fc2': PackedConv(W2, self.device, post_shift=b2, post_relu=True, tc='auto'),
-                 'fc2_bwd': BackwardDataPack(W2, 1, 1024, 1024),
-                 'W3t': torch.empty((d, 1024), dtype=F32, device=self.device),       # fc3^T  (input gradient of fc3)
-                 'W1tT': torch.empty((1024, d), dtype=F32, device=self.device)}      # fc1's theta rows, transposed
-            self._fwd_packs += [(n[0], h['fc1_phi']), (n[2], h['fc2'])]
-            self._bwd_packs += [(n[0], h['fc1_bwd']), (n[2], h['fc2_bwd']), (n[4], TransposedCopy(W3, h['W3t'])),
-                                (n[0], TransposedCopy(h['W1t'], h['W1tT']))]
-            self.ief['main' if dt == 0 else dt] = h
-        self._zeros = torch.zeros(96, dtype=F32, device=self.device)
-        self.hal = None
-        if 'fc2_res/fc1/weights' in self.names:
-            self.hal = {}
+            h = self.ief.main if dt == 0 else self.ief.deltas[dt]
+            layer(n[0], h.fc1_phi)
+            layer(n[2], h.fc2)
+            h.fc3.bwd = TransposedCopy(h.fc3.w_kn, torch.empty((h.d, 1024), **f32))                  # fc3^T  (input gradient of fc3)
+            h.fc1_theta.bwd = TransposedCopy(h.fc1_theta.w_kn, torch.empty((1024, h.d), **f32))      # fc1's theta rows, transposed
+            self._fwd_packs.append((n[4], h.fc3))
+            self._bwd_packs += [(n[4], h.fc3.bwd), (n[0], h.fc1_theta.bwd)]
+        if self.hal is not None:
             for i in (1, 2, 3):
-                wn, bn = HAL_NAMES[2 * i - 2], HAL_NAMES[2 * i - 1]
-                self.hal['fc%d' % i] = PackedConv(P(wn).data, self.device, post_shift=P(bn).data, post_relu=i < 3, tc='auto')
-                self.hal['fc%d_bwd' % i] = BackwardDataPack(P(wn).data, 1, 2048, 2048)
-                self._fwd_packs.append((wn, self.hal['fc%d' % i]))
-                self._bwd_packs.append((wn, self.hal['fc%d_bwd' % i]))
+                layer(HAL_NAMES[2 * i - 2], getattr(self.hal, 'fc%d' % i))
+        self._zeros = torch.zeros(96, **f32)
         self._packs_written(self.device)
 
     # ---------------------------------------------------------------- forward API
@@ -574,7 +481,7 @@ class TemporalModel(TrainableModule):
     def temporal_encode(self, phi):
         """az_fc2_groupnorm ("f_movie"): (B,T,2048) -> (B,T,2048)."""
         self._check_input(phi, 'temporal_encode')
-        if not self.has_fmovie:
+        if self.fmovie is None:
             raise _lib.HDError('no f_movie weights were loaded')
         self.sync_packs()
         phi = phi.contiguous()
@@ -582,7 +489,7 @@ class TemporalModel(TrainableModule):
         if self._grad_on(names, phi):
             return FMovieFunction.apply(self, phi, *[self.param(n) for n in names])
         with torch.no_grad():
-            return fmovie_forward(self, phi.detach(), False)[0]
+            return FMoviePlan(self.fmovie, phi.shape[0], phi.shape[1]).run(phi.detach())
 
     def hallucinate(self, phi):
         """fc2_res: (B,T,2048) -> (B,T,2048)   (pred_mode='hal')."""
@@ -594,7 +501,8 @@ class TemporalModel(TrainableModule):
         if self._grad_on(HAL_NAMES, x):
             return HalFunction.apply(self, x, *[self.param(n) for n in HAL_NAMES]).view(phi.shape)
         with torch.no_grad():
-            return hal_forward(self, x.detach())[0].view(phi.shape)
+            x = x.detach()
+            return self.hal.run(x, torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)).view(phi.shape)
 
     def regress(self, feats, omega_start=None, delta_keys=None):
         """call_hmr_ief: feats (N,2048) -> (omega (N,85), {dt: (N,85)}).  Starts from mean_param (tiled) unless omega_start (N,85) is
@@ -602,7 +510,7 @@ class TemporalModel(TrainableModule):
         self._check_input(feats, 'regress')
         keys = tuple(self.delta_keys) if delta_keys is None else tuple(sorted(int(k) for k in delta_keys if int(k) != 0))
         for k in keys:
-            if k not in self.ief:
+            if k not in self.ief.deltas:
                 raise _lib.HDError('no IEF head for delta_t %d' % k)
         self.sync_packs()
         feats = feats.contiguous().reshape(-1, 2048)
@@ -616,7 +524,7 @@ class TemporalModel(TrainableModule):
             outs = RegressFunction.apply(self, keys, tiled, feats, start, *[self.param(n) for n in names])
         else:
             with torch.no_grad():
-                outs = regress_forward(self, keys, tiled, feats.detach(), start.detach())[0]
+                outs = regress_plan(self, keys, tiled, feats.detach(), start.detach())[0]
         return outs[0], {k: outs[1 + i] for i, k in enumerate(keys)}
 
     def predict_from_features(self, phi, smpl, single_frame=False):
@@ -659,12 +567,13 @@ class TemporalModel(TrainableModule):
             self.sync_packs()
             if phi is not None:
                 B, T, Cc = phi.shape
-                _, saved = fmovie_forward(self, phi.contiguous(), True)
+                plan = FMoviePlan(self.fmovie, B, T, keep=True)
+                plan.run(phi.contiguous())
                 gain, offset = torch.empty((B, Cc), dtype=F32, device=self.device), torch.empty((B, Cc), dtype=F32, device=self.device)
                 a = torch.empty((Cc, B * T), dtype=F32, device=self.device)
-                for i, (x, mid) in enumerate(saved):
+                for i, (x, mid) in enumerate(plan.saved):
                     for k, src in ((1, x), (2, mid)):
-                        g, b = self.fm_blocks[i]['gn%d' % k]
+                        g, b = self.fmovie.blocks[i]['gn%d' % k]
                         check(lib.hd_groupnorm_stats(fptr(src), fptr(g), fptr(b), fptr(gain), fptr(offset), B, T, Cc, GN_GROUPS, GN_EPS, st),
                               'hd_groupnorm_stats')
                         check(lib.hd_im2col_t(fptr(src), B, T, Cc, 1, 0, fptr(gain), fptr(offset), 1, fptr(a), B * T, B * T, st), 'hd_im2col_t')
@@ -673,14 +582,15 @@ class TemporalModel(TrainableModule):
                 keys = tuple(self.delta_keys) if delta_keys is None else tuple(sorted(int(k) for k in delta_keys if int(k) != 0))
                 tiled = omega_start is None
                 start = self.param('mean_param') if tiled else omega_start.contiguous()
-                _, saved = regress_forward(self, keys, tiled, feats.contiguous(), start.detach())
-                for j, name in enumerate(['main'] + ['d%d' % k for k in keys]):
-                    h1, h2 = saved[1 + 4 * j], saved[2 + 4 * j]
+                plan = regress_plan(self, keys, tiled, feats.contiguous(), start.detach())[2]
+                for name, (h1, h2, _, _) in zip(['main'] + ['d%d' % k for k in keys], plan.saved):
                     for s in range(3):
                         out['%s.s%d.fc1' % (name, s)] = (h1[s] > 0).cpu()
                         out['%s.s%d.fc2' % (name, s)] = (h2[s] > 0).cpu()
             if hal is not None:
-                _, (h1, h2) = hal_forward(self, hal.contiguous())
+                x = hal.contiguous()
+                h1, h2 = torch.empty_like(x), torch.empty_like(x)
+                self.hal.run(x, h1, h2, torch.empty_like(x))
                 out['hal.fc1'], out['hal.fc2'] = (h1 > 0).cpu(), (h2 > 0).cpu()
         return out
 

@@ -138,7 +138,7 @@ def test_grads_match_oracle(weights, model, BT, scale):
     assert len(relaxed) <= len(names) // 4, relaxed
 
 
-def test_device_packing_equals_host_packing(engine, model, weights):
+def test_device_packing_of_engine_and_model_equals_host_packing(engine, model, weights):
     """Every tensor-core pack of an engine (ResNet units, the gather and the plane conv1, f_movie, the IEF heads, fc2_res, the SMPL blend
     and dc GEMMs), of the temporal model's forward, and a tc3 / tc1 TF32 pack, as hd_pack_weight writes them on the device, equal the
     numpy restatement (oracle/pack_ref.py) byte for byte."""
@@ -174,12 +174,12 @@ def test_device_packing_equals_host_packing(engine, model, weights):
     layers += [(engine.smpl.blend, None, 'f16'), (engine.smpl.grad_state()[2], None, 'tf32')]
     for tc in ('tc3', 'tc1'):
         layers.append((PackedConv(weights['single_view_ief/3D_module/fc2/weights'], torch.device('cuda'), tc=tc), None, 'tf32'))
-    for blk in model.fm_blocks:
+    for blk in model.fmovie.blocks:
         layers += [(blk['conv1'], None, 'f16'), (blk['conv2'], None, 'f16')]
-    for h in model.ief.values():
-        layers += [(h['fc1_phi'], None, 'f16'), (h['fc2'], None, 'f16')]
-    layers += [(model.hal['fc%d' % k], None, 'f16') for k in (1, 2, 3)]
-    assert len(layers) == 1 + 52 + 6 + 9 + 3 + 2 + 2 + 6 + 6 + 3
+    for h in [model.ief.main] + list(model.ief.deltas.values()):
+        layers += [(h.fc1_phi, None, 'f16'), (h.fc2, None, 'f16'), (h.fc3, None, 'f16')]
+    layers += [(getattr(model.hal, 'fc%d' % k), None, 'f16') for k in (1, 2, 3)]
+    assert len(layers) == 1 + 52 + 6 + 9 + 3 + 2 + 2 + 6 + 9 + 3
     torch.cuda.synchronize()
     for pc, src, kind in layers:
         assert pc.tc == kind

@@ -1,5 +1,7 @@
 """Host-side wiring of the ResNet layer plan checked WITHOUT a GPU: device allocations and library calls are stubbed, the descriptors
 the plan fills are real.  Catches plan-logic mistakes (buffer roles, dead outputs, epilogue subsampling, launch counts) on the CPU."""
+import ctypes as C
+
 import numpy as np
 import pytest
 import torch
@@ -132,6 +134,48 @@ def test_fmovie_and_ief_plan_wiring(fake_device):
         assert view.data_ptr() == ief.delta_all.data_ptr() + (i * 85 + 3) * 4 and ops[1][2] == 2 * 85 and ops[3][4] == 2 * 85
         assert ops[3][5].d == 72
     assert ief.main_ops[3][5].d == 85
+    assert all(op[4] is None for op in ief.main_ops if op[0] == 'fc1t')             # no fp32 h1
+    assert {op[6].data_ptr() for op in ief.main_ops if op[0] == 'fc3'} == {ief.h2.data_ptr()}
+
+    # keep=True (training): the same launches over per-block buffers of their own, and `saved` = [(block input, conv1 output)], in both
+    # f_movie branches (T = 25: T*64 > 1280, GroupNorm statistics + prologue)
+    def fields(d):
+        return tuple(getattr(d, f) for f, t in d._fields_ if t is not C.c_void_p)
+    for TT in (T, 25):
+        fm = nets.FMoviePlan(nets.PackedFMovie(w, 'cpu', 3, tc='auto'), B, TT, 'auto')
+        fk = nets.FMoviePlan(fm.p, B, TT, 'auto', keep=True)
+        x = torch.zeros((B, TT, 2048))
+        fm._bind(x)
+        fk._bind(x)
+        assert [s[0] for s in fk.steps] == [s[0] for s in fm.steps] == (['gns', 'conv'] if TT == T else ['gn', 'conv']) * 6
+        ck, cf = [s[1].d for s in fk.steps if s[0] == 'conv'], [s[1].d for s in fm.steps if s[0] == 'conv']
+        assert [fields(d) for d in ck] == [fields(d) for d in cf]
+        assert len({d.out for d in ck} | {x.data_ptr()}) == 7                          # three conv1 outputs, three block outputs
+        assert [(a.data_ptr(), m.data_ptr()) for a, m in fk.saved] == [(x.data_ptr(), ck[0].out), (ck[1].out, ck[2].out),
+                                                                        (ck[3].out, ck[4].out)]
+        assert [d.res for d in ck[1::2]] == [x.data_ptr(), ck[1].out, ck[3].out] and fk.out.data_ptr() == ck[5].out
+        if TT == 25:
+            assert [d.in_ for d in ck] == [x.data_ptr(), ck[0].out, ck[1].out, ck[2].out, ck[3].out, ck[4].out]
+    # IEF keep=True: per stage an fp32 h1 and an h2 of its own; stages 0 and 1 write separate outputs that feed the next stage; the delta
+    # heads write (N, 85) outputs of their own
+    ik = nets.IEFPlan(ief.p, N, 3, None, 'auto', keep=True)
+    ik._bind(phi, theta0)
+    assert ik.num_launches == ief.num_launches and not hasattr(ik, 'delta_all')
+    for j, (ops, d) in enumerate([(ik.main_ops, 85)] + [(ik.delta_ops[dt], 72) for dt in ik.delta_keys]):
+        assert [op[0] for op in ops] == kinds
+        h1, h2, out0, out1 = ik.saved[j]
+        assert h1.shape == h2.shape == (3, N, 1024) and out0.shape == out1.shape == (N, d)
+        fc1t, fc2, fc3 = ops[1::3], ops[2::3], ops[3::3]
+        assert [op[4].data_ptr() for op in fc1t] == [h1[s].data_ptr() for s in range(3)]
+        assert [op[1].d.out for op in fc2] == [op[6].data_ptr() for op in fc3] == [h2[s].data_ptr() for s in range(3)]
+        state = ik.theta if j == 0 else ik.delta_out[ik.delta_keys[j - 1]][:, 3:75]
+        assert [op[3].data_ptr() for op in fc3] == [out0.data_ptr(), out1.data_ptr(), state.data_ptr()]
+        assert [op[1].data_ptr() for op in fc1t] == [op[1].data_ptr() for op in fc3]
+        assert [op[1].data_ptr() for op in fc1t[1:]] == [out0.data_ptr(), out1.data_ptr()]
+        assert [op[2] for op in fc1t] == [op[2] for op in fc3] == [85, d, d] and [op[4] for op in fc3] == [d, d, 85]
+    assert ik.main_ops[1][1].data_ptr() == theta0.data_ptr()
+    assert all(ik.delta_out[dt].shape == (N, 85) and ik.delta_out[dt].is_contiguous() for dt in ik.delta_keys)
+    assert len({t.data_ptr() for s in ik.saved for t in s}) == 4 * 3
 
 
 @pytest.mark.parametrize('dense', [False, True])

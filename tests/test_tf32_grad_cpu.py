@@ -197,7 +197,7 @@ def _pack(shape, KH, Cin, Cout):
 
 
 @pytest.mark.parametrize('gp', ['fp32', 'tf32'])
-def test_temporal_and_dpose_backward_descriptors(rec_device, gp):
+def test_temporal_and_dpose_backward_descriptors_from_layer_packs(rec_device, gp):
     """f_movie, an IEF head, fc2_res and D_pose: every backward GEMM (data gradients and weight gradients) in the model's mode, and the
     weight gradients' B operand written as a TF32 head alone (hd_transpose_split mode 1, lo NULL) under 'tf32'."""
     from human_dynamics_b200 import adversarial, trainable
@@ -218,22 +218,25 @@ def test_temporal_and_dpose_backward_descriptors(rec_device, gp):
         rec.calls.clear()
     # f_movie (3 blocks of two 3x1 convs): per conv one weight gradient and one data gradient
     z = lambda *s: torch.zeros(s)                                # noqa: E731
-    model = types.SimpleNamespace(one_pass=one, fm_blocks=[{'gn1': (z(Cc), z(Cc)), 'gn2': (z(Cc), z(Cc))} for _ in range(3)],
-                                  fm_bwd=[[_pack((3, 1, Cc, Cc), 3, Cc, Cc) for _ in range(2)] for _ in range(3)])
+    layer = lambda bwd: types.SimpleNamespace(bwd=bwd)           # noqa: E731
+    blocks = [{'gn1': (z(Cc), z(Cc)), 'gn2': (z(Cc), z(Cc)), 'conv1': layer(_pack((3, 1, Cc, Cc), 3, Cc, Cc)),
+               'conv2': layer(_pack((3, 1, Cc, Cc), 3, Cc, Cc))} for _ in range(3)]
+    model = types.SimpleNamespace(one_pass=one, fmovie=types.SimpleNamespace(blocks=blocks))
     rec.calls.clear()
     trainable.fmovie_backward(model, [(z(B, T, Cc), z(B, T, Cc))] * 3, z(B, T, Cc))
     check(3 * 2 * 2)
     # one IEF head: fc2's and fc1's data gradients, four weight-gradient GEMMs
     feat, d = 64, 85
-    head = {'d': d, 'feat': feat, 'p': [z(feat + d, 1024), z(1024), z(1024, 1024), z(1024), z(1024, d), z(d)],
-            'W3t': z(d, 1024), 'W1tT': z(1024, d), 'fc2_bwd': _pack((1024, 1024), 1, 1024, 1024),
-            'fc1_bwd': _pack((feat + d, 1024), 1, feat, 1024)}
+    head = types.SimpleNamespace(d=d, feat=feat, fc1_phi=layer(_pack((feat, 1024), 1, feat, 1024)),
+                                 fc1_theta=layer(types.SimpleNamespace(dst=z(1024, d))), fc2=layer(_pack((1024, 1024), 1, 1024, 1024)),
+                                 fc3=layer(types.SimpleNamespace(dst=z(d, 1024))))
     model = types.SimpleNamespace(one_pass=one, _zeros=z(96))
     trainable.ief_head_backward(model, head, z(N, feat), N, (z(3, N, 1024), z(3, N, 1024), z(N, d), d, z(N, d), z(N, d)), z(N, d), d,
                                 None, None)
     check(3 + 1 + 4)
     # fc2_res: three weight gradients, three data gradients
-    model = types.SimpleNamespace(one_pass=one, hal={'fc%d_bwd' % i: _pack((2048, 2048), 1, 2048, 2048) for i in (1, 2, 3)})
+    model = types.SimpleNamespace(one_pass=one, hal=types.SimpleNamespace(**{'fc%d' % i: layer(_pack((2048, 2048), 1, 2048, 2048))
+                                                                            for i in (1, 2, 3)}))
     trainable.hal_backward(model, z(N, 2048), z(N, 2048), z(N, 2048), z(N, 2048))
     check(6)
     # D_pose: fc2's and fc1's data gradients and weight gradients
