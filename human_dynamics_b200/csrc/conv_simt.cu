@@ -258,5 +258,5 @@ extern "C" int hd_conv_gemm(const hd_conv_desc *d, void *stream) { return conv_g
 // [0] producer loop, [1] producer wait-empty (the B loads are issued by a producer thread, inside this loop),
 // [2] consumer loop (wgmma + drains + epilogue), [3] consumer wait-full, [4] epilogue, and of the epilogue: [5] waiting for the
 // residual to land in shared memory, [6] waiting for earlier TMA stores to have read a buffer before it is refilled (with the
-// warpgroup barriers around those waits); [4] - [5] - [6] is arithmetic, staging and issuing stores.  [7..9] are not written.
+// warpgroup barriers around those waits); [4] - [5] - [6] is arithmetic, staging and issuing stores.  [7] and [8] are the kernel's tile: pixels x output channels.
 extern "C" int hd_conv_gemm_profile(const hd_conv_desc *d, void *stream, long long *dbg) { return conv_gemm_impl(d, stream, dbg); }

@@ -22,7 +22,8 @@
 // N tile: 128 for pre-split layers with Cout > 64 that give the SMs enough tiles (wide_n_tile), 64 otherwise.  The 128-wide
 // tile needs 3 x 64 accumulator registers per consumer thread and halves the A gathers and the shared-memory reads per MMA
 // of the 64-wide one.  Pre-split 1x1 layers with K <= 128 (SHORT) flush the running sums once per tile, so they need only the
-// two fragments: 64-wide tiles, two CTAs per SM, one CTA's epilogue running under the other's loads and MMAs.
+// two fragments: 64-wide tiles, two CTAs per SM, one CTA's epilogue running under the other's loads and MMAs.  The root conv1 over
+// the planes (Cout = 64) puts the channels on the wgmma's M side instead (CM, below): 64 channels x 256 pixels.
 //
 // Persistent: grid = min(#tiles, #SMs) (SHORT: 2 x #SMs); each CTA walks tiles blockIdx.x, +gridDim.x, ...  Barrier phases run
 // continuously across tiles, and the producers keep prefetching the next tile's chunks while the consumers run the
@@ -48,7 +49,6 @@ namespace hd {
 namespace {
 
 constexpr int BM = 128;
-constexpr int A_TILE_BYTES = BM * 128;      // 16 KiB: 128 rows x one 128-byte swizzle row (32 tf32 or 64 fp16 of K)
 constexpr int BOX_BYTES = 64 * 128;         // one 64-row weight box (hd_make_weight_tmap)
 constexpr int W_PROD = 8;                   // first producer warp
 // `stage` argument (pre-split layers): which outputs the epilogue stages in shared memory and writes by TMA (launch_tc)
@@ -59,34 +59,46 @@ using namespace ptx;
 // SHORT: pre-split layers with K <= PCH chunks (K <= 128), two CTAs per SM.  The running sums flush exactly once per tile, so the
 // flushed fragment itself holds them; the CTA has one operand stage, and each warpgroup's residual slot doubles as its output
 // staging.
-template <bool SPLIT, bool HALF, bool ASPLIT, int BN, bool RES = false, bool SHORT = false>
+//
+// CM (channels on M, Cout = 64): the tile is 64 output channels x 256 pixels and computes the transpose, D^T = W^T A^T.  The
+// weight box is the wgmma A operand (m64) and consumer warpgroup g's 128 pixel rows of the A tile its B operand (n128).  A 64-wide
+// K chunk (SPLIT) then costs the shared-memory port 144 KB of wgmma reads and 80 KB of writes for twice the products of the 128 x 64
+// tile's 96 + 48 KB (DESIGN.md 4.1).  Each output element gets the same products in the same K order as on the 128 x 64 tile.
+template <bool SPLIT, bool HALF, bool ASPLIT, int BN, bool RES = false, bool SHORT = false, bool CM = false>
 struct Cfg {
   static_assert(BN == 64 || (BN == 128 && HALF && ASPLIT), "128-wide N tiles: pre-split fp16 path only");
   static_assert(!RES || ASPLIT, "residual by TMA: pre-split fp16 path only");
   static_assert(!SHORT || (BN == 64 && HALF && ASPLIT), "two CTAs per SM: 64-wide pre-split fp16 tiles only");
+  static_assert(!CM || (BN == 64 && HALF && ASPLIT && !RES && !SHORT), "channels on M: 64-channel pre-split fp16 tiles, no residual");
   static constexpr int CTAS = SHORT ? 2 : 1;                    // CTAs per SM (__launch_bounds__, persistent grid)
-  static constexpr int PROD_THREADS = BN == 128 || SHORT ? 128 : 256;
+  static constexpr int TM = CM ? 256 : BM;                      // pixel rows of a tile (of the A tile in shared memory)
+  static constexpr int A_BYTES = TM * 128;                      // A head tile: TM rows x one 128-byte swizzle row (32 tf32 or 64 fp16 of K)
+  static constexpr int PROD_THREADS = BN == 128 || SHORT || CM ? 128 : 256;
   static constexpr int NUM_THREADS = 256 + PROD_THREADS;
   static constexpr int ROW_STEP = PROD_THREADS / 8;             // a producer thread's rows: rb + ROW_STEP * i
-  static constexpr int ROWS = BM / ROW_STEP;
-  static constexpr int PROD_REGS = SHORT ? 32 : BN == 128 ? 40 : 104, CONS_REGS = SHORT ? 104 : BN == 128 ? 232 : 152;
-  static_assert(CTAS * (256 * CONS_REGS + PROD_THREADS * PROD_REGS) <= 65536, "setmaxnreg split beyond the register file");
-  static constexpr int NACC = BN / 2;                           // fp32 registers of one m64nBN fragment per thread
+  static constexpr int ROWS = TM / ROW_STEP;
+  static constexpr int PROD_REGS = SHORT ? 32 : CM ? 56 : BN == 128 ? 40 : 104, CONS_REGS = SHORT ? 104 : CM ? 224 : BN == 128 ? 232 : 152;
+  // setmaxnreg only moves registers inside the CTA's launch allocation (65536 / CTAS / NUM_THREADS per thread, in steps of 8): a
+  // split beyond it leaves the consumers' increase waiting forever
+  static_assert(256 * CONS_REGS + PROD_THREADS * PROD_REGS <= NUM_THREADS * (65536 / (CTAS * NUM_THREADS) / 8 * 8),
+                "setmaxnreg split beyond the CTA's registers");
+  static constexpr int NACC = CM ? 64 : BN / 2;                 // fp32 registers of one m64nBN (CM: m64n128) fragment per thread
   // RES: the residual slots do not fit beside three 64 KB stages (BN = 128) or four 48 KB ones plus the output staging (BN = 64).
-  // Residual layers have K <= 512 (<= 8 chunks).
-  static constexpr int STAGES = SHORT ? 1 : BN == 128 ? (RES ? 2 : 3) : (RES ? 3 : 4);
+  // Residual layers have K <= 512 (<= 8 chunks).  CM: two 80 KB stages beside the 2 x 32 KB output staging.
+  static constexpr int STAGES = SHORT ? 1 : CM ? 2 : BN == 128 ? (RES ? 2 : 3) : (RES ? 3 : 4);
   static constexpr int BKE = HALF ? 64 : 32;                    // K elements per chunk (one 128-byte row)
   static constexpr int B_TILE_BYTES = BN * 128;
   // a stage: the A head tile (+ its remainder), then the B head tile (+ its remainder).  !SPLIT keeps the stage counts of the split
   // kernels: the pipeline depth in chunks is the same, each chunk is half the bytes.
-  static constexpr int B_OFFSET = (SPLIT ? 2 : 1) * A_TILE_BYTES;
-  static constexpr int STAGE_BYTES = (SPLIT ? 2 : 1) * (A_TILE_BYTES + B_TILE_BYTES);
+  static constexpr int B_OFFSET = (SPLIT ? 2 : 1) * A_BYTES;
+  static constexpr int STAGE_BYTES = (SPLIT ? 2 : 1) * (A_BYTES + B_TILE_BYTES);
   static constexpr int RES_OFFSET = STAGES * STAGE_BYTES;
   // one warpgroup's 64 rows x BN fp32 residual (BN / 32 TMA boxes); SHORT: also the warpgroup's output staging
   static constexpr int RES_SLOT_BYTES = RES || SHORT ? 64 * BN * 4 : 0;
   static constexpr int STG_OFFSET = SHORT ? RES_OFFSET : RES_OFFSET + 2 * RES_SLOT_BYTES;
-  // ASPLIT: one warpgroup's output staging, two 64-row x 128-byte TMA boxes (64 columns of fp32, or of the fp16 head and remainder)
-  static constexpr int STG_BYTES = ASPLIT ? 2 * BOX_BYTES : 0;
+  // ASPLIT: one warpgroup's output staging, two 64-row x 128-byte TMA boxes (64 columns of fp32, or of the fp16 head and remainder);
+  // CM: four, for the warpgroup's 128 pixel rows
+  static constexpr int STG_BYTES = ASPLIT ? (CM ? 4 : 2) * BOX_BYTES : 0;
   static_assert(!SHORT || STG_BYTES == RES_SLOT_BYTES, "SHORT: the staging buffer is the residual slot");
   static constexpr int BAR_OFFSET = SHORT ? RES_OFFSET + 2 * RES_SLOT_BYTES : STG_OFFSET + 2 * STG_BYTES;
   static constexpr int SMEM_BYTES = BAR_OFFSET + 128 + 1024;    // + alignment slack
@@ -101,14 +113,14 @@ struct RowState {       // R output rows of one producer thread: image index and
   int n[R], iy[R], ix[R];
 };
 
-template <bool SPLIT, int PCH, bool HALF, bool GATHER, bool ASPLIT, int BN, bool RES, bool SHORT>
-__global__ void __launch_bounds__((Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT>::NUM_THREADS), (Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT>::CTAS))
+template <bool SPLIT, int PCH, bool HALF, bool GATHER, bool ASPLIT, int BN, bool RES, bool SHORT, bool CM>
+__global__ void __launch_bounds__((Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT, CM>::NUM_THREADS), (Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT, CM>::CTAS))
 conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap_hi, const __grid_constant__ CUtensorMap tmap_lo,
                     const __grid_constant__ CUtensorMap tmap_res, const __grid_constant__ CUtensorMap tmap_out,
                     const __grid_constant__ CUtensorMap tmap_out_hi, const __grid_constant__ CUtensorMap tmap_out_lo, const int stage) {
-  using C = Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT>;
-  // BN = 128 and SHORT keep the profile's start stamps and summed clocks in memory (hd_conv_gemm_profile): spill-free registers
-  constexpr bool MEM_STAMPS = BN == 128 || SHORT;
+  using C = Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT, CM>;
+  // BN = 128, SHORT and CM keep the profile's start stamps and summed clocks in memory (hd_conv_gemm_profile): spill-free registers
+  constexpr bool MEM_STAMPS = BN == 128 || SHORT || CM;
   constexpr int BKE = C::BKE, PF = C::PF, V = C::V, STAGES = C::STAGES, R = C::ROWS, RS = C::ROW_STEP, NA = C::NACC;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -121,7 +133,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_k = (GATHER ? p.K_pad : p.K) / BKE;   // GATHER: ragged Cin (conv1: K=147 zero-padded to 192)
   const int tiles_n = (p.Cout + BN - 1) / BN;
-  const int num_tiles = ((p.M + BM - 1) / BM) * tiles_n;
+  const int num_tiles = ((p.M + C::TM - 1) / C::TM) * tiles_n;
   const int my_tiles = (num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
   if (threadIdx.x == 0) {
@@ -170,7 +182,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
 
     auto enter_tile = [&](int ti, RowState<R> &rs) {
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-      const int m0 = (tile / tiles_n) * BM;
+      const int m0 = (tile / tiles_n) * C::TM;
       const int hw = p.Ho * p.Wo;
 #pragma unroll
       for (int i = 0; i < R; ++i) {
@@ -190,7 +202,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
       const __half *ihi = reinterpret_cast<const __half *>(p.in_hi);
       const __half *ilo = reinterpret_cast<const __half *>(p.in_lo);
       // SHORT: launch_conv_tc takes it for layers that meet the lean loop's conditions, and the other loops are not compiled
-      if (SHORT || (!p.planes && p.KH * p.KW <= 32 && (long long)p.n_img * p.H * p.W * p.in_ld < (1ll << 31))) {
+      if (SHORT || (!CM && !p.planes && p.KH * p.KW <= 32 && (long long)p.n_img * p.H * p.W * p.in_ld < (1ll << 31))) {
         // Lean loop (on the long-K layers these warps can pace the whole kernel: the general loop below spends instructions per
         // chunk on two integer divisions and 64-bit addressing).  Per tile: one 32-bit
         // element offset and one tap-validity bit mask per row.  Per chunk: (tap, channel) advance incrementally -- a 64-wide chunk
@@ -203,7 +215,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         for (int q = 0; q < total; ++q) {
           if (kc == 0) {
             const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-            const int m0 = (tile / tiles_n) * BM + rb;
+            const int m0 = (tile / tiles_n) * C::TM + rb;
             const int hw = p.Ho * p.Wo;
 #pragma unroll
             for (int i = 0; i < R; ++i) {
@@ -237,7 +249,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
             const bool ok = SHORT ? base[i] >= 0 : (mask[i] >> tap) & 1u;
             const int e = ok ? base[i] + eo : 0;
             cp_async16(a_hi + i * RS * 128, ihi + e, ok ? 16u : 0u);
-            if (SPLIT) cp_async16(a_hi + A_TILE_BYTES + i * RS * 128, ilo + e, ok ? 16u : 0u);
+            if (SPLIT) cp_async16(a_hi + C::A_BYTES + i * RS * 128, ilo + e, ok ? 16u : 0u);
           }
           asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(full_bar(s)) : "memory");
           ci0 += BKE;
@@ -260,7 +272,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         for (int q = 0; q < total; ++q) {
           if (kc == 0) {
             const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-            const int m0 = (tile / tiles_n) * BM + rb;
+            const int m0 = (tile / tiles_n) * C::TM + rb;
             const int hw = p.Ho * p.Wo;
 #pragma unroll
             for (int i = 0; i < R; ++i) {
@@ -288,12 +300,12 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
             const int e = ok ? base[i] + eo : 0;
             // neighbouring output pixels read overlapping 64-byte windows (each 16-byte piece 4x): keep them in L1
             cp_async16_ca(a_hi + i * RS * 128, ihi + e, ok ? 16u : 0u);
-            if (SPLIT) cp_async16_ca(a_hi + A_TILE_BYTES + i * RS * 128, ilo + e, ok ? 16u : 0u);
+            if (SPLIT) cp_async16_ca(a_hi + C::A_BYTES + i * RS * 128, ilo + e, ok ? 16u : 0u);
           }
           asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(full_bar(s)) : "memory");
           if (++kc == num_k) { kc = 0; ++ti; }
         }
-      } else if (!SHORT) {
+      } else if (!SHORT && !CM) {     // CM: launch_conv_f16 takes it only for layers the lean plane loop runs
       RowState<R> rs;
       int kc = 0, ti = 0;
       for (int q = 0; q < total; ++q) {
@@ -310,7 +322,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         const int ci = p.planes ? (j & 3) * 8 : kb - tap * p.Cin + j * 8;
         const int ky = tap / p.KW, kx = tap - ky * p.KW;
         const bool tap_ok = !p.planes || tap < 7;
-        const uint32_t a_hi = smem_base + s * C::STAGE_BYTES, a_lo = a_hi + A_TILE_BYTES;
+        const uint32_t a_hi = smem_base + s * C::STAGE_BYTES, a_lo = a_hi + C::A_BYTES;
 #pragma unroll
         for (int i = 0; i < R; ++i) {
           const int iy = rs.iy[i] + ky, ix = rs.ix[i] + kx;
@@ -401,7 +413,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
       if (prof) t_wait += clock64() - tw0;
       load_b(s, st_ti, st_kc);
       uint8_t *a_hi = smem + s * C::STAGE_BYTES;
-      uint8_t *a_lo = a_hi + A_TILE_BYTES;
+      uint8_t *a_lo = a_hi + C::A_BYTES;
       const int pci = p.pre_scale ? (st_kc * BKE) % p.Cin + j * (4 * V) : 0;
       // row by row (keeps the live set small): prologue affine (+ReLU) on real pixels only, then split every value into a
       // head and a remainder that the tensor core reads exactly (zero-mean rounding):
@@ -519,8 +531,8 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         if (!MEM_STAMPS && prof) t_wait += clock64() - tw0;
         if (MEM_STAMPS && prof) p.dbg[3] += clock64();
         if (ASPLIT) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async (generic proxy) data -> wgmma (async proxy)
-        const uint32_t a_hi = smem_base + s * C::STAGE_BYTES + wg * (64 * 128);
-        const uint32_t a_lo = a_hi + A_TILE_BYTES;
+        const uint32_t a_hi = smem_base + s * C::STAGE_BYTES + wg * (C::TM / 2 * 128);   // the warpgroup's half of the A tile's rows
+        const uint32_t a_lo = a_hi + C::A_BYTES;
         const uint32_t b_hi = smem_base + s * C::STAGE_BYTES + C::B_OFFSET;
         const uint32_t b_lo = b_hi + C::B_TILE_BYTES;
         const uint64_t da_hi = make_smem_desc(a_hi), da_lo = make_smem_desc(a_lo);
@@ -531,7 +543,13 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
 #pragma unroll
         for (int k = 0; k < 4; ++k) {                // K = 8 tf32 / 16 fp16 = 32 bytes per wgmma: advance inside the swizzle row
           const uint64_t adv = (uint64_t)((k * 32) >> 4);
-          if constexpr (BN == 128) {
+          if constexpr (CM) {                         // the transposed products: weights (A) x the warpgroup's 128 pixels (B)
+            if constexpr (SPLIT) {
+              wgmma_m64n128k16_f16(accx, db_hi + adv, da_lo + adv, (kc | k) != 0);
+              wgmma_m64n128k16_f16(accx, db_lo + adv, da_hi + adv, 1u);
+            }
+            wgmma_m64n128k16_f16(acc, db_hi + adv, da_hi + adv, !(group_start && k == 0));
+          } else if constexpr (BN == 128) {
             if constexpr (SPLIT) {
               wgmma_m64n128k16_f16(accx, da_lo + adv, db_hi + adv, (kc | k) != 0);
               wgmma_m64n128k16_f16(accx, da_hi + adv, db_lo + adv, 1u);
@@ -572,7 +590,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
       }
       if (prof) p.dbg[4] -= clock64();                   // the epilogue's clocks, summed in memory (see above)
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-      const int m0 = (tile / tiles_n) * BM, n0 = (tile % tiles_n) * BN;
+      const int m0 = (tile / tiles_n) * C::TM, n0 = (tile % tiles_n) * BN;
       if (RES && prof) p.dbg[5] -= clock64();            // of the epilogue: waiting for the residual
       if (RES) mbar_wait(res_bar(wg), (uint32_t)ti & 1u);
       if (RES && prof) p.dbg[5] += clock64();
@@ -616,7 +634,54 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
         if (p.post2_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
         split_f16x2(a0, a1, hh, ll);
       };
-      if constexpr (ASPLIT) {
+      if constexpr (CM) {
+        // Channels on M: this thread holds channels ch + 8 h of the warpgroup's pixels 8 j + fcol (+ 1), j < 16.  Transposed on
+        // the way in, v goes into the staging buffer as 2 x 2 TMA boxes of 64 pixel rows x 32 fp32 channels (row r at r * 128 B,
+        // its 16-byte piece k at (k ^ (r & 7)) * 16; a thread's pixels all have r & 7 = fcol + e), and leaves by TMA stores.  Every
+        // product and sum is rounded on its own, as on the 128 x 64 tile.  The root conv1 writes the fp32 output alone
+        // (launch_conv_f16 takes this tile for nothing else).
+        const bool st32 = (stage & STAGE_OUT) != 0;
+        uint8_t *stg = smem + C::STG_OFFSET + wg * C::STG_BYTES;
+        const uint32_t stg_a = smem_base + C::STG_OFFSET + wg * C::STG_BYTES;
+        const int r0 = m0 + 128 * wg;
+        const int ch = (warp & 3) * 16 + (lane >> 2);
+        auto acquire = [&]() {   // the staging buffer may be rewritten: its last stores have been read
+          if (prof) p.dbg[6] -= clock64();
+          if (stg_issuer) bulk_wait_read<0>();
+          named_bar_sync(3 + wg, 128);
+          if (prof) p.dbg[6] += clock64();
+        };
+        if (st32) {
+          acquire();
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int c = ch + 8 * h;
+            const float sc = p.post_scale ? __ldg(p.post_scale + c) : 0.f, sh = p.post_shift ? __ldg(p.post_shift + c) : 0.f;
+            uint8_t *cb = stg + (c >> 5) * BOX_BYTES + (c & 3) * 4;
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int r = 8 * (j & 7) + fcol + e;          // row of box 2 (j >> 3) + (c >> 5)
+                float y = sums[4 * j + 2 * h + e];
+                if (p.post_scale) y = __fmul_rn(y, sc);
+                if (p.post_shift) y = __fadd_rn(y, sh);
+                if (p.post_relu) y = fmaxf(y, 0.f);
+                *reinterpret_cast<float *>(cb + (j >> 3) * 2 * BOX_BYTES + r * 128 + ((((c & 31) >> 2) ^ (fcol + e)) << 4)) = y;
+                sums[4 * j + 2 * h + e] = y;
+              }
+            }
+          }
+          fence_proxy_async();
+          named_bar_sync(3 + wg, 128);
+          if (stg_issuer) {
+#pragma unroll
+            for (int b = 0; b < 4; ++b)
+              if (r0 + 64 * (b >> 1) < p.M) tma_store_2d(&tmap_out, stg_a + b * BOX_BYTES, 32 * (b & 1), r0 + 64 * (b >> 1));
+            bulk_commit();
+          }
+        }
+      } else if constexpr (ASPLIT) {
         // Staged: per 64-column pass, (1) v; the fp32 output goes into 32-column x 64-row boxes in the TMA box layout (row r at
         // r * 128 B, its 16-byte piece k at (k ^ (r & 7)) * 16), over the residual pair just read (RES) or in the staging
         // buffer, and v replaces the sums; (2) the pair from v into the staging buffer (head box, remainder box: 64 fp16
@@ -648,6 +713,48 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
           // pair are read once for both rows, from one base pointer per vector, and nothing per row is kept but its validity.  Each
           // product and sum is rounded on its own (__fmul_rn / __fadd_rn are never contracted), as in the row-by-row loops.
           const bool rok[2] = {m0 + frow < p.M, m0 + frow + 8 < p.M};
+          if (!RES && !st32 && st2 && !p.out && !p.res) {
+            // The pair alone, no residual (every unit's conv1 and conv2): v and the pair in one pass, the four epilogue vectors of a
+            // column pair read once for both rows, v kept in registers.  The arithmetic is that of the row-by-row pass and the pair
+            // pass below, each product and sum rounded on its own.
+            acquire(false);
+            uint8_t *brow = stg + (frow - 64 * wg) * 128 + 4 * (lane & 3);
+            const float *vsc = p.post_scale ? p.post_scale + c0 + fcol : nullptr, *vsh = p.post_shift ? p.post_shift + c0 + fcol : nullptr;
+            const float *v2sc = p.post2_scale ? p.post2_scale + c0 + fcol : nullptr, *v2sh = p.post2_shift ? p.post2_shift + c0 + fcol : nullptr;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * cc + jj;
+              if (c0 + 8 * jj + fcol >= p.Cout) continue;
+              const float2 sc = vsc ? __ldg(reinterpret_cast<const float2 *>(vsc + 8 * jj)) : make_float2(0.f, 0.f);
+              const float2 sh = vsh ? __ldg(reinterpret_cast<const float2 *>(vsh + 8 * jj)) : make_float2(0.f, 0.f);
+              const float2 sc2 = v2sc ? __ldg(reinterpret_cast<const float2 *>(v2sc + 8 * jj)) : make_float2(0.f, 0.f);
+              const float2 sh2 = v2sh ? __ldg(reinterpret_cast<const float2 *>(v2sh + 8 * jj)) : make_float2(0.f, 0.f);
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                if (!rok[h]) continue;
+                float a0 = sums[4 * j + 2 * h], a1 = sums[4 * j + 2 * h + 1];
+                if (vsc) { a0 = __fmul_rn(a0, sc.x); a1 = __fmul_rn(a1, sc.y); }
+                if (vsh) { a0 = __fadd_rn(a0, sh.x); a1 = __fadd_rn(a1, sh.y); }
+                if (p.post_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+                if (v2sc) { a0 = __fmul_rn(a0, sc2.x); a1 = __fmul_rn(a1, sc2.y); }
+                if (v2sh) { a0 = __fadd_rn(a0, sh2.x); a1 = __fadd_rn(a1, sh2.y); }
+                if (p.post2_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+                uint32_t hh, ll;
+                split_f16x2(a0, a1, hh, ll);
+                uint32_t *hs = reinterpret_cast<uint32_t *>(brow + h * 1024 + (((uint32_t)jj ^ rsw) * 16));
+                hs[0] = hh;
+                if (SPLIT) hs[BOX_BYTES / 4] = ll;
+              }
+            }
+            fence_proxy_async();
+            named_bar_sync(3 + wg, 128);
+            if (issue) {
+              tma_store_2d(&tmap_out_hi, stg_a, c0, r0);
+              if (SPLIT) tma_store_2d(&tmap_out_lo, stg_a + BOX_BYTES, c0, r0);
+            }
+            if (stg_issuer) bulk_commit();
+            continue;
+          }
           if (st32 && (RES || !p.res)) {
             uint8_t *brow = (RES ? res_sm + 2 * cc * BOX_BYTES : stg) + (frow - 64 * wg) * 128 + 8 * (lane & 1);    // row frow + 8 h: + 1024 h
             const float *vsc = p.post_scale ? p.post_scale + c0 + fcol : nullptr, *vsh = p.post_shift ? p.post_shift + c0 + fcol : nullptr;
@@ -830,6 +937,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     }
     if (stg_issuer) bulk_wait_all();                       // the last stores have completed before the CTA exits
     if (prof) { p.dbg[2] = clock64() - (RES || MEM_STAMPS ? p.dbg[2] : t_start); if (!MEM_STAMPS) p.dbg[3] = t_wait; }
+    if (prof) { p.dbg[7] = C::TM; p.dbg[8] = BN; }       // the tile: pixels x output channels
   }
 }
 
@@ -874,9 +982,10 @@ int encode_epilogue_map(CUtensorMap *tm, bool fp16, const void *base, int cols, 
   return HD_OK;
 }
 
-template <bool SPLIT, int PCH, bool HALF, bool GATHER = false, bool ASPLIT = false, int BN = 64, bool RES = false, bool SHORT = false>
+template <bool SPLIT, int PCH, bool HALF, bool GATHER = false, bool ASPLIT = false, int BN = 64, bool RES = false, bool SHORT = false,
+          bool CM = false>
 int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
-  using C = Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT>;
+  using C = Cfg<SPLIT, HALF, ASPLIT, BN, RES, SHORT, CM>;
   // function attributes and the SM count are per device: a process may drive several GPUs through this library
   static bool configured[kMaxDevices] = {};
   static int num_sms[kMaxDevices] = {};
@@ -884,7 +993,7 @@ int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= kMaxDevices) { set_last_error_text("conv_gemm_tc: device ordinal out of range"); return HD_ERR_UNSUPPORTED; }
   if (!configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES, SHORT>,
+    cudaError_t e = cudaFuncSetAttribute(conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES, SHORT, CM>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
     if (e != cudaSuccess) { set_last_error("conv_gemm_tc attr", e); return HD_ERR_CUDA; }
     cudaDeviceGetAttribute(&num_sms[dev], cudaDevAttrMultiProcessorCount, dev);
@@ -920,10 +1029,10 @@ int launch_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) {
     if (rc == HD_OK && SPLIT) rc = encode_epilogue_map(&tolo, true, p.out_lo, p.Cout, p.M, p.out2_ld * 2, "output remainder");
   }
   if (rc != HD_OK) return rc;
-  const int num_tiles = ceil_div(p.M, BM) * ceil_div(p.Cout, BN);
+  const int num_tiles = ceil_div(p.M, C::TM) * ceil_div(p.Cout, BN);
   const int ctas = C::CTAS * num_sms[dev];       // persistent: one CTA per SM (SHORT: two) walks the tile list
   dim3 grid(num_tiles < ctas ? num_tiles : ctas);
-  conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES, SHORT>
+  conv_gemm_tc_kernel<SPLIT, PCH, HALF, GATHER, ASPLIT, BN, RES, SHORT, CM>
       <<<grid, C::NUM_THREADS, C::SMEM_BYTES, st>>>(p, thi, tlo, tres, tout, tohi, tolo, stage);
   return check_launch("conv_gemm_tc_kernel");
 }
@@ -941,6 +1050,21 @@ bool wide_n_tile(const ConvParams &p) {
   return 16 * w128 <= 9 * w64;      // 2 w128 <= 1.125 w64
 }
 
+// The 64-channel x 256-pixel tile (CM) for the root conv1 over the planes (fp32 output alone, 32-bit input offsets for the lean
+// plane loop), unless the halved tile count costs more than an eighth in whole waves, as in wide_n_tile.  Block 1's 3x3 Cout = 64
+// layers measured slower on it than on the 128 x 64 tile: with two stages their consumers wait for data (DESIGN.md section 8).
+
+bool cout_on_m(const ConvParams &p) {
+  if (!p.planes || p.Cout != 64 || p.res || p.out_sub || p.out_hi || !p.out) return false;
+  if ((long long)p.n_img * p.H * p.W * p.in_ld >= (1ll << 31)) return false;
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (sms <= 0) return true;
+  const long long w256 = (ceil_div(p.M, 256) + sms - 1) / sms, w128 = (ceil_div(p.M, BM) + sms - 1) / sms;
+  return 16 * w256 <= 9 * w128;     // 2 w256 <= 1.125 w128
+}
+
 // Whether the SHORT kernel runs two CTAs per SM on this device (checked once per device); if not, its layers keep the one-CTA kernels.
 template <bool SPLIT, bool RES>
 bool short_k_two_ctas() {
@@ -950,7 +1074,7 @@ bool short_k_two_ctas() {
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= kMaxDevices) return false;
   if (two[dev] == 0) {
-    const auto kernel = conv_gemm_tc_kernel<SPLIT, 2, true, false, true, 64, RES, true>;
+    const auto kernel = conv_gemm_tc_kernel<SPLIT, 2, true, false, true, 64, RES, true, false>;
     int n = 0;
     if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) != cudaSuccess ||
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, C::NUM_THREADS, C::SMEM_BYTES) != cudaSuccess) {
@@ -971,7 +1095,7 @@ int launch_conv_f16(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st)
       set_last_error_text("hd_conv_gemm(tc planes): needs the conv1 plane geometry (Cin 32, KH 8, KW 1, stride 2, in_ld 4, even W)");
       return HD_ERR_INVALID;
     }
-    return launch_tc<SPLIT, 2, true, false, true>(p, d, st);
+    return cout_on_m(p) ? launch_tc<SPLIT, 2, true, false, true, 64, false, false, true>(p, d, st) : launch_tc<SPLIT, 2, true, false, true>(p, d, st);
   }
   // drain every 2 chunks = 8 fp16 tensor-core accumulations between round-to-nearest adds (both modes: impl 4 then runs the
   // rounded operations impl 3 runs on zero remainders)
