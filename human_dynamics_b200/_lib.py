@@ -170,6 +170,8 @@ SIGNATURES = {
     'hd_launch_count_reset': (None, []),
     'hd_conv_gemm': (_i, [C.POINTER(ConvDesc), _vp]),
     'hd_conv_gemm_profile': (_i, [C.POINTER(ConvDesc), _vp, _vp]),
+    'hd_conv_gemm_chain': (_i, [C.POINTER(ConvDesc), C.POINTER(ConvDesc), _vp]),
+    'hd_conv_gemm_chain_supported': (_i, [C.POINTER(ConvDesc), C.POINTER(ConvDesc)]),
     'hd_make_weight_tmap': (_i, [_vp, _i, _i, _i, _i, _vp]),
     'hd_make_act_tmap': (_i, [_vp, _ll, _i, _ll, _i, _vp]),
     'hd_pack_conv1_planes': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp]),

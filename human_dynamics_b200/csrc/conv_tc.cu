@@ -108,6 +108,17 @@ struct Cfg {
   static constexpr int V = HALF ? 2 : 1;                        // float4 loads per row per chunk per thread
 };
 
+// The staged epilogue of a column pair: y = relu?(y * sc + sh (+ r, ADD_R)), each product and sum rounded on its own (__fmul_rn /
+// __fadd_rn are never contracted), so every kernel that runs it gives the same bits.  sc / sh apply where their vector is given.
+template <bool ADD_R = false>
+__device__ __forceinline__ void epi2_rn(float &y0, float &y1, const float *has_sc, float2 sc, const float *has_sh, float2 sh,
+                                        const float2 *r, int relu) {
+  if (has_sc) { y0 = __fmul_rn(y0, sc.x); y1 = __fmul_rn(y1, sc.y); }
+  if (has_sh) { y0 = __fadd_rn(y0, sh.x); y1 = __fadd_rn(y1, sh.y); }
+  if (ADD_R) { const float2 v = *r; y0 = __fadd_rn(y0, v.x); y1 = __fadd_rn(y1, v.y); }
+  if (relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+}
+
 template <int R>
 struct RowState {       // R output rows of one producer thread: image index and top-left input coordinate
   int n[R], iy[R], ix[R];
@@ -733,12 +744,8 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
               for (int h = 0; h < 2; ++h) {
                 if (!rok[h]) continue;
                 float a0 = sums[4 * j + 2 * h], a1 = sums[4 * j + 2 * h + 1];
-                if (vsc) { a0 = __fmul_rn(a0, sc.x); a1 = __fmul_rn(a1, sc.y); }
-                if (vsh) { a0 = __fadd_rn(a0, sh.x); a1 = __fadd_rn(a1, sh.y); }
-                if (p.post_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
-                if (v2sc) { a0 = __fmul_rn(a0, sc2.x); a1 = __fmul_rn(a1, sc2.y); }
-                if (v2sh) { a0 = __fadd_rn(a0, sh2.x); a1 = __fadd_rn(a1, sh2.y); }
-                if (p.post2_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+                epi2_rn(a0, a1, vsc, sc, vsh, sh, nullptr, p.post_relu);
+                epi2_rn(a0, a1, v2sc, sc2, v2sh, sh2, nullptr, p.post2_relu);
                 uint32_t hh, ll;
                 split_f16x2(a0, a1, hh, ll);
                 uint32_t *hs = reinterpret_cast<uint32_t *>(brow + h * 1024 + (((uint32_t)jj ^ rsw) * 16));
@@ -770,10 +777,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
                 if (!rok[h]) continue;
                 float2 *f32 = reinterpret_cast<float2 *>(brow + h * 1024 + (jj >> 2) * BOX_BYTES + piece * 16);
                 float y0 = sums[4 * j + 2 * h], y1 = sums[4 * j + 2 * h + 1];
-                if (vsc) { y0 = __fmul_rn(y0, sc.x); y1 = __fmul_rn(y1, sc.y); }
-                if (vsh) { y0 = __fadd_rn(y0, sh.x); y1 = __fadd_rn(y1, sh.y); }
-                if (RES) { const float2 r = *f32; y0 = __fadd_rn(y0, r.x); y1 = __fadd_rn(y1, r.y); }
-                if (p.post_relu) { y0 = fmaxf(y0, 0.f); y1 = fmaxf(y1, 0.f); }
+                epi2_rn<RES>(y0, y1, vsc, sc, vsh, sh, f32, p.post_relu);
                 *f32 = make_float2(y0, y1);
                 sums[4 * j + 2 * h] = y0; sums[4 * j + 2 * h + 1] = y1;
               }
@@ -829,9 +833,7 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
                 for (int h = 0; h < 2; ++h) {
                   if (!rok[h]) continue;
                   float a0 = sums[4 * j + 2 * h], a1 = sums[4 * j + 2 * h + 1];
-                  if (vsc) { a0 = __fmul_rn(a0, sc.x); a1 = __fmul_rn(a1, sc.y); }
-                  if (vsh) { a0 = __fadd_rn(a0, sh.x); a1 = __fadd_rn(a1, sh.y); }
-                  if (p.post2_relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+                  epi2_rn(a0, a1, vsc, sc, vsh, sh, nullptr, p.post2_relu);
                   uint32_t hh, ll;
                   split_f16x2(a0, a1, hh, ll);
                   // columns 8 j + fcol, + 1 of the pass: piece jj of the 128-byte row
@@ -938,6 +940,311 @@ conv_gemm_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap
     if (stg_issuer) bulk_wait_all();                       // the last stores have completed before the CTA exits
     if (prof) { p.dbg[2] = clock64() - (RES || MEM_STAMPS ? p.dbg[2] : t_start); if (!MEM_STAMPS) p.dbg[3] = t_wait; }
     if (prof) { p.dbg[7] = C::TM; p.dbg[8] = BN; }       // the tile: pixels x output channels
+  }
+}
+
+// Chained 1x1 pair (hd_conv_gemm_chain): conv3 of a bottleneck unit (K = 64 -> 256, bias, row-aligned residual, fp32 output or its
+// strided subsample, the next unit's pre-activation as the post2 pair) and conv1 of the identity unit after it (K = 256 -> 64, whose
+// A operand is exactly that pair) in one persistent kernel.  Tile: 128 rows, the two consumer warpgroups 64 rows each, one producer
+// warpgroup.  Per tile, for each 64-column segment s of conv3's output: conv3's wgmmas (one K chunk, flushed once as in SHORT), its
+// staged epilogue (v into the residual slot and out by TMA store, or from registers for out_subsample), the pair of v written into
+// the warpgroup's pair chunk -- 64 rows x 128 bytes in the 128-byte swizzle, conv1's A layout for K chunk s -- and conv1's wgmmas on
+// it.  conv1 sees its K chunks in the same order as on its own, with the running sums flushed every PCH = 2 chunks, and every
+// epilogue product and sum is rounded as in the two launches: the outputs are the same bits.  conv1's epilogue stages its pair in
+// the pair chunk and writes it by TMA.  Neither the pair between the two convs nor conv1's reads of it ever reach HBM.
+//
+// Shared memory: two A stages (conv3's 128 x 64 input pair), two weight stages (conv3's segment box and conv1's chunk box, head and
+// remainder), per warpgroup two 16 KB residual slots (segment parity; each the fp32 staging of its segment, the next-but-one
+// segment's residual is loaded into it once the store has read it) and the 16 KB pair chunk.
+template <bool SPLIT>
+struct ChainCfg {
+  static constexpr int NUM_THREADS = 384;
+  static constexpr int SEGS = 4;                                   // conv3's 256 output columns = conv1's four 64-wide K chunks
+  static constexpr int A_BYTES = BM * 128;
+  static constexpr int A_STAGE = (SPLIT ? 2 : 1) * A_BYTES;
+  static constexpr int W1_OFFSET = (SPLIT ? 2 : 1) * BOX_BYTES;   // in a weight stage: conv3's box (+ remainder), then conv1's
+  static constexpr int W_STAGE = 2 * W1_OFFSET;
+  static constexpr int RES_SLOT = 64 * 64 * 4;
+  static constexpr int PAIR_BYTES = 2 * BOX_BYTES;
+  static constexpr int W_OFFSET = 2 * A_STAGE;
+  static constexpr int RES_OFFSET = W_OFFSET + 2 * W_STAGE;
+  static constexpr int PAIR_OFFSET = RES_OFFSET + 4 * RES_SLOT;   // slot e of warpgroup g at 2 g + e
+  static constexpr int BAR_OFFSET = PAIR_OFFSET + 2 * PAIR_BYTES;
+  static constexpr int SMEM_BYTES = BAR_OFFSET + 128 + 1024;
+  static_assert(SMEM_BYTES <= 232448, "dynamic shared memory beyond the 227 KB a CTA can opt into");
+  static constexpr int PROD_REGS = 40, CONS_REGS = 232;
+  static_assert(256 * CONS_REGS + 128 * PROD_REGS <= NUM_THREADS * (65536 / NUM_THREADS / 8 * 8), "setmaxnreg split beyond the CTA's registers");
+};
+
+template <bool SPLIT>
+__global__ void __launch_bounds__(384, 1)
+conv_chain_tc_kernel(const ConvParams p, const ConvParams q, const __grid_constant__ CUtensorMap tw3_hi,
+                     const __grid_constant__ CUtensorMap tw3_lo, const __grid_constant__ CUtensorMap tw1_hi,
+                     const __grid_constant__ CUtensorMap tw1_lo, const __grid_constant__ CUtensorMap tmap_res,
+                     const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_r1_hi,
+                     const __grid_constant__ CUtensorMap tmap_r1_lo, const int st32) {
+  using C = ChainCfg<SPLIT>;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t *smem = smem_raw + (smem_base - smem_u32(smem_raw));
+  const uint32_t bar_base = smem_base + C::BAR_OFFSET;
+  auto full_a = [&](int s) { return bar_base + 8u * s; };
+  auto empty_a = [&](int s) { return bar_base + 8u * (2 + s); };
+  auto full_w = [&](int s) { return bar_base + 8u * (4 + s); };
+  auto empty_w = [&](int s) { return bar_base + 8u * (6 + s); };
+  auto res_bar = [&](int g, int e) { return bar_base + 8u * (8 + 2 * g + e); };
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int num_tiles = (p.M + BM - 1) / BM;
+  const int my_tiles = (num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(full_a(s), 128);       // every producer thread, hardware arrive when its cp.asyncs land
+      mbar_init(empty_a(s), 8);        // one arrive per consumer warp once its conv3 wgmmas have read the stage
+      mbar_init(full_w(s), 1);         // arrive.expect_tx of the weight loads
+      mbar_init(empty_w(s), 8);
+    }
+    for (int i = 0; i < 4; ++i) mbar_init(bar_base + 8u * (8 + i), 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp >= W_PROD) {
+    // ---- producers: conv3's input pair by cp.async (1x1, stride 1: input row m is output row m), the weights by TMA ----
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(C::PROD_REGS));
+    const int t = threadIdx.x - W_PROD * 32, j = t & 7, rb = t >> 3;
+    const uint32_t off0 = (uint32_t)rb * 128u + (uint32_t)((j ^ (rb & 7)) << 4);
+    const __half *ihi = reinterpret_cast<const __half *>(p.in_hi);
+    const __half *ilo = reinterpret_cast<const __half *>(p.in_lo);
+    int wq = 0;
+    for (int ti = 0; ti < my_tiles; ++ti) {
+      const int m0 = ((int)blockIdx.x + ti * (int)gridDim.x) * BM;
+      const int sa = ti & 1;
+      mbar_wait(empty_a(sa), ((uint32_t)(ti >> 1) & 1u) ^ 1u);
+      const uint32_t a_hi = smem_base + sa * C::A_STAGE + off0;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int m = m0 + rb + 16 * i;
+        const bool ok = m < p.M;
+        const int e = ok ? m * (int)p.in_ld + j * 8 : 0;
+        cp_async16(a_hi + i * 16 * 128, ihi + e, ok ? 16u : 0u);
+        if (SPLIT) cp_async16(a_hi + C::A_BYTES + i * 16 * 128, ilo + e, ok ? 16u : 0u);
+      }
+      asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(full_a(sa)) : "memory");
+      if (t == 0) {
+        for (int s = 0; s < C::SEGS; ++s, ++wq) {
+          const int sw = wq & 1;
+          mbar_wait(empty_w(sw), ((uint32_t)(wq >> 1) & 1u) ^ 1u);
+          mbar_arrive_expect_tx(full_w(sw), 2 * C::W1_OFFSET);
+          const uint32_t wb = smem_base + C::W_OFFSET + sw * C::W_STAGE;
+          tma_load_2d(wb, &tw3_hi, full_w(sw), 0, 64 * s);                    // conv3's output channels 64 s .. 64 s + 63
+          if (SPLIT) tma_load_2d(wb + BOX_BYTES, &tw3_lo, full_w(sw), 0, 64 * s);
+          tma_load_2d(wb + C::W1_OFFSET, &tw1_hi, full_w(sw), 64 * s, 0);     // conv1's K chunk s
+          if (SPLIT) tma_load_2d(wb + C::W1_OFFSET + BOX_BYTES, &tw1_lo, full_w(sw), 64 * s, 0);
+        }
+      }
+    }
+    cp_async_commit();
+    cp_async_wait<0>();
+  } else {
+    // ---- consumers ----
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(C::CONS_REGS));
+    const int wg = warp >> 2;
+    const int frow = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's fragment rows: frow, frow + 8
+    const int fcol = 2 * (lane & 3);                            // and columns 8 j + fcol, + 1
+    const uint32_t rsw = (uint32_t)(lane >> 2);                 // the swizzle of this thread's rows
+    const bool issuer = (threadIdx.x & 127) == 0;               // the warpgroup's TMA loads and stores (bulk groups are per thread)
+    const uint32_t pb_a = smem_base + C::PAIR_OFFSET + wg * C::PAIR_BYTES;
+    uint8_t *const pbrow = smem + C::PAIR_OFFSET + wg * C::PAIR_BYTES + (frow - 64 * wg) * 128 + 4 * (lane & 3);
+    auto slot_a = [&](int e) { return smem_base + C::RES_OFFSET + (2 * wg + e) * C::RES_SLOT; };
+    // segment u = 4 ti + s of this CTA's walk: its residual rows in slot u & 1
+    auto load_res = [&](int u) {
+      if ((u >> 2) >= my_tiles) return;
+      const int r0 = ((int)blockIdx.x + (u >> 2) * (int)gridDim.x) * BM + 64 * wg, c0 = 64 * (u & 3);
+      const int boxes = r0 < p.M ? 2 : 0;
+      mbar_arrive_expect_tx(res_bar(wg, u & 1), boxes * BOX_BYTES);
+      for (int b = 0; b < boxes; ++b) tma_load_2d(slot_a(u & 1) + b * BOX_BYTES, &tmap_res, res_bar(wg, u & 1), c0 + 32 * b, r0);
+    };
+    if (issuer) { load_res(0); load_res(1); }
+    float acc3[32], accx3[SPLIT ? 32 : 1], acc1[32], accx1[SPLIT ? 32 : 1], sums1[32];
+    const int hw = p.Ho * p.Wo;
+    int wq = 0;
+    for (int ti = 0; ti < my_tiles; ++ti) {
+      const int m0 = ((int)blockIdx.x + ti * (int)gridDim.x) * BM, r0 = m0 + 64 * wg;
+      const bool rok[2] = {m0 + frow < p.M, m0 + frow + 8 < p.M};
+      const int sa = ti & 1;
+      mbar_wait(full_a(sa), (uint32_t)(ti >> 1) & 1u);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async (generic proxy) data -> wgmma (async proxy)
+      const uint32_t a_hi = smem_base + sa * C::A_STAGE + wg * 64 * 128;
+      const uint64_t da_hi = make_smem_desc(a_hi), da_lo = make_smem_desc(a_hi + C::A_BYTES);
+      const uint64_t dp_hi = make_smem_desc(pb_a), dp_lo = make_smem_desc(pb_a + BOX_BYTES);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) sums1[i] = 0.f;
+      for (int s = 0; s < C::SEGS; ++s, ++wq) {
+        const int u = 4 * ti + s, e = u & 1, sw = wq & 1;
+        mbar_wait(full_w(sw), (uint32_t)(wq >> 1) & 1u);
+        const uint32_t wb = smem_base + C::W_OFFSET + sw * C::W_STAGE;
+        const uint64_t d3_hi = make_smem_desc(wb), d3_lo = make_smem_desc(wb + BOX_BYTES);
+        const uint64_t d1_hi = make_smem_desc(wb + C::W1_OFFSET), d1_lo = make_smem_desc(wb + C::W1_OFFSET + BOX_BYTES);
+        // conv3, output columns 64 s .. 64 s + 63: one K chunk, the products of the 128 x 64 SHORT tile
+        fence_regs(acc3);
+        if constexpr (SPLIT) fence_regs(accx3);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t adv = (uint64_t)((k * 32) >> 4);
+          if constexpr (SPLIT) {
+            wgmma_m64n64k16_f16(accx3, da_lo + adv, d3_hi + adv, k != 0);
+            wgmma_m64n64k16_f16(accx3, da_hi + adv, d3_lo + adv, 1u);
+          }
+          wgmma_m64n64k16_f16(acc3, da_hi + adv, d3_hi + adv, k != 0);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(acc3);
+        if constexpr (SPLIT) fence_regs(accx3);
+        if (s == C::SEGS - 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_a(sa));
+        }
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc3[i] = __fadd_rn(0.f, acc3[i]);   // SHORT's one flush (a -0 becomes +0)
+        if constexpr (SPLIT) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) acc3[i] += accx3[i] * (1.0f / 2048.0f);
+        }
+        // v = acc + bias + residual (the slot, in the TMA box layout), staged over the residual or kept for the subsample
+        mbar_wait(res_bar(wg, e), (uint32_t)(u >> 1) & 1u);
+        uint8_t *brow = smem + C::RES_OFFSET + (2 * wg + e) * C::RES_SLOT + (frow - 64 * wg) * 128 + 8 * (lane & 1);
+        const float *vsh = p.post_shift ? p.post_shift + 64 * s + fcol : nullptr;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const uint32_t piece = (uint32_t)(2 * (jj & 3) + ((lane & 3) >> 1)) ^ rsw;
+          const float2 sh = vsh ? __ldg(reinterpret_cast<const float2 *>(vsh + 8 * jj)) : make_float2(0.f, 0.f);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (!rok[h]) continue;
+            float2 *f32 = reinterpret_cast<float2 *>(brow + h * 1024 + (jj >> 2) * BOX_BYTES + piece * 16);
+            float y0 = acc3[4 * jj + 2 * h], y1 = acc3[4 * jj + 2 * h + 1];
+            epi2_rn<true>(y0, y1, nullptr, make_float2(0.f, 0.f), vsh, sh, f32, 0);
+            if (st32) *f32 = make_float2(y0, y1);
+            acc3[4 * jj + 2 * h] = y0; acc3[4 * jj + 2 * h + 1] = y1;
+          }
+        }
+        if (!st32) {                   // x[:, ::s, ::s] from registers
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int m = m0 + frow + 8 * h;
+            if (m >= p.M) continue;
+            const int n_img = m / hw, r = m - n_img * hw, oy = r / p.Wo, ox = r - oy * p.Wo;
+            if (oy % p.out_sub != 0 || ox % p.out_sub != 0) continue;
+            const int Hs = (p.Ho + p.out_sub - 1) / p.out_sub, Ws = (p.Wo + p.out_sub - 1) / p.out_sub;
+            float *orow = p.out + ((size_t)((size_t)n_img * Hs + oy / p.out_sub) * Ws + ox / p.out_sub) * p.out_ld + 64 * s + fcol;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+              *reinterpret_cast<float2 *>(orow + 8 * jj) = make_float2(acc3[4 * jj + 2 * h], acc3[4 * jj + 2 * h + 1]);
+          }
+        }
+        // the pair of v = conv1's A operand for K chunk s.  The chunk was last read by this warpgroup's conv1 wgmmas of chunk s - 1
+        // (waited for), or at s = 0 by the previous tile's conv1 output stores.
+        if (s == 0 && ti > 0) {
+          if (issuer) bulk_wait_read<0>();
+          named_bar_sync(1 + wg, 128);
+        }
+        {
+          const float *v2sc = p.post2_scale ? p.post2_scale + 64 * s + fcol : nullptr, *v2sh = p.post2_shift ? p.post2_shift + 64 * s + fcol : nullptr;
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const float2 sc2 = v2sc ? __ldg(reinterpret_cast<const float2 *>(v2sc + 8 * jj)) : make_float2(0.f, 0.f);
+            const float2 sh2 = v2sh ? __ldg(reinterpret_cast<const float2 *>(v2sh + 8 * jj)) : make_float2(0.f, 0.f);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float a0 = acc3[4 * jj + 2 * h], a1 = acc3[4 * jj + 2 * h + 1];
+              epi2_rn(a0, a1, v2sc, sc2, v2sh, sh2, nullptr, p.post2_relu);
+              uint32_t hh, ll;
+              split_f16x2(a0, a1, hh, ll);
+              uint32_t *hs = reinterpret_cast<uint32_t *>(pbrow + h * 1024 + (((uint32_t)jj ^ rsw) * 16));
+              hs[0] = hh;
+              if (SPLIT) hs[BOX_BYTES / 4] = ll;
+            }
+          }
+        }
+        fence_proxy_async();             // the slot's fp32 values -> TMA store, the pair chunk -> wgmma
+        named_bar_sync(1 + wg, 128);
+        if (issuer && st32) {
+          if (r0 < p.M) {
+            tma_store_2d(&tmap_out, slot_a(e), 64 * s, r0);
+            tma_store_2d(&tmap_out, slot_a(e) + BOX_BYTES, 64 * s + 32, r0);
+          }
+          bulk_commit();
+        }
+        // conv1, K chunk s
+        fence_regs(acc1);
+        if constexpr (SPLIT) fence_regs(accx1);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t adv = (uint64_t)((k * 32) >> 4);
+          if constexpr (SPLIT) {
+            wgmma_m64n64k16_f16(accx1, dp_lo + adv, d1_hi + adv, (s | k) != 0);
+            wgmma_m64n64k16_f16(accx1, dp_hi + adv, d1_lo + adv, 1u);
+          }
+          wgmma_m64n64k16_f16(acc1, dp_hi + adv, d1_hi + adv, !((s & 1) == 0 && k == 0));
+        }
+        wgmma_commit();
+        if (issuer) {                    // under the wgmmas: the slot's store has read it; the next-but-one segment's residual
+          bulk_wait_read<0>();
+          load_res(u + 2);
+        }
+        wgmma_wait<0>();
+        fence_regs(acc1);
+        if constexpr (SPLIT) fence_regs(accx1);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_w(sw));
+        if (s & 1) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) sums1[i] += acc1[i];
+        }
+      }
+      if constexpr (SPLIT) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) sums1[i] += accx1[i] * (1.0f / 2048.0f);
+      }
+      // conv1's epilogue: its pair (post, then post2 where given) staged in the pair chunk and written by TMA
+      named_bar_sync(1 + wg, 128);       // every warp's wgmmas of the last chunk have read the pair chunk
+      {
+        const float *vsc = q.post_scale ? q.post_scale + fcol : nullptr, *vsh = q.post_shift ? q.post_shift + fcol : nullptr;
+        const float *v2sc = q.post2_scale ? q.post2_scale + fcol : nullptr, *v2sh = q.post2_shift ? q.post2_shift + fcol : nullptr;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const float2 sc = vsc ? __ldg(reinterpret_cast<const float2 *>(vsc + 8 * jj)) : make_float2(0.f, 0.f);
+          const float2 sh = vsh ? __ldg(reinterpret_cast<const float2 *>(vsh + 8 * jj)) : make_float2(0.f, 0.f);
+          const float2 sc2 = v2sc ? __ldg(reinterpret_cast<const float2 *>(v2sc + 8 * jj)) : make_float2(0.f, 0.f);
+          const float2 sh2 = v2sh ? __ldg(reinterpret_cast<const float2 *>(v2sh + 8 * jj)) : make_float2(0.f, 0.f);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float a0 = sums1[4 * jj + 2 * h], a1 = sums1[4 * jj + 2 * h + 1];
+            epi2_rn(a0, a1, vsc, sc, vsh, sh, nullptr, q.post_relu);
+            epi2_rn(a0, a1, v2sc, sc2, v2sh, sh2, nullptr, q.post2_relu);
+            uint32_t hh, ll;
+            split_f16x2(a0, a1, hh, ll);
+            uint32_t *hs = reinterpret_cast<uint32_t *>(pbrow + h * 1024 + (((uint32_t)jj ^ rsw) * 16));
+            hs[0] = hh;
+            if (SPLIT) hs[BOX_BYTES / 4] = ll;
+          }
+        }
+      }
+      fence_proxy_async();
+      named_bar_sync(1 + wg, 128);
+      if (issuer) {
+        if (r0 < p.M) {
+          tma_store_2d(&tmap_r1_hi, pb_a, 0, r0);
+          if (SPLIT) tma_store_2d(&tmap_r1_lo, pb_a + BOX_BYTES, 0, r0);
+        }
+        bulk_commit();
+      }
+    }
+    if (issuer) bulk_wait_all();         // the last stores have completed before the CTA exits
   }
 }
 
@@ -1172,7 +1479,98 @@ int launch_conv_tc(const ConvParams &p, const hd_conv_desc *d, cudaStream_t st) 
   return d->impl != HD_IMPL_TC_1XTF32 ? launch_tc<true, 2, false>(p, d, st) : launch_tc<false, 8, false>(p, d, st);
 }
 
+// Whether conv_chain_tc_kernel runs the pair (hd_b200.h, hd_conv_gemm_chain): shapes and pointers only, no device call.
+int chain_check(const hd_conv_desc *a, const hd_conv_desc *b) {
+  auto refuse = [](const char *why) {
+    char msg[160];
+    snprintf(msg, sizeof(msg), "hd_conv_gemm_chain: %s", why);
+    set_last_error_text(msg);
+    return HD_ERR_UNSUPPORTED;
+  };
+  if (!a || !b) return refuse("null descriptor");
+  if (a->impl != b->impl || (a->impl != HD_IMPL_TC_3XF16 && a->impl != HD_IMPL_TC_1XF16)) return refuse("both convs need impl 3 or impl 4");
+  const bool heads = a->impl == HD_IMPL_TC_1XF16;
+  auto one_by_one = [heads](const hd_conv_desc *d) {
+    return d->KH == 1 && d->KW == 1 && d->stride == 1 && d->pad_t == 0 && d->pad_l == 0 && d->Ho == d->H && d->Wo == d->W &&
+           !d->pre_scale && !d->pre_shift && !(d->flags & HD_CONV_INPUT_PLANES) && d->K_pad == d->Cin && d->tmap_hi &&
+           (heads ? !d->tmap_lo : d->tmap_lo != nullptr) && !d->tmap_hi_n64;
+  };
+  if (!one_by_one(a) || !one_by_one(b)) return refuse("both convs must be 1x1 stride 1 without prologue, with their weight maps");
+  if (a->Cin != 64 || a->Cout != 256 || b->Cin != a->Cout || b->Cout != 64)
+    return refuse("supported shape: conv3 64 -> 256 channels, then conv1 256 -> 64");
+  if (!a->in_hi || (heads ? a->in_lo != nullptr : !a->in_lo) || a->in_ld % 8 != 0 || !aligned16(a->in_hi) || (a->in_lo && !aligned16(a->in_lo)) ||
+      (long long)a->n_img * a->H * a->W * a->in_ld >= (1ll << 31))
+    return refuse("the first conv reads an aligned pre-split pair with 32-bit element offsets");
+  if (!a->res || a->res_stride != 1 || a->res_H != a->Ho || a->res_W != a->Wo || a->res_ld % 4 != 0 || !aligned16(a->res))
+    return refuse("the first conv needs a row-aligned residual");
+  if (!a->out || a->out_ld % 4 != 0 || !aligned16(a->out) || a->out_hi || a->out_lo || a->post_scale || a->post_relu ||
+      (a->post_shift && !aligned16(a->post_shift)) || (a->post2_scale == nullptr) != (a->post2_shift == nullptr))
+    return refuse("the first conv writes the fp32 output (or its subsample) and hands its post2 pair to the second");
+  if (b->n_img != a->n_img || b->H != a->Ho || b->W != a->Wo || b->in || b->in_hi || b->in_lo || b->res || b->out ||
+      b->out_subsample > 1 || !b->out_hi || (heads ? b->out_lo != nullptr : !b->out_lo) || b->out2_ld % 8 != 0 ||
+      !aligned16(b->out_hi) || (b->out_lo && !aligned16(b->out_lo)))
+    return refuse("the second conv reads the first's output rows and writes its pair alone");
+  return HD_OK;
+}
+
+template <bool SPLIT>
+int launch_chain(const ConvParams &p, const ConvParams &q, const hd_conv_desc *a, const hd_conv_desc *b, cudaStream_t st) {
+  using C = ChainCfg<SPLIT>;
+  static bool configured[kMaxDevices] = {};
+  static int num_sms[kMaxDevices] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= kMaxDevices) { set_last_error_text("hd_conv_gemm_chain: device ordinal out of range"); return HD_ERR_UNSUPPORTED; }
+  if (!configured[dev]) {
+    cudaError_t e = cudaFuncSetAttribute(conv_chain_tc_kernel<SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    if (e != cudaSuccess) { set_last_error("hd_conv_gemm_chain attr", e); return HD_ERR_CUDA; }
+    cudaDeviceGetAttribute(&num_sms[dev], cudaDevAttrMultiProcessorCount, dev);
+    if (num_sms[dev] <= 0) { set_last_error_text("hd_conv_gemm_chain: no multiprocessor count"); return HD_ERR_CUDA; }
+    configured[dev] = true;
+  }
+  alignas(64) CUtensorMap w3h, w3l, w1h, w1l, tres, tout, r1h, r1l;
+  memcpy(&w3h, a->tmap_hi, sizeof(CUtensorMap));
+  memcpy(&w3l, SPLIT ? a->tmap_lo : a->tmap_hi, sizeof(CUtensorMap));
+  memcpy(&w1h, b->tmap_hi, sizeof(CUtensorMap));
+  memcpy(&w1l, SPLIT ? b->tmap_lo : b->tmap_hi, sizeof(CUtensorMap));
+  memcpy(&tout, &w3h, sizeof(CUtensorMap));
+  memcpy(&r1l, &w3h, sizeof(CUtensorMap));
+  const int st32 = p.out_sub ? 0 : 1;
+  int rc = encode_epilogue_map(&tres, false, p.res, p.Cout, p.M, p.res_ld * 4, "residual");
+  if (rc == HD_OK && st32) rc = encode_epilogue_map(&tout, false, p.out, p.Cout, p.M, p.out_ld * 4, "output");
+  if (rc == HD_OK) rc = encode_epilogue_map(&r1h, true, q.out_hi, q.Cout, q.M, q.out2_ld * 2, "second output head");
+  if (rc == HD_OK && SPLIT) rc = encode_epilogue_map(&r1l, true, q.out_lo, q.Cout, q.M, q.out2_ld * 2, "second output remainder");
+  if (rc != HD_OK) return rc;
+  const int num_tiles = ceil_div(p.M, BM);
+  dim3 grid(num_tiles < num_sms[dev] ? num_tiles : num_sms[dev]);
+  conv_chain_tc_kernel<SPLIT><<<grid, C::NUM_THREADS, C::SMEM_BYTES, st>>>(p, q, w3h, w3l, w1h, w1l, tres, tout, r1h, r1l, st32);
+  return check_launch("conv_chain_tc_kernel");
+}
+
 }  // namespace hd
+
+extern "C" int hd_conv_gemm_chain_supported(const hd_conv_desc *first, const hd_conv_desc *second) {
+  return hd::chain_check(first, second) == HD_OK ? 1 : 0;
+}
+
+extern "C" int hd_conv_gemm_chain(const hd_conv_desc *first, const hd_conv_desc *second, void *stream) {
+  int rc = hd::chain_check(first, second);
+  if (rc) return rc;
+  hd::ConvParams p, q;
+  if ((rc = hd::fill_params(first, p))) return rc;
+  // the second conv's input is the first conv's pair, which never leaves the kernel: the first conv's input stands in for the
+  // validation of fill_params (same rows, and the kernel never reads it)
+  hd_conv_desc b = *second;
+  b.in_hi = first->in_hi;
+  b.in_lo = first->in_lo;
+  if ((rc = hd::fill_params(&b, q))) return rc;
+  if (!p.vec_out || !q.vec_out) {
+    hd::set_last_error_text("hd_conv_gemm_chain: outputs and epilogue vectors must be 16-byte aligned");
+    return HD_ERR_INVALID;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  return first->impl == HD_IMPL_TC_3XF16 ? hd::launch_chain<true>(p, q, first, second, st) : hd::launch_chain<false>(p, q, first, second, st);
+}
 
 // K-major weight matrix [rows, k_pad] (fp32 for the tf32 path, fp16 for the fp16 path) -> CUtensorMap with a
 // {128 bytes x box_rows} box and 128-byte swizzle.  box_rows must be 64: the kernel loads its 64- or 128-wide N tile as

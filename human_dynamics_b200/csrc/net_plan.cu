@@ -403,6 +403,8 @@ int hd_resnet50_create(hd_weight_fn get, void *user, int n_frames, int size, hd_
   float *x = bufA, *y = bufB;
   int H = H2;
   bool sub_ready = false;              // bufS already holds x[:, ::s, ::s] of the current unit's input
+  hd_conv_desc prev3;                  // the previous unit's conv3, the last step pushed when the loop reaches the next unit's conv1
+  bool has_prev3 = false;
   for (size_t ui = 0; ui < units.size() && b.rc == HD_OK; ++ui) {
     const Unit &un = units[ui];
     const int s = un.stride, Ho = (H - 1) / s + 1;
@@ -425,7 +427,20 @@ int hd_resnet50_create(hd_weight_fn get, void *user, int n_frames, int size, hd_
     }
     Builder::Bind b1; b1.n = n; b1.H = H; b1.W = H; b1.in = xs; b1.out2 = r1;
     if (!b.bind(un.conv1, b1, d)) break;
-    b.conv_step(d);
+    // an identity unit's conv1 reads only the pair the previous conv3 writes: one launch for both where the library runs the pair
+    // (nets.py ResNetPlan, ChainOp)
+    bool chained = false;
+    if (has_prev3 && !un.has_shortcut && !(s > 1 && !sub_ready)) {
+      hd_conv_desc c3 = prev3, c1 = d;
+      c3.out_hi = c3.out_lo = nullptr;
+      c3.tmap_out_hi = c3.tmap_out_lo = nullptr;
+      c1.in_hi = c1.in_lo = nullptr;
+      if (hd_conv_gemm_chain_supported(&c3, &c1) == 1) {
+        net->steps.back() = [c3, c1](cudaStream_t st) { return hd_conv_gemm_chain(&c3, &c1, (void *)st); };
+        chained = true;
+      }
+    }
+    if (!chained) b.conv_step(d);
     Builder::Bind b2; b2.n = n; b2.H = H; b2.W = H; b2.in = r1; b2.out2 = r2;
     if (!b.bind(un.conv2, b2, d)) break;
     b.conv_step(d);
@@ -447,6 +462,8 @@ int hd_resnet50_create(hd_weight_fn get, void *user, int n_frames, int size, hd_
     }
     if (!b.bind(un.conv3, b3, d)) break;
     b.conv_step(d);
+    prev3 = d;
+    has_prev3 = true;
     std::swap(x, y);
     std::swap(xs, ys);
     H = Ho;

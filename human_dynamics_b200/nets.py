@@ -355,6 +355,41 @@ class ConvOp(object):
             check(rc, 'hd_conv_gemm')
 
 
+class ChainOp(object):
+    """conv3 of a unit and conv1 of the identity unit after it in one launch (hd_conv_gemm_chain): the pre-activated pair conv3 hands to
+    conv1 stays in shared memory.  `d` / `ref` are conv3's descriptor, so the op reads as that conv to code that walks a plan's convs."""
+    __slots__ = ('first', 'second', 'd', 'ref')
+
+    def __init__(self, first, second):
+        self.first, self.second = first, second
+        self.d, self.ref = first.d, first.ref
+
+    @staticmethod
+    def bind(first, second):
+        """The chain of two bound ConvOps (conv3 writing the pair that conv1 reads), or None when the library does not run the pair as
+        one launch; then both ops are left as they were."""
+        d3, d1 = first.d, second.d
+        saved = (d3.out_hi, d3.out_lo, d1.in_hi, d1.in_lo)
+        d3.out_hi = d3.out_lo = d1.in_hi = d1.in_lo = None
+        if lib.hd_conv_gemm_chain_supported(first.ref, second.ref) == 1:
+            first.encode_act_maps()
+            return ChainOp(first, second)
+        d3.out_hi, d3.out_lo, d1.in_hi, d1.in_lo = saved
+        return None
+
+    def rebind(self, field, tensor):
+        self.first.rebind(field, tensor)
+
+    def encode_act_maps(self):
+        self.first.encode_act_maps()
+        self.second.encode_act_maps()
+
+    def run(self, stream):
+        rc = lib.hd_conv_gemm_chain(self.first.ref, self.second.ref, stream)
+        if rc:
+            check(rc, 'hd_conv_gemm_chain')
+
+
 class PackedConv1Planes(object):
     """ResNet root conv1 (7x7 stride 2, explicit pad 3+3, bias; A.2) on the tensor cores, reading its input as two padded
     RGBX fp16 planes [n, S+6, WP, 4] (head / remainder, hd_pack_conv1_planes): every (output pixel, kernel row) needs 8
@@ -570,7 +605,13 @@ class ResNetPlan(object):
                     res, res_geom = self.bufS, (unit['depth'], Ho, Ho, 1)
                 else:
                     res, res_geom = x, (unit['depth'], H, H, 1)
-                self.ops.append(unit['conv1'].bind(None, n, H, H, None, inp_split=xs, out_split=r1, impl=impl))
+                conv1 = unit['conv1'].bind(None, n, H, H, None, inp_split=xs, out_split=r1, impl=impl)
+                # an identity unit's conv1 reads only the pair the previous conv3 writes: one launch for both where the library runs it
+                chain = ChainOp.bind(self.ops[-1], conv1) if ui > 0 and 'shortcut' not in unit and isinstance(self.ops[-1], ConvOp) else None
+                if chain is not None:
+                    self.ops[-1] = chain
+                else:
+                    self.ops.append(conv1)
                 if ui == 0:
                     self.in_refs += self._split_refs(self.ops[-1])
                 self.ops.append(unit['conv2'].bind(None, n, H, H, None, inp_split=r1, out_split=r2, impl=impl))

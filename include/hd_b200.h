@@ -119,6 +119,15 @@ int hd_conv_gemm(const hd_conv_desc *d, void *stream);
 /* Same launch; additionally CTA (0,0) of the tensor-core kernel writes per-role clock64 counters to dbg[0..15]
  * (device int64; layout in conv_simt.cu).  Tuning aid, not part of the reference surface. */
 int hd_conv_gemm_profile(const hd_conv_desc *d, void *stream, long long *dbg);
+/* Two 1x1 convs in one launch, the second reading the first's pre-activated output pair, which then never reaches memory: conv3 of a
+ * bottleneck unit (`first`: pre-split input, bias, a row-aligned residual, the fp32 output or its out_subsample, and the next unit's
+ * pre-activation in post2_*; out_hi / out_lo NULL) and conv1 of the identity unit after it (`second`: in_hi / in_lo NULL, its fp16
+ * pair in out_hi / out_lo).  The outputs are the same bits as hd_conv_gemm(first with out_hi / out_lo set) then hd_conv_gemm(second
+ * reading that pair).  Supported: both 1x1 stride 1, impl 3 or 4 alike, first 64 -> 256 channels, second 256 -> 64 over the same rows;
+ * any other pair is refused with HD_ERR_UNSUPPORTED and a message (hd_last_error). */
+int hd_conv_gemm_chain(const hd_conv_desc *first, const hd_conv_desc *second, void *stream);
+/* 1 if hd_conv_gemm_chain runs this pair, else 0 (hd_last_error says why).  Shapes and pointers only: no device call. */
+int hd_conv_gemm_chain_supported(const hd_conv_desc *first, const hd_conv_desc *second);
 
 /* Encode the TMA descriptor (CUtensorMap, 128 B, written to host memory `tmap_out`) for a K-major weight matrix
  * [rows, k_pad] of elem_bytes-wide elements (4 = fp32/tf32 path, 2 = fp16 path) with a {128 bytes x box_rows} box and

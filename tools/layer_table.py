@@ -1,4 +1,6 @@
-"""Per-layer table of one C3 trunk pass: time, TFLOP/s, and the layer's compulsory HBM traffic / time (GB/s).
+"""Per-layer table of one C3 trunk pass: time, TFLOP/s, and the layer's compulsory HBM traffic / time (GB/s).  A chained launch
+(hd_conv_gemm_chain: conv3 and the next unit's conv1) is one row with K < 0: both GEMMs' FLOPs, and as bytes its input pair, residual,
+fp32 output (or its subsample) and the conv1 pair.
 --impl picks the precision mode of the trunk (default 'auto'; 'tc1h' = the half-precision inference mode)."""
 import argparse, sys, os, ctypes
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -44,6 +46,11 @@ for stage, c in (('A', min(eng.config.frame_chunk, N)), ('B', min(eng.config.lat
         fl = 2.0 * M * K * Nn * reps
         inb = d.n_img * d.H * d.W * d.Cin * 4
         outb = M * Nn * ((4 if d.out else 0) + (4 if d.out_hi else 0)) + (M * Nn * 4 if d.res else 0)
+        chain = getattr(op, 'second', None)
+        if chain is not None:             # hd_conv_gemm_chain: both GEMMs' FLOPs, and the second conv's pair is its only other traffic
+            fl += 2.0 * M * chain.d.Cin * chain.d.Cout * reps
+            outb += M * chain.d.Cout * 4
+            K = -K                        # a negative K marks the chained row
         rows.append((t, stage, M, K, Nn, d.KH, d.stride, bool(d.res), bool(d.out_hi), fl / t / 1e12, (inb + outb) * reps / t / 1e9, d.impl))
 tot = sum(r[0] for r in rows)
 print('trunk conv total %.2f ms  (%.0f TFLOP/s avg)' % (tot * 1e3, sum(r[0] * r[9] for r in rows) / tot))
