@@ -161,7 +161,7 @@ class JpegTables(C.Structure):
 
 
 # name -> (restype, argtypes); must list every symbol include/hd_b200.h declares.
-_vp, _i, _ll, _f, _sz = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_size_t
+_vp, _i, _ll, _f, _sz, _ull = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_size_t, C.c_ulonglong
 SIGNATURES = {
     'hd_version': (_i, []),
     'hd_status_string': (C.c_char_p, [_i]),
@@ -196,6 +196,9 @@ SIGNATURES = {
     'hd_split_f16': (_i, [_vp, _vp, _vp, _ll, _vp]),
     'hd_ief_fc1_theta': (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _i, _vp]),
     'hd_ief_fc3': (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp]),
+    'hd_ief_fc1_theta_dropout': (_i, [_vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _i, _ull, _ull, _i, _f, _vp]),
+    'hd_ief_fc3_dropout': (_i, [_vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _ull, _ull, _i, _f, _vp]),
+    'hd_dropout_mask': (_i, [_ull, _ull, _i, _i, _i, _f, _vp, _vp]),
     'hd_ief_delta_init': (_i, [_vp, _vp, _i, _i, _vp]),
     'hd_net_destroy': (None, [_vp]),
     'hd_net_error': (C.c_char_p, [_vp]),
@@ -231,6 +234,8 @@ SIGNATURES = {
     'hd_col_sum': (_i, [_vp, _ll, _i, _ll, _vp, _vp]),
     'hd_relu_backward': (_i, [_vp, _vp, _vp, _ll, _vp]),
     'hd_fc_small_dgrad': (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _i, _vp]),
+    'hd_relu_dropout_backward': (_i, [_vp, _vp, _vp, _ll, _f, _vp]),
+    'hd_fc_small_dgrad_dropout': (_i, [_vp, _i, _vp, _i, _i, _vp, _f, _vp, _i, _vp]),
     'hd_add_strided': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _vp]),
     'hd_dpose_workspace_bytes': (_sz, [_i]),
     'hd_dpose_trunk_forward': (_i, [_vp] * 10 + [_i, _vp]),

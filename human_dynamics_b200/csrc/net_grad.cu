@@ -198,18 +198,21 @@ __global__ void __launch_bounds__(256) col_sum_kernel(const float *__restrict__ 
   }
 }
 
-// dx = dy * (y > 0) (TF ReluGrad: 0 at 0); y is the ReLU's output (or input).
-__global__ void relu_backward_kernel(const float *__restrict__ y, const float *dy, float *dx, long long n) {
+// dx = dy * (y > 0) (TF ReluGrad: 0 at 0); y is the ReLU's output (or input).  p < 1: y is the output of a dropout after the ReLU
+// (y > 0 <=> kept and positive) and dx = y > 0 ? dy / p : 0, TF's gradient through the dropout's Mul by the 0 / 1 mask, then its
+// RealDiv by keep_prob.
+__global__ void relu_backward_kernel(const float *__restrict__ y, const float *dy, float *dx, long long n, float p) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  dx[i] = __ldg(y + i) > 0.f ? dy[i] : 0.f;
+  dx[i] = __ldg(y + i) > 0.f ? (p < 1.f ? __fdiv_rn(dy[i], p) : dy[i]) : 0.f;
 }
 
 // out[n, k] = (mask[n, k] > 0) * sum_{j < D} g[n, j] * Wt[j, k]    (Wt [D, K] row-major, D <= 96, mask nullable).
 // The K = 85 / 72 input-gradient product of the IEF fc3 (dh2 = dtheta . W3^T): too short for the tensor-core tile.  A block takes 8
-// rows and all K columns (thread = 4 columns); j runs in order, so each output has a fixed summation order.
+// rows and all K columns (thread = 4 columns); j runs in order, so each output has a fixed summation order.  p < 1: mask is the output
+// of a dropout after the ReLU and a kept element's gradient is divided by p (relu_backward_kernel).
 __global__ void __launch_bounds__(256) fc_small_dgrad_kernel(const float *__restrict__ g, int g_ld, const float *__restrict__ Wt, int K,
-                                                             int D, const float *__restrict__ mask, float *__restrict__ out, int N) {
+                                                             int D, const float *__restrict__ mask, float *__restrict__ out, int N, float p) {
   __shared__ float gs[8][96];
   const int r0 = blockIdx.x * 8;
   for (int i = threadIdx.x; i < 8 * 96; i += 256) {
@@ -237,6 +240,7 @@ __global__ void __launch_bounds__(256) fc_small_dgrad_kernel(const float *__rest
       if (mask) {
         const float4 m = __ldg(reinterpret_cast<const float4 *>(mask + o));
         y.x = m.x > 0.f ? y.x : 0.f; y.y = m.y > 0.f ? y.y : 0.f; y.z = m.z > 0.f ? y.z : 0.f; y.w = m.w > 0.f ? y.w : 0.f;
+        if (p < 1.f) { y.x = __fdiv_rn(y.x, p); y.y = __fdiv_rn(y.y, p); y.z = __fdiv_rn(y.z, p); y.w = __fdiv_rn(y.w, p); }
       }
       *reinterpret_cast<float4 *>(out + o) = y;
     }
@@ -310,7 +314,13 @@ int hd_col_sum(const float *x, long long rows, int cols, long long ld, float *ou
 
 int hd_relu_backward(const float *y, const float *dy, float *dx, long long n, void *stream) {
   HD_REQUIRE(y && dy && dx && n > 0, "hd_relu_backward: bad arguments");
-  relu_backward_kernel<<<hd::ceil_div(n, 256), 256, 0, (cudaStream_t)stream>>>(y, dy, dx, n);
+  relu_backward_kernel<<<hd::ceil_div(n, 256), 256, 0, (cudaStream_t)stream>>>(y, dy, dx, n, 1.f);
+  return hd::check_launch("relu_backward_kernel");
+}
+
+int hd_relu_dropout_backward(const float *y, const float *dy, float *dx, long long n, float p, void *stream) {
+  HD_REQUIRE(y && dy && dx && n > 0 && p > 0.f && p <= 1.f, "hd_relu_dropout_backward: bad arguments (0 < p <= 1)");
+  relu_backward_kernel<<<hd::ceil_div(n, 256), 256, 0, (cudaStream_t)stream>>>(y, dy, dx, n, p);
   return hd::check_launch("relu_backward_kernel");
 }
 
@@ -318,7 +328,16 @@ int hd_fc_small_dgrad(const float *g, int g_ld, const float *Wt, int K, int D, c
   HD_REQUIRE(g && Wt && out && N > 0 && D > 0 && D <= 96 && g_ld >= D && K > 0 && K % 4 == 0 && hd::aligned16(Wt) && hd::aligned16(out) &&
                  (!mask || hd::aligned16(mask)),
              "hd_fc_small_dgrad: bad arguments (D <= 96, K % 4 == 0, 16-byte aligned Wt / mask / out)");
-  fc_small_dgrad_kernel<<<hd::ceil_div(N, 8), 256, 0, (cudaStream_t)stream>>>(g, g_ld, Wt, K, D, mask, out, N);
+  fc_small_dgrad_kernel<<<hd::ceil_div(N, 8), 256, 0, (cudaStream_t)stream>>>(g, g_ld, Wt, K, D, mask, out, N, 1.f);
+  return hd::check_launch("fc_small_dgrad_kernel");
+}
+
+int hd_fc_small_dgrad_dropout(const float *g, int g_ld, const float *Wt, int K, int D, const float *mask, float p, float *out, int N,
+                              void *stream) {
+  HD_REQUIRE(g && Wt && mask && out && N > 0 && D > 0 && D <= 96 && g_ld >= D && K > 0 && K % 4 == 0 && p > 0.f && p <= 1.f &&
+                 hd::aligned16(Wt) && hd::aligned16(out) && hd::aligned16(mask),
+             "hd_fc_small_dgrad_dropout: bad arguments (D <= 96, K % 4 == 0, 0 < p <= 1, 16-byte aligned Wt / mask / out)");
+  fc_small_dgrad_kernel<<<hd::ceil_div(N, 8), 256, 0, (cudaStream_t)stream>>>(g, g_ld, Wt, K, D, mask, out, N, p);
   return hd::check_launch("fc_small_dgrad_kernel");
 }
 

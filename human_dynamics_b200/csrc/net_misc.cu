@@ -1,6 +1,7 @@
 // Small non-GEMM pieces of the network path: ResNet root/tail, GroupNorm statistics, IEF glue.
 #include <cuda_fp16.h>
 #include "conv_common.cuh"
+#include "dropout.cuh"
 
 namespace {
 
@@ -255,10 +256,12 @@ __global__ void split_f16_kernel(const float4 *__restrict__ x, uint2 *__restrict
 // IEF fc1, theta part (src/models.py:402,102: state = concat[phi, theta] -> fc1): h1 = relu(P + theta . W1[2048:]) with P = phi . W1[:2048]
 // + b1 hoisted out of the stage loop.  K = 85 / 72 is far too short for the tensor-core tile; here a block takes 8 rows and all C
 // columns (thread = 4 columns), theta rows sit in smem, W streams from L2 (348 KB, read once per block).  Output = the pre-split
-// fp16 pair fc2's cp.async producer loads (and optionally fp32).
+// fp16 pair fc2's cp.async producer loads (and optionally fp32).  drop.p < 1: the dropout1 mask (dropout.cuh) is applied to h1 before
+// either is written.
 __global__ void __launch_bounds__(256) ief_fc1_theta_kernel(const float *__restrict__ P, const float *__restrict__ theta, int theta_ld,
                                                             const float *__restrict__ W, int K, int Cc, __half *__restrict__ out_hi,
-                                                            __half *__restrict__ out_lo, float *__restrict__ out_f32, int N) {
+                                                            __half *__restrict__ out_lo, float *__restrict__ out_f32, int N,
+                                                            const hd::DropoutSite drop) {
   __shared__ float th[8][96];
   const int r0 = blockIdx.x * 8;
   for (int i = threadIdx.x; i < 8 * 96; i += 256) {
@@ -289,8 +292,12 @@ __global__ void __launch_bounds__(256) ief_fc1_theta_kernel(const float *__restr
       if (r0 + r >= N) break;
       const size_t o = (size_t)(r0 + r) * Cc + c;
       const float4 p = __ldg(reinterpret_cast<const float4 *>(P + o));
-      const float y0 = fmaxf(acc[r][0] + p.x, 0.f), y1 = fmaxf(acc[r][1] + p.y, 0.f), y2 = fmaxf(acc[r][2] + p.z, 0.f),
-                  y3 = fmaxf(acc[r][3] + p.w, 0.f);
+      float y0 = fmaxf(acc[r][0] + p.x, 0.f), y1 = fmaxf(acc[r][1] + p.y, 0.f), y2 = fmaxf(acc[r][2] + p.z, 0.f),
+            y3 = fmaxf(acc[r][3] + p.w, 0.f);
+      if (drop.p < 1.f) {            // Cc % 4 == 0: columns c .. c+3 are the four words of one Philox call
+        const float4 m = hd::dropout_apply4(drop, o >> 2, make_float4(y0, y1, y2, y3));
+        y0 = m.x; y1 = m.y; y2 = m.z; y3 = m.w;
+      }
       if (out_f32) *reinterpret_cast<float4 *>(out_f32 + o) = make_float4(y0, y1, y2, y3);
       if (out_hi) {
         uint32_t h0, l0, h1, l1;
@@ -305,18 +312,33 @@ __global__ void __launch_bounds__(256) ief_fc1_theta_kernel(const float *__restr
 
 // IEF fc3 + update (models.py:113,410): theta_out = theta_prev + h2 . W3 + b3, W3 [K, D] with D = 85 / 72: one tensor-core tile
 // would serialise K = 1024 on 5 CTAs.  Block = 8 rows x 8 warps; warp w sums k in [w*K/8, (w+1)*K/8) for the block's rows (lane = output
-// column, 3 per lane), partial sums meet in smem in warp order: fixed summation order, bit-reproducible.
-__global__ void __launch_bounds__(256) ief_fc3_kernel(const float *__restrict__ h2, const float *__restrict__ W, const float *__restrict__ bias,
+// column, 3 per lane), partial sums meet in smem in warp order: fixed summation order, bit-reproducible.  drop.p < 1: h2 is read
+// through the dropout2 mask (dropout.cuh) and the masked rows are written back over it (fc3's weight gradient reads them); the sums
+// are the same code.
+__global__ void __launch_bounds__(256) ief_fc3_kernel(const float *h2, const float *__restrict__ W, const float *__restrict__ bias,
                                                       const float *__restrict__ prev, int prev_ld, float *__restrict__ out, int out_ld, int N,
-                                                      int K, int D) {
+                                                      int K, int D, const hd::DropoutSite drop, float *h2_masked) {
   extern __shared__ float sm[];
   float *hs = sm;                         // [8][K]
   float *part = sm + 8 * K;               // [8 warps][8 rows][96]
   const int r0 = blockIdx.x * 8;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int i = threadIdx.x; i < 8 * K; i += 256) {
-    const int r = i / K, k = i - r * K;
-    hs[i] = (r0 + r < N) ? __ldg(h2 + (size_t)(r0 + r) * K + k) : 0.f;
+  if (drop.p < 1.f) {
+    for (int i = threadIdx.x * 4; i < 8 * K; i += 1024) {        // K % 64 == 0: four columns of one row, one Philox call
+      const int r = i / K, k = i - r * K;
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (r0 + r < N) {
+        const size_t o = (size_t)(r0 + r) * K + k;
+        v = hd::dropout_apply4(drop, o >> 2, *reinterpret_cast<const float4 *>(h2 + o));
+        *reinterpret_cast<float4 *>(h2_masked + o) = v;
+      }
+      *reinterpret_cast<float4 *>(hs + i) = v;
+    }
+  } else {
+    for (int i = threadIdx.x; i < 8 * K; i += 256) {
+      const int r = i / K, k = i - r * K;
+      hs[i] = (r0 + r < N) ? __ldg(h2 + (size_t)(r0 + r) * K + k) : 0.f;
+    }
   }
   __syncthreads();
   float acc[8][3];
@@ -473,14 +495,28 @@ extern "C" int hd_ief_fc1_theta(const float *P, const float *theta, int theta_ld
                  (!out_f32 || hd::aligned16(out_f32)),
              "hd_ief_fc1_theta: bad arguments");
   ief_fc1_theta_kernel<<<hd::ceil_div(N, 8), 256, 0, (cudaStream_t)stream>>>(P, theta, theta_ld, W, K, C, reinterpret_cast<__half *>(out_hi),
-                                                                            reinterpret_cast<__half *>(out_lo), out_f32, N);
+                                                                            reinterpret_cast<__half *>(out_lo), out_f32, N,
+                                                                            hd::DropoutSite{0, 0, 0, 1.f});
   return hd::check_launch("ief_fc1_theta_kernel");
 }
 
-extern "C" int hd_ief_fc3(const float *h2, const float *W, const float *bias, const float *prev, int prev_ld, float *out, int out_ld, int N,
-                          int K, int D, void *stream) {
-  HD_REQUIRE(h2 && W && bias && prev && out && N > 0 && K > 0 && K % 64 == 0 && D > 0 && D <= 96 && prev_ld >= D && out_ld >= D,
-             "hd_ief_fc3: bad arguments (K % 64 == 0, D <= 96)");
+extern "C" int hd_ief_fc1_theta_dropout(const float *P, const float *theta, int theta_ld, const float *W, int K, int C, void *out_hi,
+                                        void *out_lo, float *out_f32, int N, unsigned long long seed, unsigned long long step, int site,
+                                        float p, void *stream) {
+  HD_REQUIRE(P && theta && W && (out_hi || out_f32) && (out_hi || !out_lo) && N > 0 && K > 0 && K <= 96 && theta_ld >= K &&
+                 C > 0 && C % 4 == 0 && (long long)N * C <= (1ll << 34) && site >= 0 && p > 0.f && p <= 1.f && hd::aligned16(P) &&
+                 hd::aligned16(W) && (!out_hi || (hd::aligned16(out_hi) && hd::aligned16(out_lo))) && (!out_f32 || hd::aligned16(out_f32)),
+             "hd_ief_fc1_theta_dropout: bad arguments (0 < p <= 1, site >= 0, N*C <= 2^34)");
+  ief_fc1_theta_kernel<<<hd::ceil_div(N, 8), 256, 0, (cudaStream_t)stream>>>(P, theta, theta_ld, W, K, C, reinterpret_cast<__half *>(out_hi),
+                                                                            reinterpret_cast<__half *>(out_lo), out_f32, N,
+                                                                            hd::DropoutSite{seed, step, (unsigned)site, p});
+  return hd::check_launch("ief_fc1_theta_kernel");
+}
+
+namespace {
+
+int launch_ief_fc3(const float *h2, const float *W, const float *bias, const float *prev, int prev_ld, float *out, int out_ld, int N, int K,
+                   int D, const hd::DropoutSite &drop, float *h2_masked, void *stream) {
   const size_t smem = (size_t)(8 * K + 8 * 8 * 96) * sizeof(float);
   static bool configured[64] = {};
   int dev = 0;
@@ -491,6 +527,44 @@ extern "C" int hd_ief_fc3(const float *h2, const float *W, const float *bias, co
     configured[dev] = true;
   }
   HD_REQUIRE(smem <= 100 * 1024, "hd_ief_fc3: K too large");
-  ief_fc3_kernel<<<hd::ceil_div(N, 8), 256, smem, (cudaStream_t)stream>>>(h2, W, bias, prev, prev_ld, out, out_ld, N, K, D);
+  ief_fc3_kernel<<<hd::ceil_div(N, 8), 256, smem, (cudaStream_t)stream>>>(h2, W, bias, prev, prev_ld, out, out_ld, N, K, D, drop, h2_masked);
   return hd::check_launch("ief_fc3_kernel");
+}
+
+// One thread per group of 4 elements (one Philox call): out[w] = keep of element w, for w < N*C.
+__global__ void dropout_mask_kernel(const hd::DropoutSite d, long long total, uint8_t *__restrict__ out) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g * 4 >= total) return;
+  const uint4 w = hd::dropout_words(d, (unsigned long long)g);
+  const uint32_t words[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+  for (int e = 0; e < 4; ++e)
+    if (g * 4 + e < total) out[g * 4 + e] = hd::dropout_keep(words[e], d.p) ? 1 : 0;
+}
+
+}  // namespace
+
+extern "C" int hd_ief_fc3(const float *h2, const float *W, const float *bias, const float *prev, int prev_ld, float *out, int out_ld, int N,
+                          int K, int D, void *stream) {
+  HD_REQUIRE(h2 && W && bias && prev && out && N > 0 && K > 0 && K % 64 == 0 && D > 0 && D <= 96 && prev_ld >= D && out_ld >= D,
+             "hd_ief_fc3: bad arguments (K % 64 == 0, D <= 96)");
+  return launch_ief_fc3(h2, W, bias, prev, prev_ld, out, out_ld, N, K, D, hd::DropoutSite{0, 0, 0, 1.f}, nullptr, stream);
+}
+
+extern "C" int hd_ief_fc3_dropout(float *h2, const float *W, const float *bias, const float *prev, int prev_ld, float *out, int out_ld, int N,
+                                  int K, int D, unsigned long long seed, unsigned long long step, int site, float p, void *stream) {
+  HD_REQUIRE(h2 && W && bias && prev && out && N > 0 && K > 0 && K % 64 == 0 && D > 0 && D <= 96 && prev_ld >= D && out_ld >= D &&
+                 (long long)N * K <= (1ll << 34) && site >= 0 && p > 0.f && p <= 1.f && hd::aligned16(h2),
+             "hd_ief_fc3_dropout: bad arguments (K % 64 == 0, D <= 96, 0 < p <= 1, site >= 0, h2 16-byte aligned)");
+  return launch_ief_fc3(h2, W, bias, prev, prev_ld, out, out_ld, N, K, D, hd::DropoutSite{seed, step, (unsigned)site, p}, h2, stream);
+}
+
+extern "C" int hd_dropout_mask(unsigned long long seed, unsigned long long step, int site, int N, int C, float p, unsigned char *out,
+                               void *stream) {
+  HD_REQUIRE(out && N > 0 && C > 0 && (long long)N * C <= (1ll << 34) && site >= 0 && p > 0.f && p <= 1.f,
+             "hd_dropout_mask: bad arguments (N, C > 0, N*C <= 2^34, site >= 0, 0 < p <= 1)");
+  const long long total = (long long)N * C;
+  dropout_mask_kernel<<<hd::ceil_div((total + 3) / 4, 256), 256, 0, (cudaStream_t)stream>>>(hd::DropoutSite{seed, step, (unsigned)site, p},
+                                                                                          total, out);
+  return hd::check_launch("dropout_mask_kernel");
 }

@@ -1185,10 +1185,22 @@ class IEFPlan(object):
     keep=True (training, fast heads only): every head writes each stage's h1 in fp32 (hd_ief_fc1_theta's out_f32) and h2 into buffers of
     its own, and its stages other than the last into separate outputs instead of updating the state in place; each delta head writes an
     (N,85) output of its own instead of a slot of delta_all.  `saved` = per head, in the order main, delta_keys: (h1 [S,N,1024],
-    h2 [S,N,1024], the outputs of stages 0 .. S-2) -- what the backward reads.  The launches are the same, so are the outputs' bits."""
+    h2 [S,N,1024], the outputs of stages 0 .. S-2) -- what the backward reads.  The launches are the same, so are the outputs' bits.
 
-    def __init__(self, packed: PackedIEF, N, num_stage=3, delta_keys=None, impl='auto', keep=False):
+    dropout=(seed, step, call, keep_prob) (training, keep=True): slim.dropout(keep_prob) after the ReLU of fc1 and fc2 at every stage of
+    every head, as the reference trains (src/models.py:101-105, is_training=True).  The masks are drawn in hd_ief_fc1_theta_dropout and
+    hd_ief_fc3_dropout from (seed, step, site, row, column) alone (csrc/dropout.cuh), site = ief_dropout_site(call, head, stage, layer)
+    with head 0 = main and 1.. = the packed delta heads in ascending dt; the saved h1 / h2 are the masked activations.  keep_prob 1 or
+    dropout=None: today's launches."""
+
+    def __init__(self, packed: PackedIEF, N, num_stage=3, delta_keys=None, impl='auto', keep=False, dropout=None):
         self.p, self.N, self.num_stage, self.keep = packed, N, num_stage, bool(keep)
+        self.dropout = ief_dropout(dropout, len(packed.deltas) + 1, num_stage)
+        if self.dropout is not None and not self.keep:
+            raise _lib.HDError('IEFPlan: dropout is a training mode and needs keep=True')
+        self.dropout_p = self.dropout[3] if self.dropout is not None else None
+        self._head_index = {id(packed.main): 0}
+        self._head_index.update({id(packed.deltas[k]): 1 + i for i, k in enumerate(sorted(packed.deltas))})
         dev = packed.device
         f32 = dict(dtype=torch.float32, device=dev)
         self.P = torch.empty((N, 1024), **f32)
@@ -1227,10 +1239,14 @@ class IEFPlan(object):
         else:
             h1, h2, outs = [None] * S, [self.h2] * S, [state_view] * S
         prev = start_view
+        sites = [(None, None)] * S
+        if self.dropout is not None:
+            hi = self._head_index[id(head)]
+            sites = [tuple(ief_dropout_site(self.dropout[2], hi, s, layer) for layer in (0, 1)) for s in range(S)]
         for s in range(S):
-            ops.append(('fc1t', prev, prev.stride(0), head, h1[s]))
+            ops.append(('fc1t', prev, prev.stride(0), head, h1[s], sites[s][0]))
             ops.append(('conv', head.fc2.bind(None, N, 1, 1, h2[s], inp_split=self.h1_split, impl=self.impl)))
-            ops.append(('fc3', prev, prev.stride(0), outs[s], outs[s].stride(0), head, h2[s]))
+            ops.append(('fc3', prev, prev.stride(0), outs[s], outs[s].stride(0), head, h2[s], sites[s][1]))
             prev = outs[s]
         return ops
 
@@ -1243,14 +1259,25 @@ class IEFPlan(object):
             elif kind == 'conv':
                 op[1].run(st)
             elif kind == 'fc1t':
-                _, prev, prev_ld, head, h1 = op
-                check(lib.hd_ief_fc1_theta(fptr(self.P), fptr(prev), prev_ld, fptr(head.fc1_theta.w_kn), head.d, 1024,
-                                           _vp(self.h1_split[0]), _vp(self.h1_split[1]), _vp(h1), N, st),
-                      'hd_ief_fc1_theta')
+                _, prev, prev_ld, head, h1, site = op
+                if site is None:
+                    check(lib.hd_ief_fc1_theta(fptr(self.P), fptr(prev), prev_ld, fptr(head.fc1_theta.w_kn), head.d, 1024,
+                                               _vp(self.h1_split[0]), _vp(self.h1_split[1]), _vp(h1), N, st),
+                          'hd_ief_fc1_theta')
+                else:
+                    seed, step, _, p = self.dropout
+                    check(lib.hd_ief_fc1_theta_dropout(fptr(self.P), fptr(prev), prev_ld, fptr(head.fc1_theta.w_kn), head.d, 1024,
+                                                       _vp(self.h1_split[0]), _vp(self.h1_split[1]), _vp(h1), N, seed, step, site, p, st),
+                          'hd_ief_fc1_theta_dropout')
             else:
-                _, prev, prev_ld, out, out_ld, head, h2 = op
-                check(lib.hd_ief_fc3(fptr(h2), fptr(head.fc3.w_kn), fptr(head.fc3.post_shift), fptr(prev), prev_ld, fptr(out), out_ld, N,
-                                     1024, head.d, st), 'hd_ief_fc3')
+                _, prev, prev_ld, out, out_ld, head, h2, site = op
+                if site is None:
+                    check(lib.hd_ief_fc3(fptr(h2), fptr(head.fc3.w_kn), fptr(head.fc3.post_shift), fptr(prev), prev_ld, fptr(out), out_ld,
+                                         N, 1024, head.d, st), 'hd_ief_fc3')
+                else:
+                    seed, step, _, p = self.dropout
+                    check(lib.hd_ief_fc3_dropout(fptr(h2), fptr(head.fc3.w_kn), fptr(head.fc3.post_shift), fptr(prev), prev_ld, fptr(out),
+                                                 out_ld, N, 1024, head.d, seed, step, site, p, st), 'hd_ief_fc3_dropout')
 
     def _head_ops(self, head, phi, start_view, state_view):
         """ops for one hmr_ief: start_view = theta_prev of stage 0, state_view = in-place theta afterwards."""
@@ -1296,6 +1323,37 @@ class IEFPlan(object):
     def num_launches(self):
         per = 1 + 3 * self.num_stage
         return per + len(self.delta_keys) * (per + 1) + (1 if self.fast else 0)
+
+
+def ief_dropout_site(call, head, stage, layer):
+    """The dropout site of one IEF call's layer: call 0 = the pred strips, 1 = the hal strips; head 0 = main, then the delta heads in
+    ascending dt; stage 0..3; layer 0 = dropout1 (after fc1), 1 = dropout2 (after fc2)."""
+    return ((call * 8 + head) * 4 + stage) * 2 + layer
+
+
+def nn_keep_prob(keep_prob):
+    """The float32 keep_prob TF 1.8's nn.dropout computes with for slim.dropout(keep_prob): core_layers.Dropout keeps rate = 1 -
+    keep_prob and calls nn.dropout(1 - rate), a Python float64 that becomes a float32 tensor."""
+    return float(np.float32(1.0 - (1.0 - float(keep_prob))))
+
+
+def ief_dropout(spec, num_heads, num_stage):
+    """IEFPlan's dropout argument -> (seed, step, call, nn.dropout's float32 keep_prob), or None for the identity (None, keep_prob 1)."""
+    if spec is None:
+        return None
+    seed, step, call, p = spec
+    p = float(p)
+    if not 0.0 < p <= 1.0:
+        raise _lib.HDError('IEF dropout: keep_prob must be in (0, 1], got %r' % (p,))
+    seed, step, call = int(seed), int(step), int(call)
+    if not (0 <= seed < 2 ** 64 and 0 <= step < 2 ** 64 and call >= 0):
+        raise _lib.HDError('IEF dropout: need 0 <= seed, step < 2^64 and call >= 0, got %r' % (spec,))
+    if num_heads > 8 or num_stage > 4 or ief_dropout_site(call + 1, 0, 0, 0) > 2 ** 31:
+        raise _lib.HDError('IEF dropout: at most 8 heads and 4 stages per call')
+    p32 = nn_keep_prob(p)
+    if p32 <= 0.0:
+        raise _lib.HDError('IEF dropout: keep_prob %r is 0 in float32' % (p,))
+    return None if p32 == 1.0 else (seed, step, call, p32)
 
 
 def ief_head_ops(head: PackedIEFHead, phi, start, state, P, h1, h2, num_stage, impl):

@@ -22,8 +22,14 @@ and batch-norm gamma / beta (trunk.TrainableResNet) join E's optimizer, e_loss's
 save_checkpoint writes their trained values.  Like the reference (whose gather_losses never adds slim's regularisation losses), the
 trunk trains without weight decay.
 
-Differences from the reference trainer: IEF dropout is the identity (trainable.TemporalModel runs the inference plans forward and
-follows the inference graph back); the default optimizer, torch's Adam, adds eps to sqrt(v_hat) where TF's adds it to sqrt(v) before the bias correction, and
+IEF dropout: the reference trains every IEF call with is_training=True, so slim.dropout(keep_prob=0.5) follows the ReLU of fc1 and
+fc2 at each stage of every head, in both IEF calls of a step.  `TrainConfig(ief_keep_prob=0.5)` does the same on the GPU: the masks
+are a documented function of (seed, global_step at the start of the step, call, head, stage, layer, row, column) (csrc/dropout.cuh,
+restated by oracle/dropout_ref.py), so a run is reproducible from `seed` and a resumed run continues the mask stream where it
+stopped.  The default, ief_keep_prob=1.0, keeps the inference graph (dropout the identity).
+
+Differences from the reference trainer: with dropout, TF's own random stream, whose op seeds come from graph construction, is not
+reproduced -- the placement and arithmetic of the masks are the reference's, the bits drawn are not; the default optimizer, torch's Adam, adds eps to sqrt(v_hat) where TF's adds it to sqrt(v) before the bias correction, and
 `optimizer=optim.TFAdam` removes that difference (TF's arithmetic, with its slots, beta powers and global_step in the checkpoint, so
 that `HMMRTrainer.resume(config, prefix, smpl_model)` continues a run where it stopped); the static `use_hmr_only` branch is not built, and freeze_phi=False needs image input (precomputed phis have no trunk to train).  A frame with no visible keypoint in an optimal-camera term
 contributes 0 (the reference's procrustes2d_vis divides 0 / 0 there and the loss is NaN).  The moving statistics start from whatever
@@ -71,9 +77,17 @@ class TrainConfig(HMMRConfig):
     # FP32-class) or 'tf32' (one TF32 MMA per product on round-to-nearest heads).  The forward passes, losses and optimizers are the
     # same in both (DESIGN.md section 2).
     grad_precision: str = 'fp32'
+    # keep_prob of the IEF heads' dropout (slim.dropout after the ReLU of fc1 and fc2, src/models.py:101-105): 1.0 = the identity,
+    # the reference trains with 0.5.  `seed` (src/config.py:132) keys its masks.
+    ief_keep_prob: float = 1.0
+    seed: int = 1
 
     def __post_init__(self):
         grad_one_pass(self.grad_precision, 'TrainConfig')
+        if not 0.0 < float(self.ief_keep_prob) <= 1.0:
+            raise _lib.HDError('TrainConfig: ief_keep_prob must be in (0, 1], got %r' % (self.ief_keep_prob,))
+        if int(self.seed) != self.seed or not 0 <= int(self.seed) < 2 ** 64:
+            raise _lib.HDError('TrainConfig: seed must be an integer in [0, 2^64), got %r' % (self.seed,))
 
 
 def loss_weights(config):
@@ -457,14 +471,14 @@ class HMMRTrainer(object):
         omegas = {}
         strips = model.temporal_encode(phis)
         keys = model.delta_keys if cfg.predict_delta else ()
-        om, dl = model.regress(strips.reshape(N, 2048), delta_keys=keys)
+        om, dl = model.regress(strips.reshape(N, 2048), delta_keys=keys, dropout=self._ief_dropout(0))
         omegas[('pred', 0)] = om
         omegas.update({('dt', k): v for k, v in dl.items()})
         inputs = {}
         if cfg.do_hallucinate:
             pstrips = model.hallucinate(phis)
             hk = keys if cfg.do_hallucinate_preds else ()
-            om, dl = model.regress(pstrips.reshape(N, 2048), delta_keys=hk)
+            om, dl = model.regress(pstrips.reshape(N, 2048), delta_keys=hk, dropout=self._ief_dropout(1))
             omegas[('hal', 0)] = om
             omegas.update({('hal', k): v for k, v in dl.items()})
             inputs['strips'], inputs['pred_strips'] = strips, pstrips
@@ -487,6 +501,11 @@ class HMMRTrainer(object):
         e_loss = sum(named[k] * w[k] for k in obj.names) + named['e_pose'] * w['e_pose']
         d_loss = named['d_pose'] * w['d_pose']
         return {k: named[k] for k in loss_keys(cfg)}, e_loss, d_loss
+
+    def _ief_dropout(self, call):
+        """The IEF dropout of call 0 (the pred strips) or 1 (the hal strips) at the current global_step; None with ief_keep_prob 1."""
+        p = float(self.config.ief_keep_prob)
+        return None if p == 1.0 else (int(self.config.seed), self.global_step, call, p)
 
     def step(self, batch, mocap_poses):
         """One iteration: both updates computed from the same pre-step parameters, then applied.  e_loss moves the temporal model,

@@ -6,7 +6,8 @@ after the ResNet.  The model packs its parameters in place with the inference en
 and each forward runs the inference plans over them (nets.FMoviePlan and IEFPlan with keep=True, which hold what the backward reads, and
 PackedHal.run), so its outputs are bit-identical to HMMREngine's; the weights are packed on the device (hd_pack_weight) and repacked
 before a forward whenever a parameter was changed in place (optimizer.step()).  The backward (csrc/net_grad.cu + hd_conv_gemm in its
-3xTF32 mode, or 1xTF32 with TrainConfig.grad_precision='tf32') is first-order, deterministic and follows the inference graph: dropout is the identity (is_training=False).
+3xTF32 mode, or 1xTF32 with TrainConfig.grad_precision='tf32') is first-order, deterministic and follows the inference graph: dropout is the identity (is_training=False)
+unless a call asks for the reference's training-mode IEF dropout explicitly (`regress(..., dropout=(seed, step, call, keep_prob))`).
 
 All arithmetic goes through libhd_b200.so; torch provides buffers, streams and the autograd plumbing.  The user's loss and optimizer
 are ordinary torch code:
@@ -143,10 +144,12 @@ def fmovie_backward(model, saved, g):
 # ------------------------------------------------------------------------------------------------------------------------------------
 # IEF heads
 # ------------------------------------------------------------------------------------------------------------------------------------
-def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st):
+def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st, p=None):
     """Backward of one hmr_ief head.  saved = (h1, h2, start, start_ld, stage-0 output, stage-1 output); g: gradient of the head's
     output (rows of d at stride g_ld).  Accumulates dL/dphi into `dphi`
-    (None: written).  Returns (dstart [N, d], [dW1, db1, dW2, db2, dW3, db3], dphi)."""
+    (None: written).  p: nn.dropout's float32 keep_prob when the forward ran the IEF dropout (h1 / h2 are then the masked
+    activations, so h > 0 <=> kept and positive, and a kept element's gradient is divided by p), None for the identity.
+    Returns (dstart [N, d], [dW1, db1, dW2, db2, dW3, db3], dphi)."""
     dev = phi.device
     d, feat = head.d, head.feat
     h1, h2, start, start_ld, mid0, mid1 = saved
@@ -160,9 +163,17 @@ def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st):
         if s == 2:
             G[2].copy_(torch.as_strided(g, (N, d), (g_ld, 1)))
         # dpre2 = (g . W3^T) * (h2 > 0);  dpre1 = (dpre2 . W2^T) * (h1 > 0);  dprev = g + dpre1 . W1theta^T
-        check(lib.hd_fc_small_dgrad(fptr(gs), gld, fptr(head.fc3.bwd.dst), 1024, d, fptr(h2[s]), fptr(DP2[s]), N, st), 'hd_fc_small_dgrad')
+        if p is None:
+            check(lib.hd_fc_small_dgrad(fptr(gs), gld, fptr(head.fc3.bwd.dst), 1024, d, fptr(h2[s]), fptr(DP2[s]), N, st),
+                  'hd_fc_small_dgrad')
+        else:
+            check(lib.hd_fc_small_dgrad_dropout(fptr(gs), gld, fptr(head.fc3.bwd.dst), 1024, d, fptr(h2[s]), p, fptr(DP2[s]), N, st),
+                  'hd_fc_small_dgrad_dropout')
         dgrad_op(head.fc2.bwd, DP2[s], N, 1, 1, 1, 1, DP1[s], one_pass=model.one_pass).run(st)
-        check(lib.hd_relu_backward(fptr(h1[s]), fptr(DP1[s]), fptr(DP1[s]), N * 1024, st), 'hd_relu_backward')
+        if p is None:
+            check(lib.hd_relu_backward(fptr(h1[s]), fptr(DP1[s]), fptr(DP1[s]), N * 1024, st), 'hd_relu_backward')
+        else:
+            check(lib.hd_relu_dropout_backward(fptr(h1[s]), fptr(DP1[s]), fptr(DP1[s]), N * 1024, p, st), 'hd_relu_dropout_backward')
         dst = G[s - 1] if s > 0 else dstart
         check(lib.hd_ief_fc3(fptr(DP1[s]), fptr(head.fc1_theta.bwd.dst), fptr(model._zeros), fptr(gs), gld, fptr(dst), d, N, 1024, d, st),
               'hd_ief_fc3')
@@ -186,12 +197,13 @@ def ief_head_backward(model, head, phi, N, saved, g, g_ld, dphi, st):
     return dstart, [W1, b1, W2, b2, W3, b3], out
 
 
-def regress_plan(model, keys, tiled, phi, start):
+def regress_plan(model, keys, tiled, phi, start, dropout=None):
     """call_hmr_ief over phi (N,2048) from start (N,85), or the tiled (1,85) when `tiled`, through a keep=True IEFPlan built for this
-    call: the main head, then the delta heads `keys` from its pose.  Returns ((theta, deltas...), the start rows (N,85), the plan)."""
+    call (with its `dropout`): the main head, then the delta heads `keys` from its pose.  Returns ((theta, deltas...), the start rows
+    (N,85), the plan)."""
     N = phi.shape[0]
     s0 = start.expand(N, 85).contiguous() if tiled else start
-    plan = IEFPlan(model.ief, N, 3, list(keys), keep=True)
+    plan = IEFPlan(model.ief, N, 3, list(keys), keep=True, dropout=dropout)
     theta, deltas = plan.run(phi, s0)
     return (theta,) + tuple(deltas[k] for k in keys), s0, plan
 
@@ -249,14 +261,14 @@ class FMovieFunction(torch.autograd.Function):
 class RegressFunction(torch.autograd.Function):
     """call_hmr_ief as Tester wires it: phi (N,2048), start (N,85) or the tiled mean_param (1,85) -> (theta (N,85), deltas (N,85)...).
     The delta heads start from theta's pose and carry its beta, so their gradients flow back into the main head; a tiled start's
-    gradient is its column sum."""
+    gradient is its column sum.  dropout: IEFPlan's; the backward reads the masked activations the plan saved and the keep_prob."""
 
     @staticmethod
-    def forward(ctx, model, keys, tiled, phi, start, *params):
-        outs, s0, plan = regress_plan(model, keys, tiled, phi, start)
+    def forward(ctx, model, keys, tiled, dropout, phi, start, *params):
+        outs, s0, plan = regress_plan(model, keys, tiled, phi, start, dropout)
         # Everything the backward reads goes through save_for_backward (theta, an output, included): no tensor or view of one is held on
         # ctx, so an unused graph is freed with its outputs and retain_graph works.  The delta heads' start is theta's pose, rebuilt there.
-        ctx.model, ctx.keys, ctx.tiled = model, keys, tiled
+        ctx.model, ctx.keys, ctx.tiled, ctx.p = model, keys, tiled, plan.dropout_p
         ctx.save_for_backward(phi, outs[0], s0, *[t for head in plan.saved for t in head])
         ctx.set_materialize_grads(False)
         return outs
@@ -284,11 +296,11 @@ class RegressFunction(torch.autograd.Function):
                 continue
             dd = dd.contiguous()
             ds, hg, dphi = ief_head_backward(model, model.ief.deltas[k], phi, N, state[1 + i],
-                                             torch.as_strided(dd, (N, 72), (85, 1), dd.storage_offset() + 3), 85, dphi, st)
+                                             torch.as_strided(dd, (N, 72), (85, 1), dd.storage_offset() + 3), 85, dphi, st, ctx.p)
             head_grads[k] = hg
             check(lib.hd_add_strided(fptr(gm[:, 3:]), 85, fptr(ds), 72, fptr(gm[:, 3:]), 85, N, 72, st), 'hd_add_strided')
             check(lib.hd_add_strided(fptr(gm[:, 75:]), 85, fptr(dd[:, 75:]), 85, fptr(gm[:, 75:]), 85, N, 10, st), 'hd_add_strided')
-        dstart, hg, dphi = ief_head_backward(model, model.ief.main, phi, N, state[0], gm, 85, dphi, st)
+        dstart, hg, dphi = ief_head_backward(model, model.ief.main, phi, N, state[0], gm, 85, dphi, st, ctx.p)
         head_grads['main'] = hg
         if ctx.tiled:
             ds = torch.empty((1, 85), dtype=F32, device=dev)
@@ -297,7 +309,7 @@ class RegressFunction(torch.autograd.Function):
         flat = []
         for k in ['main'] + list(keys):
             flat += head_grads.get(k, [None] * 6)
-        return (None, None, None, dphi, dstart) + tuple(flat)
+        return (None, None, None, None, dphi, dstart) + tuple(flat)
 
 
 class HalFunction(torch.autograd.Function):
@@ -504,9 +516,14 @@ class TemporalModel(TrainableModule):
             x = x.detach()
             return self.hal.run(x, torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)).view(phi.shape)
 
-    def regress(self, feats, omega_start=None, delta_keys=None):
+    def regress(self, feats, omega_start=None, delta_keys=None, dropout=None):
         """call_hmr_ief: feats (N,2048) -> (omega (N,85), {dt: (N,85)}).  Starts from mean_param (tiled) unless omega_start (N,85) is
-        given; the delta heads start from the main prediction (use_delta_from_pred=True, use_optcam=True, as Tester wires them)."""
+        given; the delta heads start from the main prediction (use_delta_from_pred=True, use_optcam=True, as Tester wires them).
+
+        dropout=(seed, step, call, keep_prob): the reference's training-mode IEF (is_training=True): slim.dropout(keep_prob) after the
+        ReLU of fc1 and fc2 at every stage of every head, forward and backward, with masks that are a function of (seed, step, call,
+        head, stage, layer, row, column) alone (nets.IEFPlan, csrc/dropout.cuh).  call 0 = the pred strips, 1 = the hal strips.
+        None (the default) or keep_prob 1: the inference graph.  Dropout is never implied by `training` or by grad mode."""
         self._check_input(feats, 'regress')
         keys = tuple(self.delta_keys) if delta_keys is None else tuple(sorted(int(k) for k in delta_keys if int(k) != 0))
         for k in keys:
@@ -521,10 +538,10 @@ class TemporalModel(TrainableModule):
             start = start.contiguous()
         names = [n for dt in (0,) + keys for n in ief_names(dt)]
         if self._grad_on(names + ['mean_param'], feats, start):
-            outs = RegressFunction.apply(self, keys, tiled, feats, start, *[self.param(n) for n in names])
+            outs = RegressFunction.apply(self, keys, tiled, dropout, feats, start, *[self.param(n) for n in names])
         else:
             with torch.no_grad():
-                outs = regress_plan(self, keys, tiled, feats.detach(), start.detach())[0]
+                outs = regress_plan(self, keys, tiled, feats.detach(), start.detach(), dropout)[0]
         return outs[0], {k: outs[1 + i] for i, k in enumerate(keys)}
 
     def predict_from_features(self, phi, smpl, single_frame=False):

@@ -313,6 +313,19 @@ int hd_ief_fc1_theta(const float *P, const float *theta, int theta_ld, const flo
 int hd_ief_fc3(const float *h2, const float *W, const float *bias, const float *prev, int prev_ld, float *out, int out_ld, int N, int K,
                int D, void *stream);
 
+/* ---- IEF dropout (training: slim.dropout after the ReLU of fc1 and fc2, src/models.py:101-105) ----
+ * The mask of element (n, j) of site `site` at step `step` is a function of (seed, step, site, n*C + j) alone (Philox4x32-10 and TF
+ * 1.8 nn.dropout's float32 arithmetic: csrc/dropout.cuh, restated by oracle/dropout_ref.py); p is nn.dropout's float32 keep_prob,
+ * 0 < p <= 1.  A kept element becomes x / p, a dropped one 0.  N*C <= 2^34.
+ * hd_ief_fc1_theta_dropout: hd_ief_fc1_theta with the mask applied to relu(P + theta . W) before either output is written.
+ * hd_ief_fc3_dropout: hd_ief_fc3 reading h2 through the mask (same summation order), the masked h2 written back over h2 (16-byte
+ * aligned).  hd_dropout_mask: out[n*C + j] = 1 where element (n, j) is kept, else 0. */
+int hd_ief_fc1_theta_dropout(const float *P, const float *theta, int theta_ld, const float *W, int K, int C, void *out_hi, void *out_lo,
+                             float *out_f32, int N, unsigned long long seed, unsigned long long step, int site, float p, void *stream);
+int hd_ief_fc3_dropout(float *h2, const float *W, const float *bias, const float *prev, int prev_ld, float *out, int out_ld, int N, int K,
+                       int D, unsigned long long seed, unsigned long long step, int site, float p, void *stream);
+int hd_dropout_mask(unsigned long long seed, unsigned long long step, int site, int N, int C, float p, unsigned char *out, void *stream);
+
 /* ---- IEF glue (src/models.py:349-371): dst[n*dst_ld + :85] = [1, 0, 0, theta[n,3:75], theta[n,75:85]] ---- */
 int hd_ief_delta_init(const float *theta, float *dst, int dst_ld, int N, void *stream);
 
@@ -508,9 +521,14 @@ int hd_groupnorm_relu_backward(const float *x, const float *gamma, const float *
 int hd_col_sum(const float *x, long long rows, int cols, long long ld, float *out, void *stream);
 /* dx[i] = y[i] > 0 ? dy[i] : 0 (y = the ReLU's output; dx may alias dy). */
 int hd_relu_backward(const float *y, const float *dy, float *dx, long long n, void *stream);
+/* The same through a dropout after the ReLU (y = the dropout's output, p its keep_prob, 0 < p <= 1): dx[i] = y[i] > 0 ? dy[i] / p : 0. */
+int hd_relu_dropout_backward(const float *y, const float *dy, float *dx, long long n, float p, void *stream);
 /* Short-K input gradient of an FC layer with D <= 96 outputs (the IEF fc3, D = 85 / 72):
  * out[n, k] = (mask[n, k] > 0) * sum_j g[n*g_ld + j] * Wt[j, k], Wt = W^T [D, K] fp32, out / mask dense [N, K] (mask nullable). */
 int hd_fc_small_dgrad(const float *g, int g_ld, const float *Wt, int K, int D, const float *mask, float *out, int N, void *stream);
+/* The same with mask = the output of a dropout after the ReLU (required), p its keep_prob: out[n, k] = mask[n, k] > 0 ? sum / p : 0. */
+int hd_fc_small_dgrad_dropout(const float *g, int g_ld, const float *Wt, int K, int D, const float *mask, float p, float *out, int N,
+                              void *stream);
 /* out[r, c] = a[r, c] + b[r, c] at independent row strides (out may alias a or b): gradient accumulation of the IEF glue. */
 int hd_add_strided(const float *a, long long lda, const float *b, long long ldb, float *out, long long ldo, int rows, int cols, void *stream);
 
